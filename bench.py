@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — throughput of the HR-VITON hot path on B200 (driver contract: see the task statement).
+"""bench.py — throughput of the HR-VITON hot path on one H100 (sm_90a).
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
     python bench.py --impl reference ...      # the reference algorithm on the host CPU cores (oracle port)
+    python bench.py ... --dump-outputs DIR    # also write what the last timed step returned as DIR/<name>.npy
 
 Prints ONE JSON line on rank 0.  Workloads (config.workload):
   train_stage2  (default) one full train_generator.py step per "step": frozen tocg -> warp -> SPADE G fwd+bwd -> D fwd+bwd
@@ -39,28 +40,17 @@ TRAIN_STAGE2_WORKLOAD = ("train_stage2: full train_generator.py step (tocg fwd, 
                          "Adam x2), 1024x768")
 
 
-def conv_traffic():
-    """Average DRAM bytes (read+write) per conv_igemm launch of one step, from the committed ncu pass
-    (profiles/r2_conv_dram_traffic.json, written by tools/summarise_ncu_traffic.py from the ncu launch list of one step of the default
-    command); None when that pass was not taken."""
-    p = os.path.join(ROOT, "profiles", "r2_conv_dram_traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f)["avg_dram_bytes_per_launch"]
-    except Exception:
-        return None
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d["bf16_tflops_sustained"], "src": "measured"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "src": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s — an upper bound, not a measured rate
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "src": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -175,11 +165,11 @@ def cpu_baseline_gen(steps=1, warmup=0, budget_s=240.0):
 
 
 def _reference_modules():
-    """(networks, network_generator) of the UNMODIFIED reference (baseline/_ref — an untracked verbatim copy made by
-    tools/install_reference.py / __graft_entry__.build() — or /root/reference), imported under private names so that they cannot
+    """(networks, network_generator) of the UNMODIFIED reference (oracle/_ref — an untracked copy that __graft_entry__.build()
+    makes with oracle/install_reference.py where a reference checkout exists), imported under private names so that they cannot
     be confused with this repo's drop-ins of the same file names.  None when no reference checkout travelled with the tree."""
     import importlib.util
-    for d in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+    for d in (os.path.join(ROOT, "oracle", "_ref"),):
         if os.path.exists(os.path.join(d, "networks.py")) and os.path.exists(os.path.join(d, "network_generator.py")):
             mods = []
             for name in ("networks", "network_generator"):
@@ -320,7 +310,7 @@ def host_threads():
 
 
 def cpu_baseline_train(steps=3, warmup=1, budget_s=200.0, size=(512, 384)):
-    """The reference's own modules (baseline/_ref) running one REAL train_generator.py step per timed step on the host cores: tocg
+    """The reference's own modules (oracle/_ref) running one REAL train_generator.py step per timed step on the host cores: tocg
     fwd (256x192, as in the reference) -> glue -> G fwd+bwd -> D -> hinge/feature-matching/VGG -> Adam(G) -> 2nd G fwd -> D fwd+bwd ->
     Adam(D), fp32, batch 1 at 512x384 — a quarter of the benchmarked pixel count and the smallest 4:3 size the reference generator
     admits (its latent grid is fine_width // 128 wide).  Reported as 1024x768-equivalent images/s (x 1/4: the three networks are fully
@@ -427,7 +417,7 @@ def run_torch_gpu(args):
     import torch
     ref = _reference_modules()
     if ref is None:
-        print(json.dumps({"impl": "torch_gpu", "unavailable": "no reference checkout (baseline/_ref) on this box"}))
+        print(json.dumps({"impl": "torch_gpu", "unavailable": "no reference copy (oracle/_ref) on this box"}))
         return
     import hrv_loader
     hrv_loader.load()
@@ -459,6 +449,35 @@ def run_torch_gpu(args):
                                  "per_gpu_batch": B, "peak_mem_GB": torch.cuda.max_memory_allocated() / 1e9}}))
 
 
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(d, result, trained=None):
+    """Writes each tensor of `result` (a tensor, or a dict / tuple of them) as d/<name>.npy in float32, plus, for a training step,
+    the updated parameters of `trained` as d/param.<name>.npy.  A tensor larger than its even share of the 64 MB budget is written as
+    a fixed sample: the elements at the sorted first indices of a seeded permutation of its flat index range, the same every run."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    items = []
+    if torch.is_tensor(result):
+        items.append(("out", result))
+    elif isinstance(result, dict):
+        items += [(str(k), v) for k, v in result.items() if torch.is_tensor(v)]
+    elif isinstance(result, (list, tuple)):
+        items += [("out%d" % i, v) for i, v in enumerate(result) if torch.is_tensor(v)]
+    if trained is not None:
+        items += [("param." + n, p) for n, p in trained.named_parameters()]
+    share = DUMP_BUDGET // max(1, len(items)) // 4  # float32 elements per tensor
+    for name, t in items:
+        flat = t.detach().reshape(-1)
+        if flat.numel() > share:
+            gen = torch.Generator(device="cpu").manual_seed(1234)
+            idx = torch.randperm(flat.numel(), generator=gen)[:max(1, share)].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(d, name + ".npy"), flat.float().cpu().numpy().reshape(t.shape if flat.numel() == t.numel() else (-1,)))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -472,6 +491,8 @@ def main():
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="weak: per-GPU batch fixed (default 8); strong: GLOBAL batch fixed at --batch (default 8), split over the ranks")
     ap.add_argument("--dump-profile", default="", help="write the per-launch CUDA-event profile of one step as CSV")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -656,12 +677,14 @@ def main():
                 out = g(xd, sd)
                 out_h.copy_(out, non_blocking=True)
 
+    last = [None]  # what the last timed step returned
+
     def timed(fn, k):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(k):
-            fn()
+            last[0] = fn()
         e1.record()
         barrier()
         ms = e0.elapsed_time(e1)
@@ -683,6 +706,9 @@ def main():
     launches = ops.LAUNCHES[0] - l0
     clocks = sampler.stop() if rank == 0 else None
     value = B * world * K / (ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        trained = (tocg if stage1 else g) if train else None  # a training step's result is also the model it updated
+        dump_outputs(args.dump_outputs, last[0], trained)
 
     for _ in range(2):
         step_e2e()
@@ -720,10 +746,9 @@ def main():
     conv_ms = agg.get("conv", [0, 0, 0])[1] + agg.get("conv_spade", [0, 0, 0])[1]
     conv_launches = agg.get("conv", [0, 0, 0])[2] + agg.get("conv_spade", [0, 0, 0])[2]
     achieved = conv_flops / (conv_ms * 1e-3) / 1e12 if conv_ms > 0 else 0.0
-    roofline = {"kernel": "conv_pair_kernel + conv_pixn_kernel + conv_igemm_kernel (tcgen05 implicit-GEMM convolution, all %d launches of one step)" % conv_launches,
+    roofline = {"kernel": "conv_wgmma_kernel (wgmma implicit-GEMM convolution, all %d launches of one step)" % conv_launches,
                 "bound": "tensor", "achieved": achieved, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
                 "frac": achieved / peaks["tf_sustained"],
-                "traffic": conv_traffic() if (train and not stage1 and B == 8) else None,  # the ncu pass was taken on the default workload only
                 "peak_source": peaks["src"] + " (bf16 sustained)",
                 "avg_launch_ms": conv_ms / max(1, conv_launches), "algorithmic_gflop_per_launch": conv_flops / 1e9 / max(1, conv_launches)}
     # The convolution launches are not all tensor-bound: the thin-channel full-resolution layers (3->64, 9->16, 32->3, the 1x1 64->128
@@ -769,7 +794,7 @@ def main():
                                        if (train and not stage1) else "this repo's kernels (see DESIGN.md)"),
                            "launch": (("cuda-graph replay of the whole step" + (" (NCCL bucket all-reduces captured in the graph)" if world > 1 else "")) if (train and use_graph) else "eager"),
                            "feeding": "e2e: pinned host batch -> device on a copy stream, double-buffered (overlaps the previous step); one-hot parse maps shipped as uint8 labels and expanded by hrv_onehot_u8" if train else "e2e: pinned host -> device on the compute stream", "per_gpu_batch": B, "global_batch": B * world, "parallelism": "dp%d" % world,
-                           "l2": "activations per step (>10 GB) exceed the 126 MB L2; no explicit flush",
+                           "l2": "activations per step (>10 GB) exceed the 50 MB L2; no explicit flush",
                            "weights": "xavier(0.02) random init, noise_scale~N(0,0.1)"},
                 "e2e": {"value": e2e_value, "unit": "images/s", "ms_per_step": ms_e2e / K,
                         "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes},

@@ -4,7 +4,7 @@ torch.autograd carries the graph; every node is a fused C-ABI op on pixel-major 
 
   ConvFn    y = act(conv(x, W) * 1 + b (+ res))          fwd: hrv_conv2d_fwd
             dX  = conv(dY', flip(W)^T)                     bwd: hrv_conv2d_fwd again (dgrad IS a convolution)
-            dW  = x^T (*) dY'                              bwd: hrv_conv2d_wgrad (tcgen05, pixel-K GEMM with MN-major operands)
+            dW  = x^T (*) dY'                              bwd: hrv_conv2d_wgrad (wgmma, pixel-K GEMM with MN-major operands)
   SpadeFn   h = act(IN(cat(up(x0),x1) + noise*ns) * (1+gamma(actv)) + beta(actv))
             fwd: hrv_instnorm_stats + hrv_conv2d_fwd(SPADE epilogue); bwd: modulation / InstanceNorm backward +
             dgrad/wgrad of the gamma|beta GEMM.
@@ -37,7 +37,7 @@ def _act_grad(dy, y, act):
 
 
 def _wgrad(x_buf, cin, dy_buf, cout, kh, kw, pad):
-    """dW (cout,cin,kh,kw) fp32 = sum over pixels of dY[p,co] * X[p+tap-pad,ci] on tcgen05 (hrv_conv2d_wgrad).
+    """dW (cout,cin,kh,kw) fp32 = sum over pixels of dY[p,co] * X[p+tap-pad,ci] on wgmma (hrv_conv2d_wgrad).
     HRV_WGRAD=cudnn selects the library weight-gradient instead (A/B comparisons only)."""
     if os.environ.get("HRV_WGRAD") == "cudnn":
         x = x_buf[..., :cin].permute(0, 3, 1, 2)

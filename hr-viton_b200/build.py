@@ -1,4 +1,4 @@
-"""Builds libhrviton_sm100.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libhrviton_sm100.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
 Every kernel translation unit is compiled twice: once as is (bf16 activation storage, entry points hrv_<op>) and once with
 -DHRV_F16 -Dhrv=hrv_f16 (IEEE fp16 storage, entry points hrv_<op>_f16; csrc/hrv_f16_rename.h).  capi.cu (error text, device
@@ -14,7 +14,7 @@ LIB = os.path.join(PKG, "libhrviton_sm100.so")
 SHARED = ["capi.cu"]
 KERNEL_TUS = ["conv_igemm.cu", "aux_kernels.cu", "norm_bwd.cu", "conv_wgrad.cu", "glue_kernels.cu", "conv_f32.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 F16_FLAGS = ["-DHRV_F16", "-Dhrv=hrv_f16"]
 
@@ -58,7 +58,7 @@ def build(force=False, verbose=False):
         if r.returncode:
             raise RuntimeError("nvcc failed on %s %s" % (src, " ".join(extra)))
     objs = [os.path.join(CSRC, j[1]) for j in jobs]
-    r = subprocess.run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"], capture_output=True, text=True)
+    r = subprocess.run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"], capture_output=True, text=True)
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("link failed")

@@ -1,27 +1,20 @@
-// conv_igemm.cu — NHWC convolution as an im2col-free implicit GEMM on sm_100a.
+// conv_igemm.cu — NHWC convolution as an im2col-free implicit GEMM on sm_90a (wgmma + TMA + mbarrier).
 //
-//   GEMM view:  M = output pixels (128 per tile = TN x TH x TW box), N = output channels (BN <= 256 per tile),
-//               K = taps x input channels, walked tap by tap in chunks of BK channels.
-//   A operand:  one TMA 4-D box {BK ch, TW, TH, TN} of the NHWC input per (tap, channel chunk), shifted by the tap
-//               offset; TMA zero-fills out-of-range pixels (= the convolution's zero padding) and channels.
-//   B operand:  one TMA 2-D box {BK, BN} of the packed weights [n_pad][taps*cin_k] (K-major).
-//   MMA:        tcgen05.mma.cta_group::1.kind::f16, M=128 x N=BN x K=16, bf16 inputs, fp32 accumulators in TMEM.
-//   Halo mode:  (default for images >= 12 rows) the tile is 16 rows x 8 pixels of one image; ONE TMA box of
-//               (16+KH-1) x (8+KW-1) pixels per channel chunk lands in shared memory and every tap is a *shifted view* of
-//               it: the UMMA descriptor starts at row (ky*(8+KW-1)+kx) with SBO = (8+KW-1) rows.  tcgen05 applies the
-//               128B/64B/32B swizzle on absolute shared-memory address bits (probed on B200: tools/umma_halo_probe.cu),
-//               exactly as TMA wrote it, so unaligned starts are legal.  KH*KW-fold less L2->smem traffic and TMA issue
-//               than tap-by-tap loading.  Weights ride a second ring with `tpb` taps per TMA (3-D box).
-//   Pipeline:   persistent CTAs (one per SM); warp 0 = A (halo / tap) TMA producer, warp 3 = weight TMA producer of the halo
-//               mainloops, warp 1 = MMA issuer (issue_tap_group: one elected region per weight stage), warp 2 = TMEM allocator,
-//               warps 4.. = epilogue warpgroups (column split, or one whole tile per warpgroup: epi_own / pair kernel).  Rings of
-//               A and B stages with full/empty mbarriers; TMEM holds min(8, 512/BN) accumulators so epilogues overlap the MMAs.
-//   Kernels:    conv_igemm_kernel<BK> (one CTA, M = 128 pixels), conv_pair_kernel (2-CTA cluster, cta_group::2, M = 256 pixels,
-//               half of every weight stage per CTA), conv_pixn_kernel (weights as M, 256 pixels as N); hrv_conv2d_fwd picks one
-//               per layer from a measured table (profiles/r2_kernel_selection_ab.txt).
+//   GEMM view:  M = output pixels (128 per tile = TN x TH x TW box), N = output channels (BNT = 64 or 128 per tile),
+//               K = taps x input channels, walked tap by tap in chunks of 64 channels.
+//   A operand:  one TMA 4-D box {64 ch, TW, TH, TN} of the NHWC input per (tap, channel chunk), shifted by the tap offset;
+//               TMA zero-fills out-of-range pixels (= the convolution's zero padding) and channels past the input's or the packed
+//               weight's channel count, so every layer runs on 64-channel K blocks whatever block size its weights were packed with.
+//   B operand:  one TMA box {64, BNT} of the packed weights [taps][n_pad][cin_k] (K-major); rows past n_pad are zero fill.
+//   MMA:        wgmma.mma_async m64nBNTk16, bf16 (fp16 flavour: f16) operands from 128B-swizzled shared memory, fp32 accumulators in
+//               the registers of the consumer warpgroups.
+//   Pipeline:   one CTA per (pixel tile, N tile), two CTAs per SM (the epilogue of one overlaps the mainloop of the other).
+//               Warp 8 = TMA producer, warpgroups 0 / 1 = consumers for pixels 0-63 / 64-127 of the tile.  A ring of `stages`
+//               (A + B) stages with full (transaction count) / empty (one arrival per consumer warp) mbarriers.
 //   Epilogues:  LINEAR  out = act(acc*scale + shift (+ residual))      (bias / folded BatchNorm / residual / tanh)
-//               SPADE   out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta), gamma/beta = interleaved GEMM columns:
-//                       the SPADE modulation never leaves registers (network_generator.py:115-121,170-171).
+//               SPADE   out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta), gamma/beta = interleaved GEMM columns: a thread's
+//                       accumulator pair (2j, 2j+1) is (gamma, beta) of one channel, so the SPADE modulation never leaves registers
+//                       (network_generator.py:115-121,170-171).
 //
 // Replaces nn.Conv2d at networks.py:60-93,178-192 and network_generator.py:97-99,132-135,184-201,263-272.
 #include <stdlib.h>
@@ -31,13 +24,12 @@
 
 namespace hrv {
 
-constexpr int kMaxStages = 32;
-constexpr int kEpiWG = 4;                       // pixel-N kernel: epilogue warpgroups (each owns 64 of the tile's 256 pixel columns)
-constexpr int kThreads = 128 + 128 * kEpiWG;  // warps 0-3: TMA / MMA / TMEM-alloc / spare; then the epilogue warpgroups
-// Classic kernel: 3 epilogue warpgroups (each handles every 3rd 16-column chunk) = 512 threads, i.e. 128 registers per thread: room to
-// keep the x operand of every chunk of a tile in flight while the MMAs of that tile still run (see the SPADE epilogue).
-constexpr int kEpiC = 3;
-constexpr int kThreadsC = 128 + 128 * kEpiC;
+constexpr int kMaxStages = 16;
+constexpr int kConsumers = 2;                       // consumer warpgroups (64 pixels each)
+constexpr int kThreads = 128 * kConsumers + 32;     // + one producer warp
+constexpr uint32_t kRowBytes = 128;                 // 64 channels of 2 bytes: one SWIZZLE_128B row
+constexpr uint32_t kABytes = 128 * kRowBytes;       // 128 pixels
+constexpr uint32_t kSmemPerCta = 110u * 1024u;      // two CTAs per SM (plus 1 KB reserved per CTA)
 
 struct alignas(64) ConvArgs {
   CUtensorMap tmA;
@@ -46,8 +38,7 @@ struct alignas(64) ConvArgs {
   int tw_log, th_log;
   int tiles_x, tiles_y, tiles_img, tiles_n;
   int KH, KW, off_y, off_x, chunks;
-  int BN, stages, n_gemm, nacc;  // nacc = TMEM accumulator stages = min(8, 512/BN)
-  int halo, tpb, sb_stages, a_stage_bytes, a_stage_bytes_tx, b_stage_bytes, line_pitch;  // halo mode: `stages` A-halo stages + sb_stages weight stages
+  int stages, n_gemm;
   int epi, act;
   const float* scale;
   const float* shift;
@@ -66,1151 +57,199 @@ struct alignas(64) ConvArgs {
   int C_mod;
   __nv_bfloat16* gamma_out;
   int gamma_pitch;
-  int pairs, tiles_m, store_c;  // pixel-N variant: 256-pixel tiles (pairs of 128-pixel boxes), channels written per pixel
-  int epi_tab;                  // CTA-pair kernel, SPADE: per-warpgroup constant tables in shared memory
-  int tap_group;                // halo mainloops, 3x3: MMAs of a whole weight stage (9 taps, or one kernel row of 3) issued from one elected region
-  int epi_own;                  // one-CTA kernel, LINEAR: accumulator i is drained by epilogue warpgroup i % kEpiC alone (whole tile)
-  unsigned long long* stats;    // debug (tools/conv_stall_probe.py): per-CTA cycle counters of the warp roles, or nullptr
 };
 
-__device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-
-// wait on an mbarrier, optionally accounting the stall cycles (stats != nullptr only under the stall probe)
-__device__ __forceinline__ void mbar_wait_acct(uint32_t bar, uint32_t parity, bool acct, unsigned long long& acc) {
-  if (!acct) { mbar_wait(bar, parity); return; }
-  const long long t0 = clock64();  // try_wait itself may block for a hardware-defined time: time the whole wait
-  mbar_wait(bar, parity);
-  acc += (unsigned long long)(clock64() - t0);
-}
-
-// Activation as a compile-time choice: with a run-time `act` every element of an epilogue chunk carried its own uniform-branch ladder,
-// which serialised the eight elements of a thread (no ILP: ~500 dependent cycles per chunk in the SASS of the round-2 pair kernel).
-template <int ACT>
-__device__ __forceinline__ float act_t(float v) {
-  if (ACT == 1) return fmaxf(v, 0.f);
-  if (ACT == 2) return v > 0.f ? v : 0.2f * v;
-  if (ACT == 3) return tanhf(v);
-  return v;
-}
-// Activation of a chunk's eight values with ONE branch ladder per chunk (not one per element): the arithmetic above it stays
-// straight-line code, so the eight elements overlap instead of running one after the other.
-__device__ __forceinline__ void apply_act8(float (&f)[8], int act) {
-  if (act == 2) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[i] = f[i] > 0.f ? f[i] : 0.2f * f[i];
-  } else if (act == 1) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[i] = fmaxf(f[i], 0.f);
-  } else if (act == 3) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) f[i] = tanhf(f[i]);
-  }
-}
-
-// One tile of the output as seen by an epilogue thread: TMEM lane r = pixel (x, y) of image n.
-struct EpiTile {
+// One output pixel as seen by an epilogue thread.
+struct EpiPix {
   int x, y, n;
   bool valid;
   long long pix;
-  int n_base;       // first GEMM column of the tile's N tile
-  uint32_t taddr;   // TMEM address of this warp's lane quarter of the accumulator
 };
-constexpr int kMaxChunks = (256 / 16 + kEpiC - 1) / kEpiC;  // BN <= 256: at most 6 chunks of 16 columns per warpgroup
 
-// LINEAR epilogue of one tile (accumulator complete): out = act(acc*scale + shift (+ res | * act'(res))) for this warpgroup's chunks.
-__device__ __forceinline__ void epi_linear(const ConvArgs& a, const EpiTile& t, int wg, int nwg = kEpiC) {
-  const bool valid = t.valid;
-  const long long pix = t.pix;
-  const int n_base = t.n_base, n = t.n, y = t.y, x = t.x;
-  const uint32_t taddr = t.taddr;
-  const int store_c = (a.out_dtype == 0 && a.out_layout == 0) ? ((a.out_c + 7) & ~7) : a.out_c;
-  for (int col = wg * 16; col < a.BN; col += 16 * nwg) {
-    uint32_t v[16];
-    __syncwarp();
-    tmem_ld16(taddr + col, v);
-    tmem_wait_ld();
-    const int j0 = n_base + col;
-    if (!valid || j0 >= store_c) continue;
+// LINEAR epilogue of two adjacent GEMM columns (c, c+1) of one pixel: out = act(acc*scale + shift (+ res | * act'(res))).
+// bf16 NHWC outputs also write the pad channels up to the next multiple of 8 (as act(0) + res), fp32 outputs stop at out_c.
+__device__ __forceinline__ void epi_linear2(const ConvArgs& a, const EpiPix& p, int c, float v0, float v1) {
+  const bool bf16_nhwc = a.out_dtype == 0 && a.out_layout == 0;
+  const int store_c = bf16_nhwc ? ((a.out_c + 7) & ~7) : a.out_c;
+  if (!p.valid || c >= store_c) return;
+  float f[2] = {v0, v1};
 #pragma unroll
-    for (int g = 0; g < 2; ++g) {
-      const int jg = j0 + g * 8;
-      if (jg >= store_c) break;
-      float f[8];
-      if (jg + 8 <= a.n_gemm) {  // vector path (scale/shift arrays are 16-byte aligned torch allocations)
-        float sc[8] = {1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f, 1.f}, sh[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        if (a.scale) {
-          *reinterpret_cast<float4*>(sc) = __ldg(reinterpret_cast<const float4*>(a.scale + jg));
-          *reinterpret_cast<float4*>(sc + 4) = __ldg(reinterpret_cast<const float4*>(a.scale + jg) + 1);
-        }
-        if (a.shift) {
-          *reinterpret_cast<float4*>(sh) = __ldg(reinterpret_cast<const float4*>(a.shift + jg));
-          *reinterpret_cast<float4*>(sh + 4) = __ldg(reinterpret_cast<const float4*>(a.shift + jg) + 1);
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) f[i] = fmaf(__uint_as_float(v[g * 8 + i]), sc[i], sh[i]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int j = jg + i;
-          const bool in = j < a.n_gemm;
-          const float sc = in ? (a.scale ? __ldg(a.scale + j) : 1.f) : 0.f;
-          const float sh = (in && a.shift) ? __ldg(a.shift + j) : 0.f;
-          f[i] = fmaf(__uint_as_float(v[g * 8 + i]), sc, sh);
-        }
-      }
-      if (a.res) {
-        if (a.res_dtype == 0) {
-          const uint4 rv = __ldg(reinterpret_cast<const uint4*>(
-              reinterpret_cast<const __nv_bfloat16*>(a.res) + pix * a.res_pitch + jg));
-          const float rf[8] = {bf16_lo(rv.x), bf16_hi(rv.x), bf16_lo(rv.y), bf16_hi(rv.y), bf16_lo(rv.z), bf16_hi(rv.z), bf16_lo(rv.w), bf16_hi(rv.w)};
-          if (a.res_mode == 0) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[i] += rf[i];
-          } else {  // activation backward of the layer below, fused: multiply by act'(its saved output)
-            const float slope = a.res_mode == 1 ? 0.f : 0.2f;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[i] = rf[i] > 0.f ? f[i] : f[i] * slope;
-          }
-        } else {
-          const float* rp = reinterpret_cast<const float*>(a.res) + pix * a.res_pitch + jg;
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            if (jg + i < a.out_c) f[i] += __ldg(rp + i);
-        }
-      }
-      apply_act8(f, a.act);
-      if (a.out_dtype == 0) {
-        uint4 o;
-        o.x = pack_bf16(f[0], f[1]); o.y = pack_bf16(f[2], f[3]);
-        o.z = pack_bf16(f[4], f[5]); o.w = pack_bf16(f[6], f[7]);
-        *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + pix * a.out_pitch + jg) = o;
-      } else if (a.out_layout == 0) {
-        float* op = reinterpret_cast<float*>(a.out) + pix * a.out_pitch + jg;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (jg + i < a.out_c) op[i] = f[i];
-      } else {  // fp32 NCHW
-        float* op = reinterpret_cast<float*>(a.out);
-        const long long hw = (long long)a.Hout * a.Wout;
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          if (jg + i < a.out_c) op[((long long)n * a.out_c + jg + i) * hw + (long long)y * a.Wout + x] = f[i];
-      }
-    }
+  for (int i = 0; i < 2; ++i) {
+    const int j = c + i;
+    const bool in = j < a.n_gemm;
+    const float sc = in ? (a.scale ? __ldg(a.scale + j) : 1.f) : 0.f;
+    const float sh = (in && a.shift) ? __ldg(a.shift + j) : 0.f;
+    f[i] = fmaf(f[i], sc, sh);
   }
-}
-
-// SPADE epilogue, part 1 (BEFORE waiting for the accumulator): issue the x loads of every chunk this warp owns and the noise load.
-// They do not depend on the MMAs, so their DRAM/L2 latency overlaps the mainloop instead of sitting on the epilogue's critical
-// path (the ncu source view of round 1 showed the epilogue warps stalled on the first use of x; profiles/r2_conv_stall_*.txt).
-__device__ __forceinline__ void epi_spade_prefetch(const ConvArgs& a, const EpiTile& t, int wg, uint4 (&xv)[kMaxChunks], float& nz_out) {
-  const bool valid = t.valid;
-  const long long pix = t.pix;
-  const int n_base = t.n_base, n = t.n, y = t.y, x = t.x;
-  const int sh0 = a.x0_shift;
-  const long long pix0 = ((long long)n * (a.Hout >> sh0) + (y >> sh0)) * (a.Wout >> sh0) + (x >> sh0);
+  if (a.res) {
+    if (a.res_dtype == 0) {
+      const uint32_t rv = __ldg(reinterpret_cast<const unsigned int*>(reinterpret_cast<const __nv_bfloat16*>(a.res) + p.pix * a.res_pitch + c));
+      const float rf[2] = {bf16_lo(rv), bf16_hi(rv)};
+      if (a.res_mode == 0) {
+        f[0] += rf[0]; f[1] += rf[1];
+      } else {  // activation backward of the layer below, fused: multiply by act'(its saved output)
+        const float slope = a.res_mode == 1 ? 0.f : 0.2f;
 #pragma unroll
-  for (int k = 0; k < kMaxChunks; ++k) {
-    const int col = wg * 16 + k * 16 * kEpiC;
-    const int c0 = (n_base + col) >> 1;
-    xv[k] = make_uint4(0, 0, 0, 0);
-    if (col < a.BN && valid && c0 < a.C_mod) {
-      const __nv_bfloat16* xp = (c0 < a.x0_c) ? (a.x0 + pix0 * a.x0_pitch + c0)
-                                               : (a.x1 + pix * a.x1_pitch + (c0 - a.x0_c));
-      xv[k] = __ldg(reinterpret_cast<const uint4*>(xp));
-    }
-  }
-  nz_out = (valid && a.noise) ? __ldg(a.noise + pix) : 0.f;
-}
-
-// SPADE epilogue, part 2 (accumulator complete): 16 GEMM columns = 8 channels of (gamma, beta);
-// out = act(((x + noise*ns) - mean) * rstd * (1 + gamma) + beta), gamma optionally stored for the backward pass.
-__device__ __forceinline__ void epi_spade_finish(const ConvArgs& a, const EpiTile& t, int wg, const uint4 (&xv)[kMaxChunks], float nz) {
-  const bool valid = t.valid;
-  const long long pix = t.pix;
-  const int n_base = t.n_base, n = t.n;
-  const uint32_t taddr = t.taddr;
-#pragma unroll
-  for (int k = 0; k < kMaxChunks; ++k) {
-    const int col = wg * 16 + k * 16 * kEpiC;
-    if (col >= a.BN) break;
-    const int c0 = (n_base + col) >> 1;
-    const bool live = valid && c0 < a.C_mod;
-    // per-channel constants: warp-uniform addresses, L1-resident after the first tile of an image
-    float mu[8], rs[8], nsv[8], sh[16];
-    if (live) {
-      const float4* mp = reinterpret_cast<const float4*>(a.mean + (long long)n * a.C_mod + c0);
-      const float4* rp = reinterpret_cast<const float4*>(a.rstd + (long long)n * a.C_mod + c0);
-      *reinterpret_cast<float4*>(mu) = __ldg(mp);
-      *reinterpret_cast<float4*>(mu + 4) = __ldg(mp + 1);
-      *reinterpret_cast<float4*>(rs) = __ldg(rp);
-      *reinterpret_cast<float4*>(rs + 4) = __ldg(rp + 1);
-      if (a.noise_scale) {
-        const float4* np_ = reinterpret_cast<const float4*>(a.noise_scale + c0);
-        *reinterpret_cast<float4*>(nsv) = __ldg(np_);
-        *reinterpret_cast<float4*>(nsv + 4) = __ldg(np_ + 1);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) nsv[i] = 0.f;
+        for (int i = 0; i < 2; ++i) f[i] = rf[i] > 0.f ? f[i] : f[i] * slope;
       }
-      if (a.shift) {
-        const float4* sp = reinterpret_cast<const float4*>(a.shift + 2 * c0);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(sh + 4 * i) = __ldg(sp + i);
-      } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) sh[i] = 0.f;
-      }
-    }
-    uint32_t v[16];
-    __syncwarp();
-    tmem_ld16(taddr + col, v);
-    tmem_wait_ld();
-    if (!live) continue;
-    const uint4 xk = xv[k];
-    const float xs[8] = {bf16_lo(xk.x), bf16_hi(xk.x), bf16_lo(xk.y), bf16_hi(xk.y),
-                         bf16_lo(xk.z), bf16_hi(xk.z), bf16_lo(xk.w), bf16_hi(xk.w)};
-    float o[8], gmv[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float xval = fmaf(nz, nsv[i], xs[i]);
-      const float gm = __uint_as_float(v[2 * i]) + sh[2 * i];
-      const float bt = __uint_as_float(v[2 * i + 1]) + sh[2 * i + 1];
-      const float xn = (xval - mu[i]) * rs[i];
-      gmv[i] = gm;
-      o[i] = fmaf(xn, 1.f + gm, bt);
-    }
-    apply_act8(o, a.act);
-    if (a.gamma_out) {  // training: keep gamma for the backward pass (saves re-running this GEMM)
-      uint4 gv;
-      gv.x = pack_bf16(gmv[0], gmv[1]); gv.y = pack_bf16(gmv[2], gmv[3]);
-      gv.z = pack_bf16(gmv[4], gmv[5]); gv.w = pack_bf16(gmv[6], gmv[7]);
-      *reinterpret_cast<uint4*>(a.gamma_out + pix * a.gamma_pitch + c0) = gv;
-    }
-    uint4 ov;
-    ov.x = pack_bf16(o[0], o[1]); ov.y = pack_bf16(o[2], o[3]);
-    ov.z = pack_bf16(o[4], o[5]); ov.w = pack_bf16(o[6], o[7]);
-    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + pix * a.out_pitch + c0) = ov;
-  }
-}
-
-// SPADE epilogue of a WHOLE tile by ONE warpgroup (CTA-pair kernel: the tile in TMEM accumulator w is drained by warpgroup w).
-// The per-chunk work is a chain of dependent latencies (tcgen05.ld -> constants -> arithmetic -> store) that leaves the issue slots
-// three quarters idle, and a warp walks its chunks one after the other: with all warpgroups on the SAME tile the tile period equals
-// that latency (about 10,000 cycles, tools/conv_stall_probe.py) however the stores are done.  With each warpgroup on its OWN tile three
-// tiles drain concurrently — one per TMEM accumulator (warpgroup w owns accumulator w; two of them when the tile is too wide for three
-// accumulators) — and the period drops accordingly.
-// x runs four chunks ahead of its use (the first four loads go out before the wait for the accumulator).
-// Per-warpgroup table of the current image's SPADE constants in shared memory, rows {mean, rstd, noise_scale, gamma bias, beta bias} of
-// C_mod floats: ten global loads per chunk (an L2 round trip on the critical path of every chunk) become broadcast shared-memory reads.
-constexpr int kTabMaxC = 288;
-constexpr uint32_t kTabBytes = ((5u * kTabMaxC * 4u) + 127u) & ~127u;
-__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void lds8(uint32_t addr, float (&f)[8]) {
-  const uint4 p = ld_shared_v4(addr), q = ld_shared_v4(addr + 16u);
-  f[0] = __uint_as_float(p.x); f[1] = __uint_as_float(p.y); f[2] = __uint_as_float(p.z); f[3] = __uint_as_float(p.w);
-  f[4] = __uint_as_float(q.x); f[5] = __uint_as_float(q.y); f[6] = __uint_as_float(q.z); f[7] = __uint_as_float(q.w);
-}
-__device__ __forceinline__ uint4 epi_spade_x(const ConvArgs& a, const EpiTile& t, int col, long long pix0) {
-  const int c0 = (t.n_base + col) >> 1;
-  if (col < a.BN && t.valid && c0 < a.C_mod) {
-    const __nv_bfloat16* xp = (c0 < a.x0_c) ? (a.x0 + pix0 * a.x0_pitch + c0) : (a.x1 + t.pix * a.x1_pitch + (c0 - a.x0_c));
-    return __ldg(reinterpret_cast<const uint4*>(xp));
-  }
-  return make_uint4(0, 0, 0, 0);
-}
-__device__ __forceinline__ void epi_spade_chunk(const ConvArgs& a, const EpiTile& t, int col, const uint4& xk, float nz, uint32_t tab) {
-  const int c0 = (t.n_base + col) >> 1;
-  const bool live = t.valid && c0 < a.C_mod;
-  float mu[8], rs[8], nsv[8], sh[16];
-  if (live && tab) {
-    float bg[8], bb[8];
-    const uint32_t cp = (uint32_t)a.C_mod * 4u, tb = tab + (uint32_t)c0 * 4u;
-    lds8(tb, mu); lds8(tb + cp, rs); lds8(tb + 2u * cp, nsv); lds8(tb + 3u * cp, bg); lds8(tb + 4u * cp, bb);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { sh[2 * i] = bg[i]; sh[2 * i + 1] = bb[i]; }
-  } else if (live) {
-    const float4* mp = reinterpret_cast<const float4*>(a.mean + (long long)t.n * a.C_mod + c0);
-    const float4* rp = reinterpret_cast<const float4*>(a.rstd + (long long)t.n * a.C_mod + c0);
-    *reinterpret_cast<float4*>(mu) = __ldg(mp);
-    *reinterpret_cast<float4*>(mu + 4) = __ldg(mp + 1);
-    *reinterpret_cast<float4*>(rs) = __ldg(rp);
-    *reinterpret_cast<float4*>(rs + 4) = __ldg(rp + 1);
-    if (a.noise_scale) {
-      const float4* np_ = reinterpret_cast<const float4*>(a.noise_scale + c0);
-      *reinterpret_cast<float4*>(nsv) = __ldg(np_);
-      *reinterpret_cast<float4*>(nsv + 4) = __ldg(np_ + 1);
     } else {
+      const float* rp = reinterpret_cast<const float*>(a.res) + p.pix * a.res_pitch + c;
 #pragma unroll
-      for (int i = 0; i < 8; ++i) nsv[i] = 0.f;
-    }
-    if (a.shift) {
-      const float4* sp = reinterpret_cast<const float4*>(a.shift + 2 * c0);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) *reinterpret_cast<float4*>(sh + 4 * i) = __ldg(sp + i);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 16; ++i) sh[i] = 0.f;
+      for (int i = 0; i < 2; ++i)
+        if (c + i < a.out_c) f[i] += __ldg(rp + i);
     }
   }
-  uint32_t v[16];
-  __syncwarp();
-  tmem_ld16(t.taddr + col, v);
-  tmem_wait_ld();
-  if (!live) return;
-  const float xs[8] = {bf16_lo(xk.x), bf16_hi(xk.x), bf16_lo(xk.y), bf16_hi(xk.y), bf16_lo(xk.z), bf16_hi(xk.z), bf16_lo(xk.w), bf16_hi(xk.w)};
-  float o[8], gmv[8];
+  f[0] = apply_act(f[0], a.act);
+  f[1] = apply_act(f[1], a.act);
+  if (a.out_dtype == 0) {  // c even, pitch % 8 == 0: a 4-byte store
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(a.out) + p.pix * a.out_pitch + c) = pack_bf16(f[0], f[1]);
+  } else if (a.out_layout == 0) {
+    float* op = reinterpret_cast<float*>(a.out) + p.pix * a.out_pitch + c;
+    op[0] = f[0];
+    if (c + 1 < a.out_c) op[1] = f[1];
+  } else {  // fp32 NCHW
+    float* op = reinterpret_cast<float*>(a.out);
+    const long long hw = (long long)a.Hout * a.Wout;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float xval = fmaf(nz, nsv[i], xs[i]);
-    const float gm = __uint_as_float(v[2 * i]) + sh[2 * i];
-    const float bt = __uint_as_float(v[2 * i + 1]) + sh[2 * i + 1];
-    const float xn = (xval - mu[i]) * rs[i];
-    gmv[i] = gm;
-    o[i] = fmaf(xn, 1.f + gm, bt);
-  }
-  apply_act8(o, a.act);
-  if (a.gamma_out)
-    *reinterpret_cast<uint4*>(a.gamma_out + t.pix * a.gamma_pitch + c0) =
-        make_uint4(pack_bf16(gmv[0], gmv[1]), pack_bf16(gmv[2], gmv[3]), pack_bf16(gmv[4], gmv[5]), pack_bf16(gmv[6], gmv[7]));
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + t.pix * a.out_pitch + c0) =
-      make_uint4(pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]));
-}
-
-// the whole-tile loop (accumulator complete; xv holds the x of chunks 0..3)
-__device__ __forceinline__ void epi_spade_tile(const ConvArgs& a, const EpiTile& t, long long pix0, float nz, uint4 (&xv)[4], uint32_t tab) {
-  const int nchunks = a.BN >> 4;
-  for (int k0 = 0; k0 < nchunks; k0 += 4) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      if (k0 + j < nchunks) epi_spade_chunk(a, t, (k0 + j) * 16, xv[j], nz, tab);
-      xv[j] = epi_spade_x(a, t, (k0 + 4 + j) * 16, pix0);  // refill: the load has three chunks of work to hide behind
-    }
+    for (int i = 0; i < 2; ++i)
+      if (c + i < a.out_c) op[((long long)p.n * a.out_c + c + i) * hw + (long long)p.y * a.Wout + p.x] = f[i];
   }
 }
 
-// ------------------------------------------------------------------------------------------------ unrolled MMA issue of a tap group
-// The per-tap issue loop costs the MMA warp ~290 cycles per tap whatever the tile width: every iteration elects a lane, moves six
-// descriptor words from vector to uniform registers (R2UR; UTCHMMA takes uniform operands), re-reads its loop bound from the constant
-// bank (LDCU -> MOV -> ISETP -> BRA), reconverges (BSYNC / BRA.DIV).  For tiles of <= 64 columns that is 3-7x the tensor pipe's own
-// time for the tap (profiles/r2_conv_stall_thin_tiles_ab.txt: 2634 cycles per tile for 18 MMAs of 40 cycles).  Here ONE elected
-// region issues every MMA of a group of NT taps: the group's base descriptors cross to the uniform registers once, tap offsets inside
-// the group are compile-time constants of the 3x3 halo geometry (row pitch 8 + 3 - 1 = 10 pixels), and nothing is re-read.
-// NT = 9: all taps of a 3x3 kernel (weight stage holds 9 taps); NT = 3: one kernel row.
-template <int NT, int BKT, bool PAIR>
-__device__ __forceinline__ void issue_tap_group(uint32_t d_tmem, uint64_t da0, uint64_t db0, uint32_t b_step16, uint32_t idesc, uint32_t accumulate) {
-  constexpr uint32_t ROWB16 = (uint32_t)BKT * 2u / 16u;  // one pixel row of the halo tile, in descriptor units (16 B)
-#pragma unroll
-  for (int t = 0; t < NT; ++t) {
-    const uint32_t a_off = (uint32_t)((t / 3) * 10 + (t % 3)) * ROWB16;  // NT = 3: t / 3 == 0
-    const uint64_t da = da0 + a_off, db = db0 + (uint64_t)((uint32_t)t * b_step16);
-#pragma unroll
-    for (int kk = 0; kk < BKT / 16; ++kk) {
-      const uint32_t accf = (t == 0 && kk == 0) ? accumulate : 1u;
-      if (PAIR) umma_f16_2sm(d_tmem, da + 2u * kk, db + 2u * kk, idesc, accf);
-      else umma_f16(d_tmem, da + 2u * kk, db + 2u * kk, idesc, accf);
-    }
-  }
+// SPADE epilogue of one channel ch of one pixel; g, b = the (gamma, beta) accumulators of columns 2ch, 2ch+1.
+__device__ __forceinline__ void epi_spade1(const ConvArgs& a, const EpiPix& p, long long pix0, float nz, int ch, float g, float b) {
+  if (!p.valid || ch >= a.C_mod) return;
+  const __nv_bfloat16* xp = (ch < a.x0_c) ? (a.x0 + pix0 * a.x0_pitch + ch) : (a.x1 + p.pix * a.x1_pitch + (ch - a.x0_c));
+  const float xs = __bfloat162float(*xp);
+  const float mu = __ldg(a.mean + (long long)p.n * a.C_mod + ch);
+  const float rs = __ldg(a.rstd + (long long)p.n * a.C_mod + ch);
+  const float ns = a.noise_scale ? __ldg(a.noise_scale + ch) : 0.f;
+  const float gm = g + (a.shift ? __ldg(a.shift + 2 * ch) : 0.f);
+  const float bt = b + (a.shift ? __ldg(a.shift + 2 * ch + 1) : 0.f);
+  const float xn = (fmaf(nz, ns, xs) - mu) * rs;
+  const float o = apply_act(fmaf(xn, 1.f + gm, bt), a.act);
+  if (a.gamma_out) a.gamma_out[p.pix * a.gamma_pitch + ch] = __float2bfloat16(gm);  // training: gamma for the backward pass
+  reinterpret_cast<__nv_bfloat16*>(a.out)[p.pix * a.out_pitch + ch] = __float2bfloat16(o);
 }
 
-template <int BK>
-__global__ void __launch_bounds__(kThreadsC, 1) conv_igemm_kernel(const __grid_constant__ ConvArgs a) {
-  constexpr uint32_t ROW_BYTES = BK * 2;               // one K chunk of one pixel / one output channel
-  constexpr uint32_t A_BYTES = 128 * ROW_BYTES;        // 128 pixels
-  constexpr uint32_t SBO = 8 * ROW_BYTES;              // 8-row core-matrix group stride
-  constexpr uint32_t LAYOUT = (BK == 64) ? 2u : (BK == 32 ? 4u : 6u);  // SW128 / SW64 / SW32
+template <int BNT>
+__device__ __forceinline__ void wgmma_tile(float (&d)[BNT / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (BNT == 64) wgmma_n64<0, 0>(d, da, db, scale_d);
+  else wgmma_n128<0, 0>(d, da, db, scale_d);
+}
+
+template <int BNT>
+__global__ void __launch_bounds__(kThreads, 2) conv_wgmma_kernel(const __grid_constant__ ConvArgs a) {
+  constexpr uint32_t B_BYTES = (uint32_t)BNT * kRowBytes;
+  constexpr uint32_t STAGE = kABytes + B_BYTES;  // both parts multiples of 1024 B: every operand starts at swizzle phase 0
+  constexpr int R = BNT / 2;                     // accumulator registers per consumer thread
 
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  // control block [0,2048): four barrier arrays of kMaxStages (A full/empty, B full/empty), TMEM barriers, TMEM pointer.
-  // Tap-by-tap mode uses only the "A" ring (each stage = A box + B box); halo mode uses both rings.
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   auto bar_full = [&](int s) { return base + 8u * s; };
-  auto bar_empty = [&](int s) { return base + 256u + 8u * s; };
-  auto bar_bfull = [&](int s) { return base + 512u + 8u * s; };
-  auto bar_bempty = [&](int s) { return base + 768u + 8u * s; };
-  auto bar_tfull = [&](int i) { return base + 1024u + 8u * i; };
-  auto bar_tempty = [&](int i) { return base + 1088u + 8u * i; };
-  const uint32_t tmem_slot = base + 1152u;
-  const uint32_t NACC = (uint32_t)a.nacc;
-  const uint32_t b_bytes = (uint32_t)a.BN * ROW_BYTES;
-  const uint32_t stage_bytes = a.halo ? (uint32_t)a.a_stage_bytes : A_BYTES + ((b_bytes + 1023u) & ~1023u);
-  const uint32_t stage0 = base + 2048u;
-  const uint32_t bstage0 = stage0 + (uint32_t)a.stages * stage_bytes;  // halo mode: weight ring after the halo ring
+  auto bar_empty = [&](int s) { return base + 128u + 8u * s; };
+  const uint32_t stage0 = base + 1024u;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int S = a.stages;
-  const int SB = a.sb_stages;
   const int KT = a.KH * a.KW * a.chunks;
-  const int total_tiles = a.tiles_n * a.tiles_x * a.tiles_y * a.tiles_img;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)a.nacc * a.BN) tmem_cols <<= 1;
+  const int nt = blockIdx.x % a.tiles_n;
+  int mt = blockIdx.x / a.tiles_n;
+  const int tx = mt % a.tiles_x;
+  mt /= a.tiles_x;
+  const int ty = mt % a.tiles_y;
+  const int ti = mt / a.tiles_y;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&a.tmA);
-    tma_prefetch_desc(&a.tmB);
-  } else if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(bar_full(s), 1);
-      mbar_init(bar_empty(s), 1);
-    }
-    for (int s = 0; s < SB; ++s) {
-      mbar_init(bar_bfull(s), 1);
-      mbar_init(bar_bempty(s), 1);
-    }
-    for (int i = 0; i < a.nacc; ++i) {
-      mbar_init(bar_tfull(i), 1);
-      mbar_init(bar_tempty(i), a.epi_own ? 4 : 4 * kEpiC);  // one arrival per epilogue warp that drains the accumulator
+      mbar_init(bar_empty(s), 4 * kConsumers);  // one arrival per consumer warp
     }
     fence_mbar_init();
-  } else if (warp == 2) {
-    tmem_alloc(tmem_slot, tmem_cols);
-    tmem_relinquish();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
-  const bool acct = a.stats != nullptr;
-  unsigned long long w0 = 0, w1 = 0, w2 = 0;  // stall cycles per barrier class of this warp's role
-  const long long t_begin = acct ? clock64() : 0;
 
-  if (warp == 0) {
-    // ===================================================== TMA producer (whole warp, warp-uniform; one elected lane issues)
-    // All ring cursors (stage index, phase bit, smem address) advance incrementally: no divisions in the hot loops.
-    const int taps = a.KH * a.KW;
-    (void)taps;
-    if (a.halo) {
-      // halo (A) producer: runs ahead of the MMAs by up to S channel chunks, possibly into later tiles.  The weights have their own
-      // producer (warp 3): coupling the two in one loop made the weight loads of chunk k wait until the MMAs had released the halo
-      // stage of chunk k-1 (tools/conv_stall_probe.py: producer 59% blocked on a free halo stage while the MMA warp starved on weights)
-      int as = 0, akc = 0, atile = blockIdx.x;
-      uint32_t aph = 0, a_addr = stage0;
-      for (; atile < total_tiles;) {
-        int mta = atile / a.tiles_n;
-        const int txa = mta % a.tiles_x;
-        mta /= a.tiles_x;
-        const int tya = mta % a.tiles_y;
-        const int an0 = mta / a.tiles_y;
-        const int ax0 = (txa << a.tw_log) - a.off_x;
-        const int ay0 = (tya << a.th_log) - a.off_y;
-        for (akc = 0; akc < a.chunks; ++akc) {
-          mbar_wait_acct(bar_empty(as), aph ^ 1u, acct, w0);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(bar_full(as), (uint32_t)a.a_stage_bytes_tx);
-            tma_load_4d(a_addr, &a.tmA, bar_full(as), akc * BK, ax0, ay0, an0);
-          }
-          __syncwarp();
-          a_addr += stage_bytes;
-          if (++as == S) { as = 0; aph ^= 1u; a_addr = stage0; }
-        }
-        atile += gridDim.x;
-      }
-    } else {
-      int st = 0;
+  if (warp == 4 * kConsumers) {
+    // ===================================================== TMA producer (one lane)
+    if (lane == 0) {
+      tma_prefetch_desc(&a.tmA);
+      tma_prefetch_desc(&a.tmB);
+      const int x0 = (tx << a.tw_log) - a.off_x;
+      const int y0 = (ty << a.th_log) - a.off_y;
+      const int n0 = ti << (7 - a.tw_log - a.th_log);
+      int st = 0, ky = 0, kx = 0, kc = 0, tap = 0;
       uint32_t ph = 0, sa = stage0;
-      const uint32_t tx_bytes = A_BYTES + b_bytes;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int nt = tile % a.tiles_n;
-        int mt = tile / a.tiles_n;
-        const int tx = mt % a.tiles_x;
-        mt /= a.tiles_x;
-        const int ty = mt % a.tiles_y;
-        const int ti = mt / a.tiles_y;
-        const int x0 = (tx << a.tw_log) - a.off_x;
-        const int y0 = (ty << a.th_log) - a.off_y;
-        const int n0 = ti << (7 - a.tw_log - a.th_log);
-        int tap = 0;
-        for (int ky = 0; ky < a.KH; ++ky) {
-          for (int kx = 0; kx < a.KW; ++kx, ++tap) {
-            for (int kc = 0; kc < a.chunks; ++kc) {
-              mbar_wait_acct(bar_empty(st), ph ^ 1u, acct, w0);
-              if (elect_one()) {
-                mbar_arrive_expect_tx(bar_full(st), tx_bytes);
-                tma_load_4d(sa, &a.tmA, bar_full(st), kc * BK, x0 + kx, y0 + ky, n0);
-                tma_load_3d(sa + A_BYTES, &a.tmB, bar_full(st), kc * BK, nt * a.BN, tap);
-              }
-              __syncwarp();
-              sa += stage_bytes;
-              if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
-            }
-          }
-        }
-      }
-    }
-    if (acct && lane == 0) a.stats[blockIdx.x * 16 + 4] = w0;
-  } else if (warp == 3) {
-    // ===================================================== weight (B) producer of the halo mainloop: `tpb` taps per TMA
-    if (a.halo) {
-      const int taps = a.KH * a.KW;
-      int bs = 0;
-      uint32_t bph = 0, b_addr = bstage0;
-      const uint32_t b_tx = (uint32_t)a.tpb * b_bytes;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        const int nt = tile % a.tiles_n;
-        for (int kc = 0; kc < a.chunks; ++kc) {
-          for (int t0 = 0; t0 < taps; t0 += a.tpb) {
-            mbar_wait_acct(bar_bempty(bs), bph ^ 1u, acct, w1);
-            if (elect_one()) {
-              mbar_arrive_expect_tx(bar_bfull(bs), b_tx);
-              tma_load_3d(b_addr, &a.tmB, bar_bfull(bs), kc * BK, nt * a.BN, t0);
-            }
-            __syncwarp();
-            b_addr += (uint32_t)a.b_stage_bytes;
-            if (++bs == SB) { bs = 0; bph ^= 1u; b_addr = bstage0; }
-          }
-        }
-      }
-      if (acct && lane == 0) a.stats[blockIdx.x * 16 + 5] = w1;
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer (whole warp, warp-uniform; one elected lane issues)
-    const uint32_t idesc = make_idesc_bf16(128, (uint32_t)a.BN);
-    const int taps = a.KH * a.KW;
-    const uint64_t db_hi = make_smem_desc(0, SBO, LAYOUT);
-    uint32_t acc = 0, acc_ph = 0;  // TMEM accumulator buffer and its phase
-    if (a.halo) {
-      // descriptors = constant high words | (address >> 4); taps advance by adding row offsets
-      const uint64_t da_hi = make_smem_desc(0, (uint32_t)a.line_pitch * ROW_BYTES, LAYOUT);  // SBO = one output row of 8 px
-      const uint32_t row_wrap = (uint32_t)(a.line_pitch - a.KW) * ROW_BYTES;
-      const int group_mode = a.tap_group;  // 0 / 3 / 9 (host: 3x3, row pitch 10, tpb == group size)
-      int as = 0, bs = 0;
-      uint32_t aph = 0, bph = 0, a_addr = stage0, b_addr = bstage0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait_acct(bar_tempty(acc), acc_ph ^ 1u, acct, w2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * (uint32_t)a.BN;
-        uint32_t accumulate = 0;
-        for (int kc = 0; kc < a.chunks; ++kc) {
-          mbar_wait_acct(bar_full(as), aph, acct, w0);
-          uint32_t sa_tap = a_addr;  // shifted view of the halo tile, advanced tap by tap
-          int kx = 0;
-          for (int t0 = 0; t0 < taps; t0 += a.tpb) {
-            mbar_wait_acct(bar_bfull(bs), bph, acct, w1);
-            tc_fence_after();
-            uint32_t sb_tap = b_addr;
-            if (group_mode) {  // 3x3: the whole group (9 taps, or one kernel row) from one elected region (issue_tap_group)
-              const uint64_t da0 = da_hi | (uint64_t)((sa_tap & 0x3FFFFu) >> 4);
-              const uint64_t db0 = db_hi | (uint64_t)((sb_tap & 0x3FFFFu) >> 4);
-              if (elect_one()) {
-                if (group_mode == 9) issue_tap_group<9, BK, false>(d_tmem, da0, db0, b_bytes >> 4, idesc, accumulate);
-                else issue_tap_group<3, BK, false>(d_tmem, da0, db0, b_bytes >> 4, idesc, accumulate);
-              }
-              __syncwarp();
-              accumulate = 1;
-              sa_tap += 10u * ROW_BYTES;  // next kernel row (unused after a 9-tap group)
-            } else
-            for (int t = 0; t < a.tpb; ++t) {
-              const uint64_t da = da_hi | (uint64_t)((sa_tap & 0x3FFFFu) >> 4);
-              const uint64_t db = db_hi | (uint64_t)((sb_tap & 0x3FFFFu) >> 4);
-              if (elect_one()) {
-#pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk) umma_f16(d_tmem, da + 2u * kk, db + 2u * kk, idesc, (kk == 0) ? accumulate : 1u);
-              }
-              __syncwarp();
-              accumulate = 1;
-              sb_tap += b_bytes;
-              sa_tap += ROW_BYTES;
-              if (++kx == a.KW) { kx = 0; sa_tap += row_wrap; }
-            }
-            if (elect_one()) umma_commit(bar_bempty(bs));
-            __syncwarp();
-            b_addr += (uint32_t)a.b_stage_bytes;
-            if (++bs == SB) { bs = 0; bph ^= 1u; b_addr = bstage0; }
-          }
-          if (elect_one()) umma_commit(bar_empty(as));
-          __syncwarp();
-          a_addr += stage_bytes;
-          if (++as == S) { as = 0; aph ^= 1u; a_addr = stage0; }
-        }
-        if (elect_one()) umma_commit(bar_tfull(acc));  // accumulator complete -> epilogue
-        __syncwarp();
-        if (++acc == NACC) { acc = 0; acc_ph ^= 1u; }
-      }
-    } else {
-      const uint64_t da_hi = make_smem_desc(0, SBO, LAYOUT);
-      int st = 0;
-      uint32_t ph = 0, sa = stage0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait_acct(bar_tempty(acc), acc_ph ^ 1u, acct, w2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * (uint32_t)a.BN;
-        for (int k = 0; k < KT; ++k) {
-          mbar_wait_acct(bar_full(st), ph, acct, w0);
-          tc_fence_after();
-          const uint64_t da = da_hi | (uint64_t)((sa & 0x3FFFFu) >> 4);
-          const uint64_t db = db_hi | (uint64_t)(((sa + A_BYTES) & 0x3FFFFu) >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) umma_f16(d_tmem, da + 2u * kk, db + 2u * kk, idesc, (uint32_t)((k | kk) != 0));
-            umma_commit(bar_empty(st));  // frees this smem stage once the MMAs above have read it
-          }
-          __syncwarp();
-          sa += stage_bytes;
-          if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
-        }
-        if (elect_one()) umma_commit(bar_tfull(acc));  // accumulator complete -> epilogue
-        __syncwarp();
-        if (++acc == NACC) { acc = 0; acc_ph ^= 1u; }
-      }
-    }
-    if (acct && lane == 0) {
-      unsigned long long* o = a.stats + blockIdx.x * 16;
-      o[0] = (unsigned long long)(clock64() - t_begin); o[1] = w0; o[2] = w1; o[3] = w2;
-      o[8] = (unsigned long long)((total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1);
-    }
-  } else if (warp >= 4) {
-    // ===================================================== epilogue (one TMEM lane = one pixel per thread)
-    const int q = warp & 3;             // TMEM lane quarter this warp may access
-    const int wg = (warp - 4) >> 2;     // epilogue warpgroup: owns 16-column chunks wg, wg+kEpiC, ...
-    const int r = q * 32 + lane;
-    const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
-    uint32_t acc = 0, aph = 0;
-    // Owner mode (thin LINEAR tiles): the tile in accumulator i belongs to warpgroup i % kEpiC, which drains all of its columns, so
-    // kEpiC tiles are in their epilogue at once.  With every warpgroup on the same tile the tile period is the LATENCY of one
-    // epilogue (wait -> tcgen05.ld -> convert -> st.global -> arrive: ~2800 cycles, profiles/r2_conv_stall_thin_tiles_ab.txt: every
-    // full-resolution layer with <= 64 columns took 0.54 ms whatever its K and N).  The accumulator count is a multiple of kEpiC
-    // (host), so a barrier always meets the same waiter in consecutive phases (mbarrier parity cannot tell phases two apart).
-    const bool own = a.epi_own != 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      if (own && (int)(acc % (uint32_t)kEpiC) != wg) {
-        if (++acc == NACC) { acc = 0; aph ^= 1u; }
-        continue;
-      }
-      const int nt = tile % a.tiles_n;
-      int mt = tile / a.tiles_n;
-      const int tx = mt % a.tiles_x;
-      mt /= a.tiles_x;
-      const int ty = mt % a.tiles_y;
-      const int ti = mt / a.tiles_y;
-      const int x = (tx << a.tw_log) + (r & tw_mask);
-      const int y = (ty << a.th_log) + ((r >> a.tw_log) & th_mask);
-      const int n = (ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
-      const bool valid = (x < a.Wout) && (y < a.Hout) && (n < a.Nimg);
-      const long long pix = ((long long)n * a.Hout + y) * a.Wout + x;
-
-      EpiTile et;
-      et.x = x; et.y = y; et.n = n; et.valid = valid; et.pix = pix; et.n_base = nt * a.BN;
-      et.taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)a.BN;
-
-      if (a.epi == 0) {
-        mbar_wait_acct(bar_tfull(acc), aph, acct, w0);
-        tc_fence_after();
-        if (own) epi_linear(a, et, 0, 1);
-        else epi_linear(a, et, wg);
-      } else {
-        uint4 xv[kMaxChunks];
-        float nz;
-        epi_spade_prefetch(a, et, wg, xv, nz);
-        mbar_wait_acct(bar_tfull(acc), aph, acct, w0);
-        tc_fence_after();
-        epi_spade_finish(a, et, wg, xv, nz);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty(acc));  // one arrival per warp (12 per tile instead of 384)
-      if (++acc == NACC) { acc = 0; aph ^= 1u; }
-    }
-    if (acct && warp == 4 && lane == 0) {  // first epilogue warp: time stalled on the accumulator vs total
-      a.stats[blockIdx.x * 16 + 6] = w0;
-      a.stats[blockIdx.x * 16 + 7] = (unsigned long long)(clock64() - t_begin);
-    }
-  }
-
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ CTA-pair variant (cta_group::2)
-// The one-CTA kernel above is bound by SHARED-MEMORY bandwidth, not by the tensor pipe, whenever the GEMM's N is wide and K is
-// streamed: per 128-pixel tile of the 128 -> 160 SPADE GEMM the tensor core reads 72 x (4 KB of A + 5 KB of B) = 663 KB and TMA
-// writes 46 KB (halo) + 368 KB (weights) = 414 KB; 1077 KB at 128 B/clk = 8400 cycles against 5760 cycles of MMAs
-// (tools/conv_stall_probe.py: the MMA warp spends 75% of its life blocked on issue, 23% waiting for weights; tools/umma_rate_probe.cu:
-// the same MMAs run at 100% when nothing else touches shared memory).  A CTA PAIR issues ONE tcgen05.mma.cta_group::2 of M = 256:
-// each CTA brings its own 128 pixels (halo box) and only HALF of every weight stage, so per CTA the weight bytes through shared
-// memory halve (written: 184 KB, read: 72 x 2.5 KB) -> 705 KB per tile, under the MMA time.
-//   pair = thread-block cluster of 2 on one TPC; rank 0 = leader.  Work item = (pair of adjacent pixel tiles, N tile).
-//   TMA:  both CTAs load into their own shared memory and signal the LEADER's full barriers (cp.async.bulk.tensor ... .cta_group::2).
-//   MMA:  the leader's warp 1 issues for both; tcgen05.commit ... .multicast::cluster releases the ring stages / publishes the
-//         accumulator in BOTH CTAs.
-//   Epilogue: each CTA drains its own TMEM; all 2 x 384 epilogue threads arrive on the leader's accumulator-empty barrier.
-// Halo mainloop, BK = 64, both epilogues (shared with the one-CTA kernel).  HRV_CONV_PAIR=0 disables it.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsC, 1) conv_pair_kernel(const __grid_constant__ ConvArgs a) {
-  constexpr uint32_t ROW_BYTES = 128;  // BK = 64 bf16
-  constexpr uint32_t LAYOUT = 2u;      // SWIZZLE_128B
-  constexpr int BK = 64;
-
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  auto bar_full = [&](int s) { return base + 8u * s; };            // leader: halo stage landed in BOTH CTAs
-  auto bar_empty = [&](int s) { return base + 256u + 8u * s; };    // local: this CTA's halo stage may be overwritten
-  auto bar_bfull = [&](int s) { return base + 512u + 8u * s; };    // leader: both halves of a weight stage landed
-  auto bar_bempty = [&](int s) { return base + 768u + 8u * s; };   // local
-  auto bar_tfull = [&](int i) { return base + 1024u + 8u * i; };   // local: accumulator i complete
-  auto bar_tempty = [&](int i) { return base + 1088u + 8u * i; };  // leader: accumulator i drained by both CTAs
-  const uint32_t tmem_slot = base + 1152u;
-  const uint32_t NACC = (uint32_t)a.nacc;
-  const uint32_t half_rows = (uint32_t)a.BN >> 1;
-  const uint32_t b_bytes = half_rows * ROW_BYTES;  // one tap of this CTA's half of the weight tile
-  const uint32_t stage_bytes = (uint32_t)a.a_stage_bytes;
-  const uint32_t tab0 = base + 2048u;  // kEpiC constant tables (SPADE with C_mod <= kTabMaxC), then the rings
-  const uint32_t stage0 = tab0 + (a.epi_tab ? ((uint32_t)kEpiC * kTabBytes + 1023u) & ~1023u : 0u);
-  const uint32_t bstage0 = stage0 + (uint32_t)a.stages * stage_bytes;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int cid = (int)cluster_id_x(), ncl = (int)cluster_nctaid_x();
-  const int S = a.stages, SB = a.sb_stages;
-  const int taps = a.KH * a.KW;
-  const int tiles_m = a.tiles_x * a.tiles_y * a.tiles_img;
-  const int items = a.tiles_n * ((tiles_m + 1) >> 1);
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)a.nacc * a.BN) tmem_cols <<= 1;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&a.tmA);
-    tma_prefetch_desc(&a.tmB);
-  } else if (warp == 1 && lane == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 1); }
-    for (int s = 0; s < SB; ++s) { mbar_init(bar_bfull(s), 1); mbar_init(bar_bempty(s), 1); }
-    for (int i = 0; i < a.nacc; ++i) { mbar_init(bar_tfull(i), 1); mbar_init(bar_tempty(i), 2 * 4); }  // one arrival per warp of the owning warpgroup in either CTA
-    fence_mbar_init();
-  } else if (warp == 2) {
-    tmem_alloc2(tmem_slot, tmem_cols);
-    tmem_relinquish2();
-  }
-  tc_fence_before();
-  cluster_sync_all();  // barriers of BOTH CTAs initialised before anyone signals the leader's
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
-  const bool acct = a.stats != nullptr && leader;
-  unsigned long long w0 = 0, w1 = 0, w2 = 0;
-  const long long t_begin = acct ? clock64() : 0;
-
-  if (warp == 0) {
-    // ===================================================== halo (A) producer (both CTAs): own pixel tile of every pair; runs ahead of the
-    // MMAs by up to S channel chunks.  The transaction bytes of both CTAs are expected on the LEADER's full barrier.
-    int as = 0;
-    uint32_t aph = 0, a_addr = stage0;
-    for (int item = cid; item < items; item += ncl) {
-      int mta = 2 * (item / a.tiles_n) + (int)rank;  // may lie past the last tile (odd tile count): TMA zero-fills, the epilogue skips it
-      const int txa = mta % a.tiles_x;
-      mta /= a.tiles_x;
-      const int tya = mta % a.tiles_y;
-      const int an0 = mta / a.tiles_y;
-      const int ax0 = (txa << a.tw_log) - a.off_x;
-      const int ay0 = (tya << a.th_log) - a.off_y;
-      for (int akc = 0; akc < a.chunks; ++akc) {
-        mbar_wait_acct(bar_empty(as), aph ^ 1u, acct, w0);
-        if (elect_one()) {
-          if (leader) mbar_arrive_expect_tx(bar_full(as), 2u * (uint32_t)a.a_stage_bytes_tx);
-          tma_load_4d_2sm(a_addr, &a.tmA, bar_full(as), akc * BK, ax0, ay0, an0);
-        }
-        __syncwarp();
-        a_addr += stage_bytes;
-        if (++as == S) { as = 0; aph ^= 1u; a_addr = stage0; }
-      }
-    }
-    if (acct && lane == 0) a.stats[cid * 16 + 4] = w0;
-  } else if (warp == 3) {
-    // ===================================================== weight (B) producer (both CTAs): THIS CTA's half of every weight stage
-    int bs = 0;
-    uint32_t bph = 0, b_addr = bstage0;
-    const uint32_t b_tx = (uint32_t)a.tpb * b_bytes;
-    for (int item = cid; item < items; item += ncl) {
-      const int nt = item % a.tiles_n;
-      for (int kc = 0; kc < a.chunks; ++kc) {
-        for (int t0 = 0; t0 < taps; t0 += a.tpb) {
-          mbar_wait_acct(bar_bempty(bs), bph ^ 1u, acct, w1);
-          if (elect_one()) {
-            if (leader) mbar_arrive_expect_tx(bar_bfull(bs), 2u * b_tx);
-            tma_load_3d_2sm(b_addr, &a.tmB, bar_bfull(bs), kc * BK, nt * a.BN + (int)(rank * half_rows), t0);
-          }
-          __syncwarp();
-          b_addr += (uint32_t)a.b_stage_bytes;
-          if (++bs == SB) { bs = 0; bph ^= 1u; b_addr = bstage0; }
-        }
-      }
-    }
-    if (acct && lane == 0) a.stats[cid * 16 + 5] = w1;
-  } else if (warp == 1 && leader) {
-    // ===================================================== MMA issuer (leader only): M = 256 over the pair
-    const uint32_t idesc = make_idesc_bf16(256, (uint32_t)a.BN);
-    const uint64_t db_hi = make_smem_desc(0, 8 * ROW_BYTES, LAYOUT);
-    const uint64_t da_hi = make_smem_desc(0, (uint32_t)a.line_pitch * ROW_BYTES, LAYOUT);  // SBO = one output row of 8 px
-    const uint32_t row_wrap = (uint32_t)(a.line_pitch - a.KW) * ROW_BYTES;
-    const int group_mode = a.tap_group;  // 0 / 3 / 9 (host: 3x3, row pitch 10, tpb == group size)
-    uint32_t acc = 0, acc_ph = 0;
-    int as = 0, bs = 0;
-    uint32_t aph = 0, bph = 0, a_addr = stage0, b_addr = bstage0;
-    for (int item = cid; item < items; item += ncl) {
-      mbar_wait_acct(bar_tempty(acc), acc_ph ^ 1u, acct, w2);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * (uint32_t)a.BN;
-      uint32_t accumulate = 0;
-      for (int kc = 0; kc < a.chunks; ++kc) {
-        mbar_wait_acct(bar_full(as), aph, acct, w0);
-        uint32_t sa_tap = a_addr;
-        int kx = 0;
-        for (int t0 = 0; t0 < taps; t0 += a.tpb) {
-          mbar_wait_acct(bar_bfull(bs), bph, acct, w1);
-          tc_fence_after();
-          uint32_t sb_tap = b_addr;
-          if (group_mode) {  // 3x3: the whole group (9 taps, or one kernel row) from one elected region (issue_tap_group)
-            const uint64_t da0 = da_hi | (uint64_t)((sa_tap & 0x3FFFFu) >> 4);
-            const uint64_t db0 = db_hi | (uint64_t)((sb_tap & 0x3FFFFu) >> 4);
-            if (elect_one()) {
-              if (group_mode == 9) issue_tap_group<9, BK, true>(d_tmem, da0, db0, b_bytes >> 4, idesc, accumulate);
-              else issue_tap_group<3, BK, true>(d_tmem, da0, db0, b_bytes >> 4, idesc, accumulate);
-            }
-            __syncwarp();
-            accumulate = 1;
-            sa_tap += 10u * ROW_BYTES;  // next kernel row (unused after a 9-tap group)
-          } else
-          for (int t = 0; t < a.tpb; ++t) {
-            const uint64_t da = da_hi | (uint64_t)((sa_tap & 0x3FFFFu) >> 4);
-            const uint64_t db = db_hi | (uint64_t)((sb_tap & 0x3FFFFu) >> 4);
-            if (elect_one()) {
-#pragma unroll
-              for (int kk = 0; kk < BK / 16; ++kk) umma_f16_2sm(d_tmem, da + 2u * kk, db + 2u * kk, idesc, (kk == 0) ? accumulate : 1u);
-            }
-            __syncwarp();
-            accumulate = 1;
-            sb_tap += b_bytes;
-            sa_tap += ROW_BYTES;
-            if (++kx == a.KW) { kx = 0; sa_tap += row_wrap; }
-          }
-          if (elect_one()) umma_commit_2sm(bar_bempty(bs));  // weight stage free in both CTAs
-          __syncwarp();
-          b_addr += (uint32_t)a.b_stage_bytes;
-          if (++bs == SB) { bs = 0; bph ^= 1u; b_addr = bstage0; }
-        }
-        if (elect_one()) umma_commit_2sm(bar_empty(as));  // halo stage free in both CTAs
-        __syncwarp();
-        a_addr += stage_bytes;
-        if (++as == S) { as = 0; aph ^= 1u; a_addr = stage0; }
-      }
-      if (elect_one()) umma_commit_2sm(bar_tfull(acc));  // accumulator complete -> both epilogues
-      __syncwarp();
-      if (++acc == NACC) { acc = 0; acc_ph ^= 1u; }
-    }
-    if (acct && lane == 0) {
-      unsigned long long* o = a.stats + cid * 16;
-      o[0] = (unsigned long long)(clock64() - t_begin); o[1] = w0; o[2] = w1; o[3] = w2;
-      o[8] = items > cid ? (unsigned long long)((items - 1 - cid) / ncl + 1) : 0ull;
-    }
-  } else if (warp >= 4) {
-    // ===================================================== epilogue (both CTAs, own TMEM)
-    const int q = warp & 3;
-    const int wg = (warp - 4) >> 2;
-    const int r = q * 32 + lane;
-    const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
-    uint32_t acc = 0, aph = 0;
-    const uint32_t tab = a.epi_tab ? tab0 + (uint32_t)wg * kTabBytes : 0u;
-    int tab_n = -1;  // image whose constants this warpgroup's table holds
-    for (int item = cid; item < items; item += ncl) {
-      if ((int)acc != wg) {  // the tile in accumulator `acc` belongs to warpgroup `acc` (NACC <= kEpiC): keep the ring cursor in step.
-        // One owner per accumulator also keeps every warpgroup within one phase of the barriers it waits on — an mbarrier parity wait
-        // is ambiguous for a waiter two phases ahead or behind, which a round-robin over tiles would allow when NACC != kEpiC.
-        if (++acc == NACC) { acc = 0; aph ^= 1u; }
-        continue;
-      }
-      const int nt = item % a.tiles_n;
-      int mt = 2 * (item / a.tiles_n) + (int)rank;
-      const int tx = mt % a.tiles_x;
-      mt /= a.tiles_x;
-      const int ty = mt % a.tiles_y;
-      const int ti = mt / a.tiles_y;
-      EpiTile et;
-      et.x = (tx << a.tw_log) + (r & tw_mask);
-      et.y = (ty << a.th_log) + ((r >> a.tw_log) & th_mask);
-      et.n = (ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
-      et.valid = (et.x < a.Wout) && (et.y < a.Hout) && (et.n < a.Nimg);
-      et.pix = ((long long)et.n * a.Hout + et.y) * a.Wout + et.x;
-      et.n_base = nt * a.BN;
-      et.taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)a.BN;
-      if (a.epi == 0) {
-        mbar_wait_acct(bar_tfull(acc), aph, acct, w0);
-        tc_fence_after();
-        epi_linear(a, et, 0, 1);
-      } else {
-        const int sh0 = a.x0_shift;
-        const long long pix0 = ((long long)et.n * (a.Hout >> sh0) + (et.y >> sh0)) * (a.Wout >> sh0) + (et.x >> sh0);
-        const float nz = (et.valid && a.noise) ? __ldg(a.noise + et.pix) : 0.f;
-        uint4 xv[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) xv[j] = epi_spade_x(a, et, j * 16, pix0);
-        if (tab && ti != tab_n && ti < a.Nimg) {  // (halo tiles hold one image: ti is the image index)  new image: refill the table
-          named_bar_sync(1 + wg, 128);            // every warp of the warpgroup is past its reads of the old table
-          float* T = reinterpret_cast<float*>(smem_raw + (tab - raw));
-          for (int c = r; c < a.C_mod; c += 128) {
-            T[c] = __ldg(a.mean + (long long)ti * a.C_mod + c);
-            T[a.C_mod + c] = __ldg(a.rstd + (long long)ti * a.C_mod + c);
-            T[2 * a.C_mod + c] = a.noise_scale ? __ldg(a.noise_scale + c) : 0.f;
-            T[3 * a.C_mod + c] = a.shift ? __ldg(a.shift + 2 * c) : 0.f;
-            T[4 * a.C_mod + c] = a.shift ? __ldg(a.shift + 2 * c + 1) : 0.f;
-          }
-          named_bar_sync(1 + wg, 128);
-          tab_n = ti;
-        }
-        mbar_wait_acct(bar_tfull(acc), aph, acct, w0);
-        tc_fence_after();
-        epi_spade_tile(a, et, pix0, nz, xv, tab);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_leader(bar_tempty(acc));  // ONE (possibly remote) arrival per warp: 24 per item instead of 768 — remote
-                                                           // mbarrier arrivals are DSMEM transactions and serialise at the leader
-      if (++acc == NACC) { acc = 0; aph ^= 1u; }
-    }
-    if (acct && warp == 4 && lane == 0) {
-      a.stats[cid * 16 + 6] = w0;
-      a.stats[cid * 16 + 7] = (unsigned long long)(clock64() - t_begin);
-
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // nobody leaves (or frees TMEM) while the peer may still signal / read this CTA
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc2(tmem_base, tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ pixel-N variant
-// An M128 x N x K16 tcgen05.mma takes max(N/2, 32 + N/4) cycles (tools/umma_rate_probe.cu v2, profiles/r2_umma_rate_probe.txt; the
-// round-1 "153 cycles whatever N" was that probe's own scalar loop): few output channels as the MMA's N run the pipe at 20-66 %,
-// and every pixel tile re-reads the whole weight stage from shared memory.  This variant swaps the roles for Cout <= 128 — 256
-// pixels per instruction share one weight stage:
-//   A operand (M = 128 rows) = the packed weights (rows >= n_pad are TMA zero fill), B operand (N = 256) = 256 output pixels
-//   (two 128-pixel TMA boxes back to back), D[cout][pixel] in TMEM (2 x 256 columns).  Per instruction twice the pixels.
-// The epilogue thread owns one output channel (a TMEM lane): scale/shift/activation per thread, then a bf16 transpose through
-// shared memory so that every pixel's channels leave as contiguous 16-byte vectors (coalesced stores).
-// Tap-by-tap loading, BK = 64, LINEAR epilogue, bf16 NHWC output without residual; everything else stays on conv_igemm_kernel.
-// One thread = one output channel: 64 pixels (4 x tcgen05.ld of 16 columns) -> act(acc*sc+sh) -> bf16 -> column `tp` of the
-// [64 px][pitch] staging tile.
-template <int ACT>
-__device__ __forceinline__ void pixn_stage(uint32_t taddr, __nv_bfloat16* tp, int pitch, float sc, float sh, bool store) {
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {  // two 16-column loads in flight per wait (register budget: 640 threads/CTA)
-    uint32_t v[2][16];
-    tmem_ld16(taddr + half * 32, v[0]);
-    tmem_ld16(taddr + half * 32 + 16, v[1]);
-    tmem_wait_ld();
-    if (store) {
-#pragma unroll
-      for (int cb = 0; cb < 2; ++cb) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          *tp = __float2bfloat16(act_t<ACT>(fmaf(__uint_as_float(v[cb][i]), sc, sh)));
-          tp += pitch;
-        }
-      }
-    }
-  }
-}
-
-__global__ void __launch_bounds__(kThreads, 1) conv_pixn_kernel(const __grid_constant__ ConvArgs a) {
-  constexpr uint32_t ROW = 128;              // 64 bf16 channels
-  constexpr uint32_t BOX = 128 * ROW;        // one 128-pixel box / the 128-row weight tile: 16 KB
-  constexpr uint32_t PX_BYTES = 2 * BOX;     // 256 pixels
-  constexpr uint32_t STAGE = PX_BYTES + BOX; // 48 KB
-  constexpr uint32_t SBO = 8 * ROW;
-  constexpr uint32_t NACC = 2;
-
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  auto bar_full = [&](int s) { return base + 8u * s; };
-  auto bar_empty = [&](int s) { return base + 256u + 8u * s; };
-  auto bar_tfull = [&](int i) { return base + 1024u + 8u * i; };
-  auto bar_tempty = [&](int i) { return base + 1088u + 8u * i; };
-  const uint32_t tmem_slot = base + 1152u;
-  const uint32_t stage0 = base + 2048u;
-  const int S = a.stages;
-  const uint32_t staging0 = stage0 + (uint32_t)S * STAGE;  // kEpiWG x [64 px][store_c] bf16
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int KT = a.KH * a.KW * a.chunks;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&a.tmA);
-    tma_prefetch_desc(&a.tmB);
-  } else if (warp == 1 && lane == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(bar_full(s), 1);
-      mbar_init(bar_empty(s), 1);
-    }
-    for (int i = 0; i < (int)NACC; ++i) {
-      mbar_init(bar_tfull(i), 1);
-      mbar_init(bar_tempty(i), 128 * kEpiWG);
-    }
-    fence_mbar_init();
-  } else if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
-  const int sub_shift = 7 - a.tw_log - a.th_log;  // log2(images per 128-pixel box)
-
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    int st = 0;
-    uint32_t ph = 0, sa = stage0;
-    for (int pair = blockIdx.x; pair < a.pairs; pair += gridDim.x) {
-      int x0[2], y0[2], n0[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        int mt = 2 * pair + h;  // a box past the last tile decodes to n0 >= Nimg: TMA zero-fills it entirely
-        const int tx = mt % a.tiles_x;
-        mt /= a.tiles_x;
-        const int ty = mt % a.tiles_y;
-        const int ti = mt / a.tiles_y;
-        x0[h] = (tx << a.tw_log) - a.off_x;
-        y0[h] = (ty << a.th_log) - a.off_y;
-        n0[h] = ti << sub_shift;
-      }
-      int tap = 0;
-      for (int ky = 0; ky < a.KH; ++ky) {
-        for (int kx = 0; kx < a.KW; ++kx, ++tap) {
-          for (int kc = 0; kc < a.chunks; ++kc) {
-            mbar_wait(bar_empty(st), ph ^ 1u);
-            if (elect_one()) {
-              mbar_arrive_expect_tx(bar_full(st), STAGE);
-              tma_load_4d(sa, &a.tmA, bar_full(st), kc * 64, x0[0] + kx, y0[0] + ky, n0[0]);
-              tma_load_4d(sa + BOX, &a.tmA, bar_full(st), kc * 64, x0[1] + kx, y0[1] + ky, n0[1]);
-              tma_load_3d(sa + PX_BYTES, &a.tmB, bar_full(st), kc * 64, 0, tap);
-            }
-            __syncwarp();
-            sa += STAGE;
-            if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer: D[cout 128][pixel 256] += W[128][16] * X[256][16]^T
-    const uint32_t idesc = make_idesc_bf16(128, 256);
-    const uint64_t d_hi = make_smem_desc(0, SBO, 2u);
-    uint32_t acc = 0, acc_ph = 0;
-    int st = 0;
-    uint32_t ph = 0, sa = stage0;
-    for (int pair = blockIdx.x; pair < a.pairs; pair += gridDim.x) {
-      mbar_wait(bar_tempty(acc), acc_ph ^ 1u);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * 256u;
       for (int k = 0; k < KT; ++k) {
-        mbar_wait(bar_full(st), ph);
-        tc_fence_after();
-        const uint64_t dw = d_hi | (uint64_t)(((sa + PX_BYTES) & 0x3FFFFu) >> 4);
-        const uint64_t dx = d_hi | (uint64_t)((sa & 0x3FFFFu) >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_f16(d_tmem, dw + 2u * kk, dx + 2u * kk, idesc, (uint32_t)((k | kk) != 0));
-          umma_commit(bar_empty(st));
+        mbar_wait(bar_empty(st), ph ^ 1u);
+        mbar_arrive_expect_tx(bar_full(st), STAGE);
+        tma_load_4d(sa, &a.tmA, bar_full(st), kc * 64, x0 + kx, y0 + ky, n0);
+        tma_load_3d(sa + kABytes, &a.tmB, bar_full(st), kc * 64, nt * BNT, tap);
+        if (++kc == a.chunks) {
+          kc = 0;
+          ++tap;
+          if (++kx == a.KW) { kx = 0; ++ky; }
         }
-        __syncwarp();
         sa += STAGE;
         if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
       }
-      if (elect_one()) umma_commit(bar_tfull(acc));
-      __syncwarp();
-      if (++acc == NACC) { acc = 0; acc_ph ^= 1u; }
     }
-  } else if (warp >= 4) {
-    // ===================================================== epilogue (one TMEM lane = one output channel per thread)
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int wg = (warp - 4) >> 2;    // warpgroup: pixel columns [64*wg, 64*wg+64) of the tile
-    const int r = q * 32 + lane;       // output channel, and this thread's index inside its warpgroup
-    const int sc_n = a.store_c;
-    const bool warp_active = q * 32 < sc_n;  // warp-uniform (tcgen05.ld is warp-collective)
-    const float sc = r < a.n_gemm ? (a.scale ? __ldg(a.scale + r) : 1.f) : 0.f;  // channels >= n_gemm (pad) are written as act(0)
-    const float sh = (r < a.n_gemm && a.shift) ? __ldg(a.shift + r) : 0.f;
-    __nv_bfloat16* T = reinterpret_cast<__nv_bfloat16*>(smem_raw + (staging0 - raw)) + (size_t)wg * 64 * sc_n;
-    const int vpp = sc_n >> 3;         // 16-byte vectors per pixel
-    const int nvec = 64 * vpp;
-    const int pl0 = r / vpp, c80 = r - pl0 * vpp, step_pl = 128 / vpp, step_c8 = 128 - step_pl * vpp;
-    const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
-    const int h = wg >> 1;             // which 128-pixel box of the pair this warpgroup's columns belong to
-    uint32_t acc = 0, aph = 0;
-    for (int pair = blockIdx.x; pair < a.pairs; pair += gridDim.x) {
-      int mt = 2 * pair + h;
-      const int tx = mt % a.tiles_x;
-      mt /= a.tiles_x;
-      const int ty = mt % a.tiles_y;
-      const int ti = mt / a.tiles_y;
-      mbar_wait(bar_tfull(acc), aph);
-      tc_fence_after();
-      if (warp_active) {
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * 256u + (uint32_t)(wg * 64);
-        __nv_bfloat16* tp = T + r;
-        switch (a.act) {  // activation selected once per tile: the 64-element loop below is straight-line code
-          case 1: pixn_stage<1>(taddr, tp, sc_n, sc, sh, r < sc_n); break;
-          case 2: pixn_stage<2>(taddr, tp, sc_n, sc, sh, r < sc_n); break;
-          case 3: pixn_stage<3>(taddr, tp, sc_n, sc, sh, r < sc_n); break;
-          default: pixn_stage<0>(taddr, tp, sc_n, sc, sh, r < sc_n); break;
-        }
-      }
-      __syncwarp();
-      tc_fence_before();
-      mbar_arrive(bar_tempty(acc));  // the accumulator is free: the MMAs of the tile after next may start
-      named_bar_sync(1 + wg, 128);   // this warpgroup's [64 px][store_c] staging tile is complete
-      {
-        // vector v = r, r+128, ... of the [64 px][vpp] tile; (pixel, chunk) advance incrementally (no divisions in the loop)
-        int pl = pl0, c8 = c80;
-        for (int v = r; v < nvec; v += 128) {
-          const int rr = ((wg & 1) << 6) + pl;  // pixel index inside the 128-pixel box
-          const int x = (tx << a.tw_log) + (rr & tw_mask);
-          const int y = (ty << a.th_log) + ((rr >> a.tw_log) & th_mask);
-          const int n = (ti << sub_shift) + (rr >> (a.tw_log + a.th_log));
-          if (x < a.Wout && y < a.Hout && n < a.Nimg) {
-            const long long pix = ((long long)n * a.Hout + y) * a.Wout + x;
-            uint4 o = *reinterpret_cast<const uint4*>(T + pl * sc_n + c8 * 8);
-            if (a.res_mode) {  // fused activation backward of the layer below: out *= act'(res), res = that layer's saved output
-              const uint4 gq = __ldg(reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(a.res) + pix * a.res_pitch + c8 * 8));
-              const float slope = a.res_mode == 1 ? 0.f : 0.2f;
-              const uint32_t gw[4] = {gq.x, gq.y, gq.z, gq.w};
-              uint32_t ow[4] = {o.x, o.y, o.z, o.w};
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float lo = bf16_lo(gw[i]) > 0.f ? bf16_lo(ow[i]) : bf16_lo(ow[i]) * slope;
-                const float hi = bf16_hi(gw[i]) > 0.f ? bf16_hi(ow[i]) : bf16_hi(ow[i]) * slope;
-                ow[i] = pack_bf16(lo, hi);
-              }
-              o = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-            }
-            *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + pix * a.out_pitch + c8 * 8) = o;
-          }
-          pl += step_pl;
-          c8 += step_c8;
-          if (c8 >= vpp) { c8 -= vpp; ++pl; }
-        }
-      }
-      named_bar_sync(1 + wg, 128);   // staging tile drained before the next tile overwrites it
-      if (++acc == NACC) { acc = 0; aph ^= 1u; }
-    }
+    return;
   }
 
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ===================================================== consumers: warpgroup wg computes pixels [64 wg, 64 wg + 64) of the tile
+  const int wg = warp >> 2;
+  float acc[R];
+#pragma unroll
+  for (int i = 0; i < R; ++i) acc[i] = 0.f;
+  {
+    int st = 0, prev = 0;
+    uint32_t ph = 0, sa = stage0;
+    for (int k = 0; k < KT; ++k) {
+      mbar_wait(bar_full(st), ph);
+      wgmma_fence();
+      const uint32_t a_row0 = sa + (uint32_t)wg * (64u * kRowBytes);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {  // K = 16 per instruction: +32 bytes inside the 128-byte swizzle row
+        const uint64_t da = make_wgmma_desc(a_row0 + 32u * kk, 8 * kRowBytes, 1);
+        const uint64_t db = make_wgmma_desc(sa + kABytes + 32u * kk, 8 * kRowBytes, 1);
+        wgmma_tile<BNT>(acc, da, db, (uint32_t)((k | kk) != 0));
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the MMAs of the previous stage have finished reading it
+      if (k > 0 && lane == 0) mbar_arrive(bar_empty(prev));
+      prev = st;
+      sa += STAGE;
+      if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+  }
+
+  // ===================================================== epilogue straight from the accumulator registers
+  // wgmma m64nN fragment: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 and that + 8, columns 8 j + 2 (l % 4) + {0, 1}.
+  const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
+  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int n_base = nt * BNT + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r_base + 8 * h;
+    EpiPix p;
+    p.x = (tx << a.tw_log) + (r & tw_mask);
+    p.y = (ty << a.th_log) + ((r >> a.tw_log) & th_mask);
+    p.n = (ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
+    p.valid = (p.x < a.Wout) && (p.y < a.Hout) && (p.n < a.Nimg);
+    p.pix = ((long long)p.n * a.Hout + p.y) * a.Wout + p.x;
+    if (a.epi == 0) {
+#pragma unroll
+      for (int j = 0; j < BNT / 8; ++j) epi_linear2(a, p, n_base + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    } else {
+      const int sh0 = a.x0_shift;
+      const long long pix0 = ((long long)p.n * (a.Hout >> sh0) + (p.y >> sh0)) * (a.Wout >> sh0) + (p.x >> sh0);
+      const float nz = (p.valid && a.noise) ? __ldg(a.noise + p.pix) : 0.f;
+#pragma unroll
+      for (int j = 0; j < BNT / 8; ++j) epi_spade1(a, p, pix0, nz, (n_base + 8 * j) >> 1, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
   }
 }
 
@@ -1237,45 +276,23 @@ static int pick_pow2(int dim, int cap) {
   return best;
 }
 
-template <int BK>
+template <int BNT>
 static int launch_conv(const ConvArgs& args, int grid, size_t smem, cudaStream_t st) {
   static bool attr_done = false;
   if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<BK>, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
-    if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(conv_igemm): %s", cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(conv_wgmma_kernel<BNT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemPerCta);
+    if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(conv_wgmma): %s", cudaGetErrorString(e));
     attr_done = true;
   }
-  conv_igemm_kernel<BK><<<grid, kThreadsC, smem, st>>>(args);
+  conv_wgmma_kernel<BNT><<<grid, kThreads, smem, st>>>(args);
   cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_igemm launch: %s", cudaGetErrorString(e));
-  return HRV_OK;
-}
-
-static int launch_pixn(const ConvArgs& args, int grid, size_t smem, cudaStream_t st) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_pixn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
-    if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(conv_pixn): %s", cudaGetErrorString(e));
-    attr_done = true;
-  }
-  conv_pixn_kernel<<<grid, kThreads, smem, st>>>(args);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_pixn launch: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_wgmma launch: %s", cudaGetErrorString(e));
   return HRV_OK;
 }
 
 }  // namespace hrv
 
 using namespace hrv;
-
-#ifndef HRV_F16
-// Debug hook of tools/conv_stall_probe.py (not part of the public header): subsequent bf16 convolutions on the classic kernel write
-// per-CTA stall counters (16 x u64 per CTA) into `buf` (device memory for >= sm_count CTAs); nullptr switches it off.
-static unsigned long long* g_conv_stats = nullptr;
-extern "C" void hrv_debug_set_conv_stats(void* buf) { g_conv_stats = (unsigned long long*)buf; }
-#else
-static unsigned long long* const g_conv_stats = nullptr;
-#endif
 
 extern "C" int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream) {
   if (!p) return set_error(HRV_EINVAL, "conv: null params");
@@ -1297,56 +314,20 @@ extern "C" int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream) {
   ConvArgs a;
   memset(&a, 0, sizeof(a));
   a.Nimg = out.n; a.Hout = out.h; a.Wout = out.w;
-  a.stats = g_conv_stats;
-  const char* force = getenv("HRV_CONV_HALO");  // read per call (tests / A-B runs flip it)
-  // CTA-pair kernel (cta_group::2, M = 256 over two SMs, each CTA holds half of every weight stage): 3x3 GEMMs whose one-CTA form is
-  // bound by shared-memory bandwidth (profiles/r2_conv_stall_*.txt: +20..65 % for every tile width from 64 to 256 columns).  Needs
-  // the halo mainloop, 64-channel K blocks and an even SM count.
-  const char* env_pair = getenv("HRV_CONV_PAIR");        // read per call (tests compare the two kernels on identical inputs)
-  const char* env_minbn = getenv("HRV_CONV_PAIR_MINBN");  // A-B knobs (tools/conv_stall_probe.py, bench.py)
-  const char* env_over = getenv("HRV_CONV_PAIR_OVER_PIXN_MAXBN");
-  const int pair_min_bn = env_minbn ? atoi(env_minbn) : 32;
-  const int pair_over_pixn = env_over ? atoi(env_over) : 64;
-  const bool pair_geom = p->bk == 64 && p->bn >= pair_min_bn && p->bn >= 32 && p->bn <= 256 && (p->bn % 16) == 0 && out.h >= 12 && p->kh * p->kw > 1;
-  const bool pair_ok = pair_geom && !(env_pair && env_pair[0] == '0') && !(force && force[0] == '0') && (sm_count() % 2) == 0;
-  // Pixel-N variant (weights as the M operand, 256 pixels as N): few output channels, plain bf16 NHWC output.
-  const char* env_pixn = getenv("HRV_CONV_PIXN");  // read per call: tests flip it to compare the two kernels on identical inputs
-  const bool pixn_ok = !(env_pixn && env_pixn[0] == '0') && p->epi == HRV_EPI_LINEAR && p->bk == 64 && p->n_gemm <= 128 &&
-                    out.dtype == HRV_BF16 && p->out_layout == HRV_NHWC && (!p->res.ptr || p->res_mode != 0) && in.c > 32 &&
-                    ((out.c + 7) & ~7) <= out.pitch && ((out.c + 7) & ~7) <= 128;
-  // Both kernels can run a narrow 3x3 GEMM.  Measured per layer inside the train step (profiles/r2_kernel_selection_ab.txt): the pair
-  // kernel wins for <= 64 columns fed by more than 64 channels (144->64 -14 %, 128->64 -16 %, 80->32 -29 %) and whenever the
-  // pixel-N kernel's 256-pixel tiles cannot fill the SMs (2080->128 at 32x24: -39 %); pixel-N wins for 64->64 (+21 % if moved), the
-  // 2x2 space-to-depth convolutions and everything with 128 columns at 128x96 and above.
-  const long long pixn_tiles = ((long long)out.n * out.h * out.w + 255) / 256;
-  const bool pair_beats_pixn = pair_ok && ((p->bn <= pair_over_pixn && p->kh * p->kw == 9 && in.c > 64 && !p->res.ptr) || pixn_tiles < sm_count());
-  const bool pixn = pixn_ok && !pair_beats_pixn;
-  // Halo mode (one (16+KH-1)x(8+KW-1) box per channel chunk, taps as shifted descriptor views) whenever the image is
-  // tall enough for a 16x8 single-image tile; tap-by-tap mode (tile may span images) for the tiny pyramid levels.
-  // Measured on B200 (tools/conv_bench.py, profiles/conv_variants_r1.txt): the halo path wins for narrow GEMMs
-  // (N <= 32: 1.3-1.45x) and for the 144..208-column SPADE gamma/beta GEMMs (+5%); tap-by-tap wins for 1x1 and N=256.
-  const bool halo_shape = (p->bn <= 32) || (p->bk == 16) || (p->bk == 64 && p->bn >= 144 && p->bn <= 208);
-  bool halo = out.h >= 12 && p->kh * p->kw > 1 && halo_shape && !pixn;
-  if (force && force[0] == '0') halo = false;
-  if (force && force[0] == '1') halo = true;
-  const bool pair = pair_ok && !pixn;
-  if (pair) halo = true;
-  const int TW = halo ? 8 : pick_pow2(out.w, 128);
-  const int TH = halo ? 16 : pick_pow2(out.h, 128 / TW);
+  // N tile: 64 columns for narrow GEMMs, else 128 (a 64 x 128 fp32 accumulator is 64 registers per thread, which keeps two CTAs
+  // resident per SM).  Independent of the packing's bn: the weight map's row extent is the packed n_pad, rows past it are zero fill.
+  const int bnt = p->n_gemm <= 64 ? 64 : 128;
+  const int TW = pick_pow2(out.w, 128);
+  const int TH = pick_pow2(out.h, 128 / TW);
   const int TN = 128 / (TW * TH);
   a.tw_log = log2i(TW); a.th_log = log2i(TH);
   a.tiles_x = (out.w + TW - 1) / TW;
   a.tiles_y = (out.h + TH - 1) / TH;
   a.tiles_img = (out.n + TN - 1) / TN;
-  a.tiles_n = (p->n_gemm + p->bn - 1) / p->bn;
+  a.tiles_n = (p->n_gemm + bnt - 1) / bnt;
   a.KH = p->kh; a.KW = p->kw; a.off_y = p->off_y; a.off_x = p->off_x;
-  a.chunks = (in.c + p->bk - 1) / p->bk;
-  a.BN = p->bn; a.n_gemm = p->n_gemm;
-  a.nacc = 512 / p->bn > 8 ? 8 : 512 / p->bn;
-  if (pair && a.nacc > kEpiC) a.nacc = kEpiC;  // pair kernel: accumulator w is drained by epilogue warpgroup w
-  const char* env_own = getenv("HRV_CONV_EPI_OWN");  // A-B knob
-  a.epi_own = (!pair && !pixn && p->epi == HRV_EPI_LINEAR && a.nacc >= kEpiC && !(env_own && env_own[0] == '0')) ? 1 : 0;
-  if (a.epi_own) a.nacc = (a.nacc / kEpiC) * kEpiC;
+  a.chunks = (in.c + 63) / 64;
+  a.n_gemm = p->n_gemm;
   a.epi = p->epi; a.act = p->act;
   a.scale = p->scale; a.shift = p->shift;
   a.out = out.ptr; a.out_pitch = out.pitch; a.out_dtype = out.dtype; a.out_layout = p->out_layout; a.out_c = out.c;
@@ -1378,115 +359,39 @@ extern "C" int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream) {
     return set_error(HRV_EINVAL, "conv: unknown epilogue %d", p->epi);
   }
 
-  // per-warpgroup SPADE constant tables of the pair kernel
-  a.epi_tab = (pair && p->epi == HRV_EPI_SPADE && a.C_mod <= kTabMaxC && (a.C_mod % 8) == 0) ? 1 : 0;
-  const uint32_t tab_bytes = a.epi_tab ? (((uint32_t)kEpiC * kTabBytes + 1023u) & ~1023u) : 0u;
-  // ---- pipeline geometry
+  // ---- pipeline: as many stages as fit in half of an SM's shared memory (two CTAs per SM), at most one per K step
+  const uint32_t stage_bytes = kABytes + (uint32_t)bnt * kRowBytes;
+  const int KT = p->kh * p->kw * a.chunks;
+  int stages = (int)((kSmemPerCta - 2048u) / stage_bytes);
+  if (stages > kMaxStages) stages = kMaxStages;
+  if (stages > KT) stages = KT < 2 ? 2 : KT;
+  a.stages = stages;
+  const size_t smem = 2048 + (size_t)stages * stage_bytes;  // 1 KB alignment slack + 1 KB of barriers
+
+  // ---- tensor maps
   const int elem = 2;
   const int taps = p->kh * p->kw;
-  const uint32_t row_bytes = p->bk * 2;
-  const uint32_t budget = 225u * 1024u - 3072u - tab_bytes;  // 1 KB alignment slack + 2 KB control block (+ constant tables)
-  const int LP = TW + p->kw - 1, HRows = (TH + p->kh - 1) * LP;
-  int tpb = 1;
-  if (halo) {
-    a.halo = 1;
-    a.line_pitch = LP;
-    a.a_stage_bytes_tx = (int)(HRows * row_bytes);
-    a.a_stage_bytes = (int)((HRows * row_bytes + 1023u) & ~1023u);
-    static const char* env_tpb = getenv("HRV_CONV_TPB_KB");
-    const uint32_t tpb_cap = (env_tpb ? (uint32_t)atoi(env_tpb) : 80u) * 1024u;
-    // halo ring: ~72 KB in flight (at least 3 stages), the rest of shared memory goes to the weight ring
-    int sa = (int)(72u * 1024u / (uint32_t)a.a_stage_bytes);
-    if (sa < 3) sa = 3;
-    if (sa > 16) sa = 16;
-    static const char* env_sa = getenv("HRV_CONV_SA");
-    if (env_sa) sa = atoi(env_sa);
-    // taps per weight TMA: the largest divisor of the tap count whose stage is <= tpb_cap and still leaves >= 3 weight stages
-    // (>= 2 as a last resort) next to the halo ring
-    const uint32_t b_rows = pair ? (uint32_t)p->bn / 2u : (uint32_t)p->bn;  // weight rows per tap in THIS CTA's shared memory
-    for (int want = 3; want >= 2 && tpb == 1; --want)
-      for (int d = taps; d >= 1; --d) {
-        const uint32_t bs = ((uint32_t)d * b_rows * row_bytes + 1023u) & ~1023u;
-        if (taps % d == 0 && (uint32_t)d * b_rows * row_bytes <= tpb_cap && (uint32_t)sa * a.a_stage_bytes + (uint32_t)want * bs <= budget) { tpb = d; break; }
-      }
-    a.tpb = tpb;
-    const char* env_grp = getenv("HRV_CONV_TAP_GROUP");  // A-B knob
-    a.tap_group = (p->kh == 3 && p->kw == 3 && a.line_pitch == 10 && (tpb == 9 || tpb == 3) && !(env_grp && env_grp[0] == '0')) ? tpb : 0;
-    a.b_stage_bytes = (int)(((uint32_t)tpb * b_rows * row_bytes + 1023u) & ~1023u);
-    while (sa > 2 && (uint32_t)sa * a.a_stage_bytes + 2u * a.b_stage_bytes > budget) --sa;
-    int sb = (int)((budget - (uint32_t)sa * a.a_stage_bytes) / (uint32_t)a.b_stage_bytes);
-    if (sb > kMaxStages) sb = kMaxStages;
-    if (sb < 2) return set_error(HRV_EINVAL, "conv: tile too large for shared memory (halo mode)");
-    a.stages = sa; a.sb_stages = sb;
-  } else {
-    a.tpb = 1;
-    const uint32_t stage_bytes = 128 * row_bytes + (((uint32_t)p->bn * row_bytes + 1023u) & ~1023u);
-    int stages = (int)(budget / stage_bytes);
-    if (stages > kMaxStages) stages = kMaxStages;
-    if (stages < 2) return set_error(HRV_EINVAL, "conv: tile too large for shared memory");
-    a.stages = stages; a.sb_stages = 0;
-  }
-  // ---- tensor maps
-  const CUtensorMapSwizzle sw = p->bk == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (p->bk == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
   {
     cuuint64_t dims[4] = {(cuuint64_t)in.c, (cuuint64_t)in.w, (cuuint64_t)in.h, (cuuint64_t)in.n};
     cuuint64_t strides[3] = {(cuuint64_t)in.pitch * elem, (cuuint64_t)in.w * in.pitch * elem, (cuuint64_t)in.h * in.w * in.pitch * elem};
-    cuuint32_t box[4] = {(cuuint32_t)p->bk, (cuuint32_t)(halo ? LP : TW), (cuuint32_t)(halo ? TH + p->kh - 1 : TH), (cuuint32_t)TN};
+    cuuint32_t box[4] = {64, (cuuint32_t)TW, (cuuint32_t)TH, (cuuint32_t)TN};
     cuuint32_t es[4] = {1, 1, 1, 1};
-    int rc = encode_tensor_map(&a.tmA, 4, in.ptr, dims, strides, box, es, sw);
+    int rc = encode_tensor_map(&a.tmA, 4, in.ptr, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
   {
-    // packed weights [taps][n_pad][cin_k]: a 3-D map lets one TMA fetch `tpb` taps of one (channel chunk, N tile)
-    const cuuint64_t cin_k = (cuuint64_t)a.chunks * p->bk, n_pad = (cuuint64_t)a.tiles_n * p->bn;
+    // packed weights [taps][n_pad][cin_k] as laid out by hrv_pack_conv_weight for this (bk, bn)
+    const cuuint64_t cin_k = (cuuint64_t)((in.c + p->bk - 1) / p->bk) * p->bk;
+    const cuuint64_t n_pad = (cuuint64_t)((p->n_gemm + p->bn - 1) / p->bn) * p->bn;
     cuuint64_t dims[3] = {cin_k, n_pad, (cuuint64_t)taps};
     cuuint64_t strides[2] = {cin_k * elem, n_pad * cin_k * elem};
-    cuuint32_t box[3] = {(cuuint32_t)p->bk, (cuuint32_t)(pixn ? 128 : (pair ? p->bn / 2 : p->bn)), (cuuint32_t)tpb};  // pixn: rows >= n_pad are zero fill; pair: half a tile per CTA
+    cuuint32_t box[3] = {64, (cuuint32_t)bnt, 1};
     cuuint32_t es[3] = {1, 1, 1};
-    int rc = encode_tensor_map(&a.tmB, 3, const_cast<void*>(p->wpack), dims, strides, box, es, sw);
+    int rc = encode_tensor_map(&a.tmB, 3, const_cast<void*>(p->wpack), dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  if (pixn) {
-    a.tiles_m = a.tiles_x * a.tiles_y * a.tiles_img;
-    a.pairs = (a.tiles_m + 1) / 2;
-    a.store_c = (out.c + 7) & ~7;
-    const uint32_t staging = (uint32_t)kEpiWG * 64u * (uint32_t)a.store_c * 2u;
-    int stages = (int)((budget - staging) / (48u * 1024u));
-    if (stages > 8) stages = 8;
-    if (stages < 2) return set_error(HRV_EINVAL, "conv(pixn): shared memory");
-    a.stages = stages;
-    const size_t smem_p = 3072 + (size_t)stages * 48 * 1024 + staging;
-    int gridp = sm_count();
-    if (a.pairs < gridp) gridp = a.pairs;
-    return launch_pixn(a, gridp, smem_p, st);
-  }
-  size_t smem = 3072 + tab_bytes + (halo ? (size_t)a.stages * a.a_stage_bytes + (size_t)a.sb_stages * a.b_stage_bytes
-                             : (size_t)a.stages * (128 * row_bytes + (((uint32_t)p->bn * row_bytes + 1023u) & ~1023u)));
-  if (smem < 120 * 1024) smem = 120 * 1024;  // force one CTA per SM (TMEM: up to 512 columns per CTA)
-
-  if (pair) {
-    static bool attr_done = false;
-    if (!attr_done) {
-      cudaError_t e = cudaFuncSetAttribute(conv_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
-      if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(conv_pair): %s", cudaGetErrorString(e));
-      attr_done = true;
-    }
-    const long long tiles_m = (long long)a.tiles_x * a.tiles_y * a.tiles_img;
-    const long long items = (long long)a.tiles_n * ((tiles_m + 1) / 2);
-    int clusters = sm_count() / 2;
-    if (items < clusters) clusters = (int)items;
-    conv_pair_kernel<<<2 * clusters, kThreadsC, smem, st>>>(a);  // __cluster_dims__(2,1,1): one pair per TPC
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_pair launch: %s", cudaGetErrorString(e));
-    return HRV_OK;
-  }
   const long long total = (long long)a.tiles_n * a.tiles_x * a.tiles_y * a.tiles_img;
-  int grid = sm_count();
-  if (total < grid) grid = (int)total;
-  switch (p->bk) {
-    case 64: return launch_conv<64>(a, grid, smem, st);
-    case 32: return launch_conv<32>(a, grid, smem, st);
-    default: return launch_conv<16>(a, grid, smem, st);
-  }
+  if (total > 0x7FFFFFFFLL) return set_error(HRV_EINVAL, "conv: too many tiles");
+  cudaStream_t st = (cudaStream_t)stream;
+  return bnt == 64 ? launch_conv<64>(a, (int)total, smem, st) : launch_conv<128>(a, (int)total, smem, st);
 }

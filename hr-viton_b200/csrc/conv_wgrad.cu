@@ -1,14 +1,13 @@
-// conv_wgrad.cu — convolution weight gradient on tcgen05:  dW[co,ci,ky,kx] += sum_{n,y,x} dY[n,y,x,co] * X[n,y+ky-pad,x+kx-pad,ci]
+// conv_wgrad.cu — convolution weight gradient on wgmma:  dW[co,ci,ky,kx] += sum_{n,y,x} dY[n,y,x,co] * X[n,y+ky-pad,x+kx-pad,ci]
 //
-// GEMM view per kernel row ky:  D_kx[co, ci] (M = 128 output channels, N = BN <= 128 input channels, one TMEM accumulator per kx),
-// K = pixels.  Both operands are channel-contiguous in NHWC memory, i.e. *MN-major* for the MMA (K = pixels is the strided index):
-// a TMA box {64 channels, PX pixels} lands as PX rows of 128 B (SWIZZLE_128B) = K-rows of a 64-wide MN block; blocks of 64 channels
-// sit LBO bytes apart, 8-row K atoms SBO = 1024 B apart (layout probed on B200: tools/umma_mnmajor_probe.cu).
-// The kx taps are *shifted views* of one X box of PX+KW-1 pixels (descriptor start + kx rows; absolute-address swizzle), so per
-// 64-pixel chunk one dY box and one X box feed KW*4 MMAs of 128 x BN x 16.
-// Grid = (co tiles) x (ci tiles) x KH x splits; each CTA streams its share of the (n, y, x-segment) chunks and finally writes its fp32
-// partial tile into slab `split` of the workspace [splits][cout][cin][KH][KW]; wgrad_reduce_kernel then sums the slabs in a FIXED
-// order into dW — the result is bit-reproducible run to run (round 1 accumulated with fp32 atomics, whose order is not).
+// GEMM view per tap (ky, kx):  D[co, ci] (M = 128 output channels over two consumer warpgroups, N = BN = 64 or 128 input channels,
+// fp32 accumulators in registers), K = pixels.  Both operands are channel-contiguous in NHWC memory, i.e. *MN-major* for the MMA
+// (K = pixels is the strided index): a TMA box {64 channels, PX pixels} lands as PX rows of 128 B (SWIZZLE_128B) = K-rows of a
+// 64-wide MN block; blocks of 64 channels sit LBO bytes apart, 8-row K groups SBO = 1024 B apart.
+// Grid = (co tiles) x (ci tiles) x KH x KW x splits; each CTA streams its share of the (n, y, x-segment) chunks (one dY box pair and
+// the X box shifted by its tap per chunk) and finally writes its fp32 partial tile into slab `split` of the workspace
+// [splits][cout][cin][KH][KW]; wgrad_reduce_kernel then sums the slabs in a FIXED order into dW — the result is bit-reproducible run
+// to run (fp32 atomics would not be).
 // Replaces the weight-gradient half of nn.Conv2d's backward (networks.py / network_generator.py convolutions, stage-2 training).
 #include <stdlib.h>
 
@@ -17,12 +16,13 @@
 
 namespace hrv {
 
-constexpr int kWgThreads = 192;  // warp 0: TMA producer, warp 1: MMA issuer (+TMEM alloc), warps 2-5: epilogue
+constexpr int kWgThreads = 288;  // warpgroups 0, 1: MMA + epilogue (64 output channels each), warp 8: TMA producer
 constexpr int kPX = 64;          // pixels (K) per pipeline stage
+constexpr uint32_t kWgSmem = 110u * 1024u;  // two CTAs per SM (plus 1 KB reserved per CTA)
 
 struct alignas(64) WgradArgs {
   CUtensorMap tmDY;  // dY (N,OH,OW,cout) box {64, kPX, 1, 1}
-  CUtensorMap tmX;   // X  (N,H,W,cin)    box {64, kPX+KW-1, 1, 1}
+  CUtensorMap tmX;   // X  (N,H,W,cin)    box {64, kPX, 1, 1}
   int Nimg, OH, OW, xsegs;
   int KH, KW, pad;
   int cout, cin, BN, stages, splits;
@@ -49,19 +49,14 @@ __global__ void __launch_bounds__(256) wgrad_reduce1_kernel(const float* __restr
   dw[i] = acc;
 }
 
-__global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_constant__ WgradArgs a) {
+template <int BN>
+__global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_constant__ WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   auto bar_full = [&](int s) { return base + 8u * s; };
   auto bar_empty = [&](int s) { return base + 128u + 8u * s; };
-  const uint32_t bar_done = base + 256u;
-  const uint32_t tmem_slot = base + 264u;
-  const uint32_t a_bytes = 2u * kPX * 128u;                                   // two 64-channel blocks of dY
-  const uint32_t bx_rows = (uint32_t)(kPX + a.KW - 1);
-  const uint32_t b_blk = (bx_rows * 128u + 1023u) & ~1023u;                   // one 64-channel block of X (1024-aligned TMA destination)
-  const uint32_t b_bytes = b_blk * (uint32_t)(a.BN / 64);
-  const uint32_t stage_bytes = a_bytes + b_bytes;
+  constexpr uint32_t kBlk = kPX * 128u;                                     // one 64-channel block of kPX pixel rows: 8 KB
+  constexpr uint32_t stage_bytes = kBlk * (2u + BN / 64);                  // dY: co blocks 0, 1; X: BN / 64 ci blocks
   const uint32_t stage0 = base + 1024u;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = a.stages;
@@ -69,123 +64,122 @@ __global__ void __launch_bounds__(kWgThreads, 1) conv_wgrad_kernel(const __grid_
   // tile coordinates
   int bid = blockIdx.x;
   const int split = bid % a.splits; bid /= a.splits;
+  const int kx = bid % a.KW; bid /= a.KW;
   const int ky = bid % a.KH; bid /= a.KH;
   const int nt = bid % a.n_tiles;
   const int mt = bid / a.n_tiles;
   const int m0 = mt * 128, n0 = nt * a.BN;
   const int chunks_total = a.Nimg * a.OH * a.xsegs;
   const int my_chunks = (chunks_total - split + a.splits - 1) / a.splits;  // chunks split, split+splits, ...
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)(a.KW * a.BN)) tmem_cols <<= 1;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&a.tmDY);
-    tma_prefetch_desc(&a.tmX);
-    for (int s = 0; s < S; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 1); }
-    mbar_init(bar_done, 1);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 8); }  // one arrival per consumer warp
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, tmem_cols); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
 
-  if (warp == 0) {
-    // ===================================================== TMA producer
-    int st = 0;
-    uint32_t ph = 0, sa = stage0;
-    int c = split;
-    for (int i = 0; i < my_chunks; ++i, c += a.splits) {
-      const int xs = c % a.xsegs;
-      int r = c / a.xsegs;
-      const int y = r % a.OH;
-      const int n = r / a.OH;
-      mbar_wait(bar_empty(st), ph ^ 1u);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(bar_full(st), a_bytes + bx_rows * 128u * (uint32_t)(a.BN / 64));
+  if (warp == 8) {
+    // ===================================================== TMA producer (one lane)
+    if (lane == 0) {
+      tma_prefetch_desc(&a.tmDY);
+      tma_prefetch_desc(&a.tmX);
+      int st = 0;
+      uint32_t ph = 0, sa = stage0;
+      int c = split;
+      for (int i = 0; i < my_chunks; ++i, c += a.splits) {
+        const int xs = c % a.xsegs;
+        int r = c / a.xsegs;
+        const int y = r % a.OH;
+        const int n = r / a.OH;
+        mbar_wait(bar_empty(st), ph ^ 1u);
+        mbar_arrive_expect_tx(bar_full(st), stage_bytes);
         tma_load_4d(sa, &a.tmDY, bar_full(st), m0, xs * kPX, y, n);
-        tma_load_4d(sa + kPX * 128u, &a.tmDY, bar_full(st), m0 + 64, xs * kPX, y, n);
-        for (int b = 0; b < a.BN / 64; ++b)
-          tma_load_4d(sa + a_bytes + b * b_blk, &a.tmX, bar_full(st), n0 + 64 * b, xs * kPX - a.pad, y + ky - a.pad, n);
+        tma_load_4d(sa + kBlk, &a.tmDY, bar_full(st), m0 + 64, xs * kPX, y, n);
+        for (int b = 0; b < BN / 64; ++b)
+          tma_load_4d(sa + (2u + b) * kBlk, &a.tmX, bar_full(st), n0 + 64 * b, xs * kPX - a.pad + kx, y + ky - a.pad, n);
+        sa += stage_bytes;
+        if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
       }
-      __syncwarp();
-      sa += stage_bytes;
-      if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
     }
-  } else if (warp == 1) {
-    // ===================================================== MMA issuer
-    const uint32_t idesc = make_idesc_bf16(128, (uint32_t)a.BN, 1, 1);  // A and B are MN-major
-    const uint64_t da_hi = make_smem_desc(0, 1024, 2, kPX * 128u);      // LBO = 64-channel block stride of dY
-    const uint64_t db_hi = make_smem_desc(0, 1024, 2, b_blk);           // LBO = 64-channel block stride of X
-    int st = 0;
+    return;
+  }
+
+  // ===================================================== consumers: warpgroup wg owns output channels m0 + [64 wg, 64 wg + 64)
+  // Both operands are MN-major (channels contiguous, K = pixels strided): LBO = 64-channel block stride, SBO = 8 pixel rows.
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    int st = 0, prev = 0;
     uint32_t ph = 0, sa = stage0;
     for (int i = 0; i < my_chunks; ++i) {
       mbar_wait(bar_full(st), ph);
-      tc_fence_after();
-      const uint32_t sb = sa + a_bytes;
-      if (elect_one()) {
-        for (int kx = 0; kx < a.KW; ++kx) {
-          const uint32_t d_tmem = tmem_base + (uint32_t)(kx * a.BN);
+      wgmma_fence();
+      const uint32_t sdy = sa + (uint32_t)wg * kBlk, sx = sa + 2u * kBlk;
 #pragma unroll
-          for (int kk = 0; kk < kPX / 16; ++kk) {
-            const uint64_t da = da_hi | (uint64_t)(((sa + kk * 2048u) & 0x3FFFFu) >> 4);
-            const uint64_t db = db_hi | (uint64_t)(((sb + (uint32_t)(kk * 16 + kx) * 128u) & 0x3FFFFu) >> 4);
-            umma_f16(d_tmem, da, db, idesc, (uint32_t)((i | kk) != 0));
-          }
-        }
-        umma_commit(bar_empty(st));
+      for (int kk = 0; kk < kPX / 16; ++kk) {  // 16 pixel rows per instruction
+        const uint64_t da = make_wgmma_desc(sdy + kk * 2048u, 1024, 1, kBlk);
+        const uint64_t db = make_wgmma_desc(sx + kk * 2048u, 1024, 1, kBlk);
+        const uint32_t accf = (uint32_t)((i | kk) != 0);
+        if constexpr (BN == 128) wgmma_n128<1, 1>(acc, da, db, accf);
+        else wgmma_n64<1, 1>(acc, da, db, accf);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (i > 0 && lane == 0) mbar_arrive(bar_empty(prev));
+      prev = st;
       sa += stage_bytes;
       if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
     }
-    if (elect_one()) umma_commit(bar_done);
-    __syncwarp();
-  } else {
-    // ===================================================== epilogue: fp32 partial tile -> red.add into dW[(co*cin+ci)*KH*KW + ky*KW + kx]
-    const int q = warp & 3;  // warps 2,3,4,5 -> TMEM lane quarters 2,3,0,1
-    const int co = m0 + q * 32 + lane;
-    float* const slab = a.dw + (long long)split * a.cout * a.cin * a.KH * a.KW;  // this CTA's private slab: plain stores, no atomics
-    if (my_chunks > 0) {
-      mbar_wait(bar_done, 0);
-      tc_fence_after();
-      for (int kx = 0; kx < a.KW; ++kx) {
-        for (int col = 0; col < a.BN; col += 16) {
-          uint32_t v[16];
-          __syncwarp();
-          tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(kx * a.BN + col), v);
-          tmem_wait_ld();
-          if (co < a.cout) {
+    wgmma_wait<0>();
+    fence_regs(acc);
+  }
+
+  // ===================================================== epilogue: fp32 partial tile -> dW[(co*cin+ci)*KH*KW + ky*KW + kx] of this split's slab
+  // wgmma fragment: thread (warp w, lane l) holds rows (co) 16 (w % 4) + l / 4 and that + 8, columns (ci) 8 j + 2 (l % 4) + {0, 1}.
+  float* const slab = a.dw + (long long)split * a.cout * a.cin * a.KH * a.KW;  // this CTA's private slab: plain stores, no atomics
+  const int co_base = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int ci_base = n0 + 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const int ci = n0 + col + j;
-              if (ci < a.cin) slab[(((long long)co * a.cin + ci) * a.KH + ky) * a.KW + kx] = __uint_as_float(v[j]);
-            }
-          }
-        }
+  for (int h = 0; h < 2; ++h) {
+    const int co = co_base + 8 * h;
+    if (co >= a.cout) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int ci = ci_base + 8 * j + e;
+        // a split without work (more splits than chunks) writes zeros: acc was never touched
+        if (ci < a.cin) slab[(((long long)co * a.cin + ci) * a.KH + ky) * a.KW + kx] = acc[4 * j + 2 * h + e];
       }
-    } else if (co < a.cout) {  // a split without work (more splits than chunks): its slab entries are zeros
-      for (int kx = 0; kx < a.KW; ++kx)
-        for (int ci = n0; ci < n0 + a.BN && ci < a.cin; ++ci) slab[(((long long)co * a.cin + ci) * a.KH + ky) * a.KW + kx] = 0.f;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, tmem_cols); }
+}
+
+template <int BN>
+static cudaError_t launch_wgrad(const WgradArgs& a, int grid, size_t smem, cudaStream_t st) {
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmem);
+    if (e != cudaSuccess) return e;
+    attr_done = true;
+  }
+  conv_wgrad_kernel<BN><<<grid, kWgThreads, smem, st>>>(a);
+  return cudaGetLastError();
 }
 
 }  // namespace hrv
 
 using namespace hrv;
 
-// Split-K factor: one CTA per SM is resident (512 TMEM columns each), CTAs of one launch take equal time, so the launch costs
-// waves * (chunks per CTA + fixed prologue/epilogue) with waves = ceil(grid / SMs).  Pick the split that minimises it — a grid
-// that spills a few CTAs into an extra wave (e.g. 300 CTAs on 148 SMs) costs a whole wave.
+// Split-K factor: two CTAs per SM are resident, CTAs of one launch take equal time, so the launch costs
+// waves * (chunks per CTA + fixed prologue/epilogue) with waves = ceil(grid / (2 SMs)).  Pick the split that minimises it — a grid
+// that spills a few CTAs into an extra wave (e.g. 270 CTAs on 2 x 132 slots) costs a whole wave.
 static int wgrad_splits(int tiles, int chunks) {
-  const int sms = sm_count();
+  const int sms = 2 * sm_count();
   int splits = 1;
-  const long long kFixed = 16;  // prologue + TMEM read-out + epilogue, in units of one 64-pixel chunk step
+  const long long kFixed = 16;  // prologue + epilogue, in units of one 64-pixel chunk step
   long long best = -1;
   int smax = 8 * sms / tiles + 1;
   if (smax > chunks) smax = chunks;
@@ -199,18 +193,18 @@ static int wgrad_splits(int tiles, int chunks) {
   if (env && atoi(env) > 0) splits = atoi(env) < chunks ? atoi(env) : (chunks > 0 ? chunks : 1);
   return splits;
 }
-static void wgrad_geometry(const hrv_tensor* x, const hrv_tensor* dy, int kh, int* tiles, int* chunks, int* bn, int* m_tiles, int* n_tiles) {
+static void wgrad_geometry(const hrv_tensor* x, const hrv_tensor* dy, int kh, int kw, int* tiles, int* chunks, int* bn, int* m_tiles, int* n_tiles) {
   *bn = x->c <= 64 ? 64 : 128;
   *m_tiles = (dy->c + 127) / 128;
   *n_tiles = (x->c + *bn - 1) / *bn;
   *chunks = x->n * dy->h * ((dy->w + kPX - 1) / kPX);
-  *tiles = *m_tiles * *n_tiles * kh;
+  *tiles = *m_tiles * *n_tiles * kh * kw;
 }
 
 extern "C" size_t hrv_conv2d_wgrad_workspace_bytes(const hrv_tensor* x, const hrv_tensor* dy, int32_t kh, int32_t kw) {
   if (!x || !dy || kh < 1 || kw < 1) return 0;
   int tiles, chunks, bn, mt, nt;
-  wgrad_geometry(x, dy, kh, &tiles, &chunks, &bn, &mt, &nt);
+  wgrad_geometry(x, dy, kh, kw, &tiles, &chunks, &bn, &mt, &nt);
   const int splits = wgrad_splits(tiles, chunks);
   return splits > 1 ? (size_t)splits * dy->c * x->c * kh * kw * sizeof(float) : 0;
 }
@@ -228,7 +222,7 @@ extern "C" int hrv_conv2d_wgrad(const hrv_tensor* x, const hrv_tensor* dy, int32
   a.Nimg = x->n; a.OH = dy->h; a.OW = dy->w; a.xsegs = (dy->w + kPX - 1) / kPX;
   a.KH = kh; a.KW = kw; a.pad = pad; a.cout = dy->c; a.cin = x->c;
   int tiles, chunks;
-  wgrad_geometry(x, dy, kh, &tiles, &chunks, &a.BN, &a.m_tiles, &a.n_tiles);
+  wgrad_geometry(x, dy, kh, kw, &tiles, &chunks, &a.BN, &a.m_tiles, &a.n_tiles);
   const int splits = wgrad_splits(tiles, chunks);
   const long long dw_elems = (long long)dy->c * x->c * kh * kw;
   if (splits > 1) {
@@ -240,8 +234,8 @@ extern "C" int hrv_conv2d_wgrad(const hrv_tensor* x, const hrv_tensor* dy, int32
     a.dw = dw;                 // one CTA per output element: plain stores straight into dw
   }
   a.splits = splits;
-  const uint32_t stage_bytes = 2u * kPX * 128u + ((((uint32_t)(kPX + kw - 1) * 128u + 1023u) & ~1023u) * (uint32_t)(a.BN / 64));
-  int stages = (int)((200u * 1024u) / stage_bytes);
+  const uint32_t stage_bytes = kPX * 128u * (2u + (uint32_t)(a.BN / 64));
+  int stages = (int)((kWgSmem - 2048u) / stage_bytes);
   if (stages > 16) stages = 16;
   a.stages = stages;
   {
@@ -255,22 +249,14 @@ extern "C" int hrv_conv2d_wgrad(const hrv_tensor* x, const hrv_tensor* dy, int32
   {
     cuuint64_t dims[4] = {(cuuint64_t)x->c, (cuuint64_t)x->w, (cuuint64_t)x->h, (cuuint64_t)x->n};
     cuuint64_t strides[3] = {(cuuint64_t)x->pitch * 2, (cuuint64_t)x->w * x->pitch * 2, (cuuint64_t)x->h * x->w * x->pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)(kPX + kw - 1), 1, 1};
+    cuuint32_t box[4] = {64, (cuuint32_t)kPX, 1, 1};
     cuuint32_t es[4] = {1, 1, 1, 1};
     int rc = encode_tensor_map(&a.tmX, 4, x->ptr, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 232448);
-    if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(conv_wgrad): %s", cudaGetErrorString(e));
-    attr_done = true;
-  }
-  size_t smem = 2048 + (size_t)stages * stage_bytes;
-  if (smem < 120 * 1024) smem = 120 * 1024;  // one CTA per SM: each allocates up to 512 TMEM columns
+  const size_t smem = 2048 + (size_t)stages * stage_bytes;
   const int grid = tiles * splits;
-  conv_wgrad_kernel<<<grid, kWgThreads, smem, (cudaStream_t)stream>>>(a);
-  cudaError_t e = cudaGetLastError();
+  cudaError_t e = a.BN == 128 ? launch_wgrad<128>(a, grid, smem, (cudaStream_t)stream) : launch_wgrad<64>(a, grid, smem, (cudaStream_t)stream);
   if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_wgrad launch: %s", cudaGetErrorString(e));
   if (splits > 1) {
     if ((dw_elems % 4) || ((uintptr_t)dw & 15)) {  // slabs not 16-byte aligned: scalar reduction (tiny layers, e.g. 13 -> 13 channels)

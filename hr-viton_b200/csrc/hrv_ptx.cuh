@@ -1,5 +1,4 @@
-// hrv_ptx.cuh — thin inline-PTX wrappers for sm_100a: mbarrier, TMA, tcgen05 (MMA / TMEM / commit).
-// Constants cross-checked against cute/arch/mma_sm100_desc.hpp (InstrDescriptor / SmemDescriptor bit layout).
+// hrv_ptx.cuh — thin inline-PTX wrappers for sm_90a: mbarrier, TMA, wgmma.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -7,7 +6,7 @@
 #include <stdint.h>
 #ifdef HRV_F16
 // fp16-storage flavour: the kernel sources are written against the bf16 names; this build maps them onto IEEE half.  Everything
-// between HBM and the fp32 registers (unpack/pack helpers, tcgen05 operand format) follows; TMA moves 2-byte elements either way.
+// between HBM and the fp32 registers (unpack/pack helpers, wgmma operand format) follows; TMA moves 2-byte elements either way.
 #include <cuda_fp16.h>
 #define __nv_bfloat16 __half
 #define __nv_bfloat162 __half2
@@ -21,7 +20,7 @@ namespace hrv {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // One lane of a fully converged warp (warp-uniform control flow lets the compiler keep descriptors in uniform
-// registers and issue UTMALDG / UTCHMMA directly instead of wrapping each in a per-thread election loop).
+// registers and issue UTMALDG directly instead of wrapping it in a per-thread election loop).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -83,125 +82,53 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
       : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16 inputs with fp32 accumulation.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on the mbarrier once every previously issued tcgen05.mma of this thread has completed.
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// 32 lanes x 16 consecutive 32-bit columns -> 16 registers per thread (thread i <-> lane base+i).
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Instruction descriptor, kind::f16: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1), both K-major
-// (bits 15,16 = 0) unless a_mn/b_mn, N>>3 at bits 17-22, M>>4 at bits 24-28.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn = 0, uint32_t b_mn = 0) {
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+// D[registers of one warpgroup, 64 x N fp32] (+)= A[smem desc, 64 x 16] * B[smem desc, N x 16].  TA / TB = 1: that operand is
+// MN-major in shared memory (only 16-bit operand types may be transposed).
 #ifdef HRV_F16
-  return (1u << 4) | (0u << 7) | (0u << 10) |  // A = B = f16 (format code 0)
+#define HRV_WGMMA_T "f16"
 #else
-  return (1u << 4) | (1u << 7) | (1u << 10) |
+#define HRV_WGMMA_T "bf16"
 #endif
-         (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// Shared-memory matrix descriptor (K-major, swizzled): start>>4 at bits 0-13, LBO>>4 at 16-29 (unused for
-// swizzled K-major when the MMA K extent fits one swizzle row: 1), SBO>>4 at 32-45 (= 8 rows * row bytes),
-// version=1 at bits 46-47, layout type at bits 61-63 (2=SW128, 4=SW64, 6=SW32).
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type, uint32_t lbo_bytes = 16) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)layout_type << 61);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accumulator reads/writes across an asynchronous wgmma.
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---------------------------------------------------------------- CTA pairs (cta_group::2, thread-block cluster of 2)
-// Two CTAs on the two SMs of a TPC execute ONE tcgen05.mma of M = 256: each contributes its 128 rows of A and HALF of the B tile
-// from its own shared memory and keeps its own 128 x N accumulator in its own TMEM.  Per CTA that halves the shared-memory bytes
-// of B written by TMA and read by the tensor core — the resource that bounds the one-CTA kernel (DESIGN.md, conv roofline).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // shared::cluster address -> the same offset in CTA rank 0 of the pair
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctaid_x() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA loads of a CTA pair: data lands in THIS CTA's shared memory, the transaction bytes are signalled on the LEADER's mbarrier
-// (`bar` = this CTA's address of the barrier; the peer bit is cleared here).
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_2sm(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// D[tmem, both CTAs] (+)= A * B with M = 256 over the pair; issued by ONE thread of the leader CTA.
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." HRV_WGMMA_T "." HRV_WGMMA_T " "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// Arrives on the mbarrier at this shared-memory offset in BOTH CTAs of the pair once the MMAs issued so far have completed.
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3)
-               : "memory");
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." HRV_WGMMA_T "." HRV_WGMMA_T " "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
-// Plain arrive on the LEADER's copy of a barrier (from either CTA of the pair).
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar & kPeerBitMask) : "memory");
+
+// Shared-memory matrix descriptor of sm_90a: start>>4 at bits 0-13, LBO>>4 at 16-29, SBO>>4 at 32-45, layout type at bits 62-63
+// (1 = SW128, 2 = SW64, 3 = SW32).  K-major swizzled: SBO = stride of 8-row core-matrix groups, LBO unused (1).  MN-major swizzled:
+// LBO = stride of 64-element MN blocks, SBO = stride of 8-row K groups.  Operands start on 1024-byte boundaries (swizzle phase 0).
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type, uint32_t lbo_bytes = 16) {
+  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
+         ((uint64_t)layout_type << 62);
 }
 
 // ---------------------------------------------------------------- misc

@@ -155,9 +155,8 @@ def pick_bn(n_gemm):
 
 
 def pick_bn_spade(n_gemm):
-    """N tile of a gamma|beta GEMM (n_gemm = 2C interleaved columns).  With several N tiles the staged epilogue of the CTA-pair kernel
-    needs each tile's channel range to end on a 16-channel slab, i.e. bn % 32 == 0: take the candidate with the fewest padded columns
-    (ties: the wider tile)."""
+    """N tile of a gamma|beta GEMM (n_gemm = 2C interleaved columns): with several N tiles each tile's channel range ends on a
+    16-channel slab (bn % 32 == 0); take the candidate with the fewest padded columns (ties: the wider tile)."""
     n16 = round_up(n_gemm, 16)
     if n16 <= 256:
         return n16
@@ -199,7 +198,7 @@ def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixe
     inter = 2 if interleave is not None else 1
     rows, cols = (cin, cout * inter) if dgrad else (cout * inter, cin)  # GEMM N rows, K columns
     k_eff = cols if cin_total is None else cin_total
-    # Cout <= 128: eligible for the pixel-N kernel (conv_pixn_kernel), which needs 64-channel K blocks (zero padded)
+    # Cout <= 128 with more than 32 input channels: 64-channel K blocks (zero padded), the convolution kernel's own block size
     bk = 64 if (rows <= 128 and k_eff > 32) else pick_bk(k_eff)  # K <= 32 stays on the 32-wide blocks (padding to 64 would double the MMAs)
     cin_k = round_up(k_eff, bk)
     if bn is None:
@@ -599,7 +598,7 @@ def act_bwd_bias(dy, y, act, want_dv=True, want_bias=True):
 
 
 def conv2d_wgrad(x, dy, kh, kw, pad):
-    """dW (cout,cin,kh,kw) fp32 of a stride-1 convolution, on tcgen05 (hrv_conv2d_wgrad)."""
+    """dW (cout,cin,kh,kw) fp32 of a stride-1 convolution, on wgmma (hrv_conv2d_wgrad)."""
     dw = torch.empty((dy.c, x.c, kh, kw), dtype=torch.float32, device=x.buf.device)
     tx, tdy = x.ct(), dy.ct()
     L = _L(x)

@@ -17,7 +17,7 @@ from .ops import ACT_LRELU, ACT_NONE, ACT_RELU, ACT_TANH, Act
 
 def _need_cuda(t, who):
     if not t.is_cuda:
-        raise RuntimeError("%s: hrviton_b200 runs on sm_100a only — got a CPU tensor (there is no CPU fallback)" % who)
+        raise RuntimeError("%s: hrviton_b200 runs on sm_90a only — got a CPU tensor (there is no CPU fallback)" % who)
 
 
 def _param_key(module):
@@ -193,7 +193,7 @@ class SPADEResBlock(nn.Module):
             wsh = torch.cat([m.conv_shared[0].weight.detach() for m in norms], 0)
             if 9 * wsh.shape[1] <= 64:
                 # few-channel label map: column (im2col) form, one K=64 block instead of nine K=16 taps; one 128-channel GEMM per
-                # norm (<= 128 output channels keeps each on the pixel-N kernel) writing its slice of the shared actv buffer
+                # norm writing its slice of the shared actv buffer
                 from .autograd_g import im2col_weight
                 shared = [ops.pack_weight(im2col_weight(m.conv_shared[0].weight.detach(), 64), (0, 0),
                                           flops_per_pixel=2.0 * m.conv_shared[0].weight.shape[0] * wsh.shape[1] * 9) for m in norms]

@@ -1,7 +1,7 @@
 """Environment for running the reference scripts unchanged against this repository's drop-in modules (see shims/README.md).
 
     import hrv_env; hrv_env.install()          # repo root first on sys.path, shims/ last, numpy aliases restored
-    hrv_env.load_reference_script("train_generator")   # imports baseline/_ref/train_generator.py (or /root/reference/...) with
+    hrv_env.load_reference_script("train_generator")   # imports oracle/_ref/train_generator.py with
                                                         # `networks`, `network_generator`, `sync_batchnorm` bound to the drop-ins
 """
 import importlib.util
@@ -38,10 +38,9 @@ def install():
 
 
 def reference_dir():
-    for d in (os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
-        if os.path.exists(os.path.join(d, "train_generator.py")):
-            return d
-    return None
+    """The reference copy that __graft_entry__.build() places under oracle/_ref (oracle/install_reference.py), or None."""
+    d = os.path.join(ROOT, "oracle", "_ref")
+    return d if os.path.exists(os.path.join(d, "train_generator.py")) else None
 
 
 def load_reference_script(name, alias=None):
@@ -50,7 +49,7 @@ def load_reference_script(name, alias=None):
     install()
     d = reference_dir()
     if d is None:
-        raise FileNotFoundError("no reference checkout (baseline/_ref or /root/reference)")
+        raise FileNotFoundError("no reference copy (oracle/_ref)")
     import network_generator  # noqa: F401  (bind the drop-ins before the reference directory becomes importable)
     import networks  # noqa: F401
     import sync_batchnorm  # noqa: F401

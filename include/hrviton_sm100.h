@@ -1,4 +1,4 @@
-/* hrviton_sm100.h — C-ABI of libhrviton_sm100.so (B200 / sm_100a only).
+/* hrviton_sm100.h — C-ABI of libhrviton_sm100.so (H100 / sm_90a only).
  *
  * The reference (sangyun884/HR-VITON) has no FFI layer: its seam is the Python module surface of
  * networks.py / network_generator.py, whose arithmetic is delegated to ATen/cuDNN ops.  Each entry
@@ -13,7 +13,7 @@
  *
  * Storage flavours: every entry point below exists twice in the library — hrv_<op> keeps activations and packed weights in
  * bf16 (the training configuration), hrv_<op>_f16 (include/hrviton_sm100_f16.h, generated from this file) keeps them in IEEE
- * fp16: same signatures, same kernels compiled against the other 16-bit type, tcgen05 operand format f16 instead of bf16.
+ * fp16: same signatures, same kernels compiled against the other 16-bit type, wgmma operand format f16 instead of bf16.
  * fp32 buffers (flows, logits, images, statistics, weight gradients) are identical in both.  Wherever a comment says "bf16" read
  * "the flavour's 16-bit storage type"; hrv_dtype code 0 denotes it.
  */
@@ -45,7 +45,7 @@ typedef struct hrv_tensor {
   int32_t dtype; /* hrv_dtype */
 } hrv_tensor;
 
-/* One 2-D convolution as an implicit GEMM on tcgen05 tensor cores (bf16 in, fp32 accumulate in TMEM).
+/* One 2-D convolution as an implicit GEMM on wgmma tensor cores (bf16 in, fp32 accumulate in registers).
  * Replaces nn.Conv2d forward at networks.py:60-93,178-192 ; network_generator.py:97-99,132-135,184-201,
  * 263-272 and, with HRV_EPI_SPADE, the whole SPADENorm tail `normalized*(1+gamma)+beta` + LeakyReLU
  * (network_generator.py:115-121,170-171) fused into the gamma/beta convolution.
@@ -64,9 +64,8 @@ typedef struct hrv_tensor {
  *                   x0 may be half resolution (x0_shift=1: nearest x2 up-sampling folded into the index,
  *                   network_generator.py:203,226-242); x1 supplies channels [x0.c, x0.c+x1.c) (the torch.cat).
  *
- * Kernel selection (same results bit for bit within one K order): LINEAR, bk = 64, n_gemm <= 128, bf16 NHWC output, no residual and
- * in.c > 32 run on the pixel-N kernel (weights as the MMA's M operand, 256 pixels as N); everything else on the classic kernel
- * (pixels as M), tap-by-tap or halo mainloop.  Environment switches for A/B runs, read per call: HRV_CONV_PIXN=0, HRV_CONV_HALO=0|1.
+ * One kernel (pixels as M, 64 or 128 output channels as N, K walked tap by tap in 64-channel blocks) runs every case; results are
+ * bit-identical from launch to launch.
  */
 typedef struct hrv_conv_params {
   hrv_tensor in;
@@ -143,7 +142,7 @@ int hrv_norm_bwd_apply(const hrv_tensor* dxn, const hrv_tensor* src, int32_t shi
                        int32_t W, const float* noise, const float* noise_scale, const float* mean, const float* rstd,
                        const float* m1, const float* m2, const hrv_tensor* dx, double* dns, hrv_stream stream);
 
-/* Convolution weight gradient on tcgen05: dw[co][ci][ky][kx] = sum_{n,y,x} dy[n,y,x,co] * x[n,y+ky-pad,x+kx-pad,ci]
+/* Convolution weight gradient on wgmma: dw[co][ci][ky][kx] = sum_{n,y,x} dy[n,y,x,co] * x[n,y+ky-pad,x+kx-pad,ci]
  * (stride 1; x: (n,h,w,cin), dy: (n,h+2pad-kh+1, w+2pad-kw+1, cout), both bf16 NHWC; kw <= 4). dw is fp32 in the reference's
  * parameter layout (cout,cin,kh,kw) and is OVERWRITTEN.  The pixel (K) dimension is split over CTAs; each writes its partial tile
  * into its own slab of `workspace` and a second kernel adds the slabs in a fixed order: the result is bit-reproducible run to run.

@@ -1,5 +1,5 @@
 """Drop-in for the reference's network_generator.py (network_generator.py:9-433): same public names, constructor /
-forward signatures and state_dict keys, backed by the sm_100a kernels of hrviton_b200."""
+forward signatures and state_dict keys, backed by the sm_90a kernels of hrviton_b200."""
 import hrv_loader
 
 hrv_loader.load()

@@ -1,5 +1,5 @@
 """Drop-in for the reference's networks.py (same public names, constructor / forward signatures and state_dict
-keys — networks.py:13-453) backed by the sm_100a kernels of hrviton_b200.  Put this repository first on
+keys — networks.py:13-453) backed by the sm_90a kernels of hrviton_b200.  Put this repository first on
 sys.path (or run the reference scripts from here) and `from networks import ConditionGenerator, ...` binds to it.
 """
 import os
@@ -58,7 +58,7 @@ class VGGLoss(nn.Module):
         self.layids = layids
 
     def forward(self, x, y):
-        if x.is_cuda and self.layids is None:  # sm_100a conv kernels (forward + dgrad); frozen weights need no wgrad
+        if x.is_cuda and self.layids is None:  # sm_90a conv kernels (forward + dgrad); frozen weights need no wgrad
             from hrviton_b200 import autograd_g
             return autograd_g.vgg_loss(self.vgg, self.weights, x, y)
         fx, fy = self.vgg(x), self.vgg(y)

@@ -23,7 +23,7 @@ class GaussianBlur(nn.Module):
             import hrv_loader
             hrv_loader.load()
             from hrviton_b200 import ops
-            return ops.gaussian_blur(x, kh, sy)  # hrv_gaussian_blur (sm_100a kernel)
+            return ops.gaussian_blur(x, kh, sy)  # hrv_gaussian_blur (sm_90a kernel)
         c = x.shape[1]
         gx, gy = _taps(kw, sx, x.device).to(x.dtype), _taps(kh, sy, x.device).to(x.dtype)
         x = F.conv2d(x, gx.view(1, 1, 1, kw).expand(c, 1, 1, kw), padding=(0, kw // 2), groups=c)

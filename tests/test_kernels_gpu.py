@@ -83,7 +83,7 @@ CONV_CASES = [
     (2, 96, 96, 32, 24, 3, 1, dict(act=1, scale=True, res=True)),
     (1, 32, 3, 64, 48, 3, 1, dict(act=3, out_fp32_nchw=True)),
     (1, 768, 2, 16, 12, 3, 1, dict(out_fp32_nchw=True)),
-    (2, 128, 160, 256, 192, 3, 1, dict(act=2)),  # 768 tiles: persistent loop, phase wrap, TMEM double buffering
+    (2, 128, 160, 256, 192, 3, 1, dict(act=2)),  # 768 tiles: many waves, pipeline phase wrap
     (1, 144, 64, 128, 96, 3, 1, {}),
 ]
 
@@ -397,8 +397,8 @@ PIXN_CASES = [  # n, cin, cout, h, w, k, pad, act, bias, scale, out_pitch
 
 @pytest.mark.parametrize("case", PIXN_CASES)
 def test_conv_pixn_matches_classic_kernel(case):
-    """The pixel-N kernel (weights as the MMA's M operand, 256 pixels as N, transposed epilogue) accumulates the same products in
-    the same K order as the classic kernel: outputs must be bit-identical.  HRV_CONV_PIXN=0 selects the classic kernel."""
+    """Narrow convolutions (Cout <= 128, 64-channel K blocks, every activation, bias / scale, padded output pitch): two launches on
+    identical inputs are bit-identical, and the result matches torch's convolution of the bf16-rounded operands."""
     n, cin, cout, h, w, k, pad, act, bias, scale, out_pitch = case
     x = Act(_to_buf(bf16r(synth.normalish((n, cin, h, w), 11, "x"))), c=cin)
     wt = synth.normalish((cout, cin, k, k), 11, "w", (1.0 / (cin * k * k)) ** 0.5).to(DEV)
@@ -408,17 +408,11 @@ def test_conv_pixn_matches_classic_kernel(case):
     assert pw.bk == 64
     oh, ow = h + 2 * pad - k + 1, w + 2 * pad - k + 1
     outs = []
-    try:
-        os.environ["HRV_CONV_HALO"] = "0"  # classic kernel in tap-by-tap order: the same fp32 accumulation order as the pixel-N kernel
-        for flag in ("0", "1"):
-            os.environ["HRV_CONV_PIXN"] = flag
-            o = Act(torch.zeros((n, oh, ow, out_pitch or ops.round_up(cout, 8)), dtype=torch.bfloat16, device=DEV), c=cout)
-            ops.conv2d(x, pw, o, act=act, scale=sc, shift=b)
-            torch.cuda.synchronize()
-            outs.append(o.buf.clone())
-    finally:
-        os.environ.pop("HRV_CONV_PIXN", None)
-        os.environ.pop("HRV_CONV_HALO", None)
+    for _ in range(2):
+        o = Act(torch.zeros((n, oh, ow, out_pitch or ops.round_up(cout, 8)), dtype=torch.bfloat16, device=DEV), c=cout)
+        ops.conv2d(x, pw, o, act=act, scale=sc, shift=b)
+        torch.cuda.synchronize()
+        outs.append(o.buf.clone())
     bad = outs[0] != outs[1]
     assert not bool(bad.any()), "%d mismatching elements, first at %s" % (int(bad.sum()), bad.nonzero()[:4].tolist())
     ref = F.conv2d(x.buf[..., :cin].permute(0, 3, 1, 2).float().cpu(), bf16r(wt.cpu()), None, padding=pad)
@@ -517,64 +511,58 @@ def test_conv_wgrad_is_bit_reproducible():
         assert rel_err(a, ref) < 2e-3
 
 
-PAIR_CASES = [  # spade, cin, n_gemm, h, w, batch, x0_shift, c1 (x1 channels)
+WIDE_CASES = [  # spade, cin, n_gemm, h, w, batch, x0_shift, c1 (x1 channels)
     (True, 128, 160, 64, 48, 2, 0, 0), (True, 128, 160, 64, 48, 2, 1, 16), (True, 128, 288, 48, 32, 3, 1, 16),
-    (True, 128, 544, 64, 48, 2, 1, 16),    # bn 192: two TMEM accumulators, two owner warpgroups
-    (True, 128, 2080, 16, 12, 2, 1, 16),   # 13 N tiles, more channels than the shared-memory constant table holds (global-load path)
-    (True, 128, 144, 30, 22, 1, 0, 0),     # odd number of pixel tiles: the pair's second CTA runs a tile past the end
+    (True, 128, 544, 64, 48, 2, 1, 16),    # five 128-column N tiles, the last one partly past n_gemm
+    (True, 128, 2080, 16, 12, 2, 1, 16),   # 17 N tiles over 1040 SPADE channels
+    (True, 128, 144, 30, 22, 1, 0, 0),     # pixel tiles past the image edge
     (False, 160, 160, 50, 37, 3, 0, 0), (False, 256, 256, 64, 48, 2, 0, 0), (False, 80, 192, 128, 96, 1, 0, 0),
-    # narrow tiles (32 / 64 / 128 columns: 16 / 32 / 64 weight rows per CTA)
+    # narrow tiles (32 / 64 / 128 columns)
     (True, 128, 64, 64, 48, 2, 1, 16), (True, 128, 128, 48, 32, 2, 0, 0), (False, 80, 32, 64, 48, 2, 0, 0), (False, 144, 64, 50, 37, 2, 0, 0),
     (False, 160, 128, 64, 48, 1, 0, 0), (False, 2080, 128, 16, 12, 2, 0, 0)]
 
 
-@pytest.mark.parametrize("case", PAIR_CASES)
-def test_conv_pair_kernel_matches_single_cta_kernel(case):
-    """The CTA-pair kernel (tcgen05 cta_group::2: M = 256 over two SMs, each CTA holding half of every weight stage; epilogue
-    warpgroup w drains accumulator w) against the one-CTA kernel on identical inputs (HRV_CONV_PAIR=0).  Same products, and — when the
-    one-CTA kernel also runs its halo mainloop (tiles of <= 32 or 144..208 columns) — the same fp32 accumulation order: bit-identical
-    outputs, gamma included.  Elsewhere the one-CTA kernel walks K tap by tap: equal to one bf16 ulp."""
+@pytest.mark.parametrize("case", WIDE_CASES)
+def test_conv_tiles_match_torch(case):
+    """3x3 convolutions over several N tiles and partial pixel tiles against torch on the CPU (bf16-rounded operands, fp32 sums).
+    LINEAR: LeakyReLU(conv + bias).  SPADE: the gamma|beta GEMM with its fused modulation epilogue, x0 at full or half resolution
+    (nearest x2 up-sampling folded into the index) plus x1 channels, noise, and gamma written for the backward pass."""
     spade, cin, ng, h, w, B, shift, c1 = case
     g = torch.Generator().manual_seed(1)
     rnd = lambda *s: torch.randn(*s, generator=g)
-    x = Act(rnd(B, h, w, ops.round_up(cin, 8)).to(torch.bfloat16).to(DEV), c=cin)
-    outs = []
-    try:
-        os.environ["HRV_CONV_PIXN"] = "0"
-        if spade:
-            C = ng // 2
-            pw = ops.pack_weight((rnd(C, cin, 3, 3) * 0.05).to(DEV), (1, 1), interleave=(rnd(C, cin, 3, 3) * 0.05).to(DEV))
-            x0 = Act(rnd(B, h >> shift, w >> shift, C - c1).to(torch.bfloat16).to(DEV))
-            x1 = Act(rnd(B, h, w, c1).to(torch.bfloat16).to(DEV)) if c1 else None
-            mean, rstd = (rnd(B, C) * 0.1).to(DEV), (torch.rand(B, C, generator=g) + 0.5).to(DEV)
-            noise, ns, sh = rnd(B, h, w).to(DEV), (rnd(C) * 0.1).to(DEV), (rnd(2 * C) * 0.1).to(DEV)
-        else:
-            pw = ops.pack_weight((rnd(ng, cin, 3, 3) * 0.05).to(DEV), (1, 1))
-            bias = rnd(ng).to(DEV)
-        if pw.bk != 64:
-            pytest.skip("the pair kernel needs 64-channel K blocks")
-        for flag in ("0", "1"):
-            os.environ["HRV_CONV_PAIR"] = flag
-            if spade:
-                out, gam = Act.empty(B, h, w, C, zero=True), Act.empty(B, h, w, C, zero=True)
-                ops.conv2d_spade(x, pw, out, x0, shift, x1, mean, rstd, noise, ns, sh, 2, gamma_out=gam)
-                torch.cuda.synchronize()
-                outs.append((out.buf.float().clone(), gam.buf.float().clone()))
-            else:
-                out = Act.empty(B, h, w, ng, zero=True)
-                ops.conv2d(x, pw, out, act=2, shift=bias)
-                torch.cuda.synchronize()
-                outs.append((out.buf.float().clone(), None))
-    finally:
-        os.environ.pop("HRV_CONV_PAIR", None)
-        os.environ.pop("HRV_CONV_PIXN", None)
-    (a, ga), (b, gb) = outs
-    d = float((a - b).abs().max())
-    if pw.bn <= 32 or 144 <= pw.bn <= 208:  # the one-CTA kernel runs the halo mainloop too: same accumulation order
-        assert d == 0.0 and (ga is None or float((ga - gb).abs().max()) == 0.0)
-    else:  # tap-by-tap K order in the one-CTA kernel: fp32 sums differ in the last bits -> at most one bf16 ulp of the largest output
-        assert d <= 2 ** -7 * float(a.abs().max())
-        assert ga is None or float((ga - gb).abs().max()) <= 2 ** -7 * float(ga.abs().max())
+    xb = rnd(B, h, w, ops.round_up(cin, 8)).to(torch.bfloat16)
+    x = Act(xb.to(DEV), c=cin)
+    xn = xb[..., :cin].permute(0, 3, 1, 2).float()
+    lrelu = lambda t: F.leaky_relu(t, 0.2)
+    if spade:
+        C = ng // 2
+        wg, wb = rnd(C, cin, 3, 3) * 0.05, rnd(C, cin, 3, 3) * 0.05
+        pw = ops.pack_weight(wg.to(DEV), (1, 1), interleave=wb.to(DEV))
+        x0h, x1h = rnd(B, h >> shift, w >> shift, C - c1).to(torch.bfloat16), rnd(B, h, w, c1).to(torch.bfloat16) if c1 else None
+        x0, x1 = Act(x0h.to(DEV)), (Act(x1h.to(DEV)) if c1 else None)
+        mean, rstd = rnd(B, C) * 0.1, torch.rand(B, C, generator=g) + 0.5
+        noise, ns, sh = rnd(B, h, w), rnd(C) * 0.1, rnd(2 * C) * 0.1
+        out, gam = Act.empty(B, h, w, C, zero=True), Act.empty(B, h, w, C, zero=True)
+        ops.conv2d_spade(x, pw, out, x0, shift, x1, mean.to(DEV), rstd.to(DEV), noise.to(DEV), ns.to(DEV), sh.to(DEV), 2, gamma_out=gam)
+        torch.cuda.synchronize()
+        gamma = F.conv2d(xn, bf16r(wg), sh[0::2], padding=1)
+        beta = F.conv2d(xn, bf16r(wb), sh[1::2], padding=1)
+        xs = x0h.permute(0, 3, 1, 2).float()
+        if shift:
+            xs = F.interpolate(xs, scale_factor=2, mode="nearest")
+        if c1:
+            xs = torch.cat([xs, x1h.permute(0, 3, 1, 2).float()], 1)
+        v = (xs + noise[:, None] * ns[None, :, None, None] - mean[:, :, None, None]) * rstd[:, :, None, None]
+        ref = lrelu(v * (1 + gamma) + beta)
+        assert rel_err(gam.buf[..., :C].permute(0, 3, 1, 2), gamma) < 1e-2
+    else:
+        wt, bias = rnd(ng, cin, 3, 3) * 0.05, rnd(ng)
+        pw = ops.pack_weight(wt.to(DEV), (1, 1))
+        out = Act.empty(B, h, w, ng, zero=True)
+        ops.conv2d(x, pw, out, act=2, shift=bias.to(DEV))
+        torch.cuda.synchronize()
+        ref = lrelu(F.conv2d(xn, bf16r(wt), bias, padding=1))
+    assert rel_err(out.buf[..., :ref.shape[1]].permute(0, 3, 1, 2), ref) < 1e-2
 
 
 def test_feature_matching_term_matches_torch():

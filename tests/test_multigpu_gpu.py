@@ -75,7 +75,7 @@ def _worker(rank, world, port, ret):
     dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_ranks_equal_one_process_on_the_concatenated_batch():
     from hrviton_b200 import synth
     world = 2

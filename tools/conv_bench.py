@@ -1,5 +1,5 @@
 """Micro-benchmark of hrv_conv2d_fwd on the SPADE-generator layer shapes (device-resident, CUDA events).
-Usage: python tools/conv_bench.py [batch]   (env HRV_CONV_HALO / HRV_CONV_SA / HRV_CONV_TPB_KB select kernel variants)"""
+Usage: python tools/conv_bench.py [batch]"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import hrv_loader; hrv_loader.load()
