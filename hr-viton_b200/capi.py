@@ -13,7 +13,7 @@ EPI_LINEAR, EPI_SPADE = 0, 1
 RES_ADD, RES_GATE_RELU, RES_GATE_LRELU = 0, 1, 2
 
 EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_instnorm_apply", "hrv_norm_apply_affine", "hrv_norm_bwd_reduce", "hrv_norm_bwd_apply", "hrv_act_bwd_bias", "hrv_conv2d_wgrad", "hrv_conv2d_wgrad_workspace_bytes", "hrv_nchw_to_nhwc", "hrv_nhwc_to_nchw",
-           "hrv_space_to_depth", "hrv_avgpool3s2", "hrv_bilinear_up2_add", "hrv_flow_warp", "hrv_bilinear_up2_bwd", "hrv_flow_warp_bwd", "hrv_pack_conv_weight", "hrv_space_to_depth_bwd", "hrv_maxpool2_fwd", "hrv_maxpool2_bwd",
+           "hrv_space_to_depth", "hrv_avgpool3s2", "hrv_bilinear_up2_add", "hrv_flow_warp", "hrv_bilinear_up2_bwd", "hrv_flow_warp_bwd", "hrv_pack_conv_weight", "hrv_pack_conv_weight_tf32x2", "hrv_space_to_depth_bwd", "hrv_maxpool2_fwd", "hrv_maxpool2_bwd",
            "hrv_avgpool3s2_bwd", "hrv_parse_blur_argmax", "hrv_gaussian_blur", "hrv_flow_warp_nchw", "hrv_onehot_u8", "hrv_im2col", "hrv_l1_sum", "hrv_l1_bwd", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 
@@ -95,6 +95,7 @@ def lib(dtype=None):
     L.hrv_l1_sum.argtypes = [TP, TP, vp, vp]
     L.hrv_l1_bwd.argtypes = [TP, TP, vp, TP, i32, vp]
     L.hrv_pack_conv_weight.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp]
+    L.hrv_pack_conv_weight_tf32x2.argtypes = L.hrv_pack_conv_weight.argtypes
     L.hrv_flow_warp_bwd.argtypes = [vp, vp, vp, TP, TP, vp, vp, vp, vp]
     for name in FLAVOURED:
         twin = getattr(L, name + "_f16")

@@ -29,23 +29,52 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 }
 __device__ __forceinline__ uint4 ldg16(const void* p) { return __ldg(reinterpret_cast<const uint4*>(p)); }
 
+// 8 consecutive channels of one pixel in the storage type T: one 16-byte vector of the flavour's 16-bit type, or two of fp32 (the
+// fp32 reference-precision storage).  The kernels below are templates on T; the 16-bit instantiations are the original code.
+template <typename T> struct Vec8 { uint4 u; };
+template <> struct Vec8<float> { float4 a, b; };
+__device__ __forceinline__ Vec8<__nv_bfloat16> ldv8(const __nv_bfloat16* p) { return Vec8<__nv_bfloat16>{ldg16(p)}; }
+__device__ __forceinline__ Vec8<float> ldv8(const float* p) {
+  return Vec8<float>{__ldg(reinterpret_cast<const float4*>(p)), __ldg(reinterpret_cast<const float4*>(p) + 1)};
+}
+__device__ __forceinline__ void unpack8(const Vec8<__nv_bfloat16>& v, float (&f)[8]) { unpack8(v.u, f); }
+__device__ __forceinline__ void unpack8(const Vec8<float>& v, float (&f)[8]) {
+  f[0] = v.a.x; f[1] = v.a.y; f[2] = v.a.z; f[3] = v.a.w; f[4] = v.b.x; f[5] = v.b.y; f[6] = v.b.z; f[7] = v.b.w;
+}
+__device__ __forceinline__ void stv8(__nv_bfloat16* p, const Vec8<__nv_bfloat16>& v) { *reinterpret_cast<uint4*>(p) = v.u; }
+__device__ __forceinline__ void stv8(float* p, const Vec8<float>& v) {
+  reinterpret_cast<float4*>(p)[0] = v.a;
+  reinterpret_cast<float4*>(p)[1] = v.b;
+}
+__device__ __forceinline__ void st8(__nv_bfloat16* p, const float (&f)[8]) { *reinterpret_cast<uint4*>(p) = pack8(f); }
+__device__ __forceinline__ void st8(float* p, const float (&f)[8]) {
+  reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
+  reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
+}
+template <typename T> __device__ __forceinline__ Vec8<T> zero8();
+template <> __device__ __forceinline__ Vec8<__nv_bfloat16> zero8<__nv_bfloat16>() { return Vec8<__nv_bfloat16>{make_uint4(0, 0, 0, 0)}; }
+template <> __device__ __forceinline__ Vec8<float> zero8<float>() { return Vec8<float>{make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)}; }
+
 // ------------------------------------------------------------------------------------------------ IN statistics
 // grid (chunks, N); thread = (pixel lane pl, channel group g of 8).  Each thread accumulates fp32 partial sums over its
 // pixels (4 independent 16-byte loads in flight), partials meet in shared memory (one slot per thread, no atomics),
 // then one fp64 global atomic per channel per block.
+template <typename T>
 struct StatsSrc {
-  const __nv_bfloat16* p0;
-  const __nv_bfloat16* p1;
+  const T* p0;
+  const T* p1;
   const float* noise;
   long long pitch0, pitch1;
   int W, W0, sh, from0;
 };
-__device__ __forceinline__ void stats_load(const StatsSrc& S, long long p, uint4& v, float& nz) {
+template <typename T>
+__device__ __forceinline__ void stats_load(const StatsSrc<T>& S, long long p, Vec8<T>& v, float& nz) {
   const int y = (int)(p / S.W), x = (int)(p - (long long)y * S.W);
-  const __nv_bfloat16* src = S.from0 ? S.p0 + ((long long)(y >> S.sh) * S.W0 + (x >> S.sh)) * S.pitch0 : S.p1 + p * S.pitch1;
-  v = ldg16(src);
+  const T* src = S.from0 ? S.p0 + ((long long)(y >> S.sh) * S.W0 + (x >> S.sh)) * S.pitch0 : S.p1 + p * S.pitch1;
+  v = ldv8(src);
   nz = S.noise ? __ldg(S.noise + p) : 0.f;
 }
+template <typename T>
 __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shift, View x1, int H, int W, int G, int PL,
                                                             int chunk, const float* __restrict__ noise,
                                                             const float* __restrict__ ns, double* __restrict__ acc) {
@@ -63,16 +92,16 @@ __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shi
     float s[8], q[8], nsv[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) { s[i] = 0.f; q[i] = 0.f; nsv[i] = ns ? __ldg(ns + c0 + i) : 0.f; }
-    StatsSrc S;
+    StatsSrc<T> S;
     S.from0 = c0 < x0.c;
     S.sh = x0_shift; S.W = W; S.W0 = W >> x0_shift;
     S.pitch0 = x0.pitch; S.pitch1 = x1.pitch;
-    S.p0 = reinterpret_cast<const __nv_bfloat16*>(x0.ptr) + (long long)n * (H >> x0_shift) * S.W0 * x0.pitch + c0;
-    S.p1 = reinterpret_cast<const __nv_bfloat16*>(x1.ptr) + (long long)n * HW * x1.pitch + (c0 - x0.c);
+    S.p0 = reinterpret_cast<const T*>(x0.ptr) + (long long)n * (H >> x0_shift) * S.W0 * x0.pitch + c0;
+    S.p1 = reinterpret_cast<const T*>(x1.ptr) + (long long)n * HW * x1.pitch + (c0 - x0.c);
     S.noise = noise ? noise + (long long)n * HW : nullptr;
     long long p = p_begin + pl;
     for (; p + 3LL * PL < p_end; p += 4LL * PL) {
-      uint4 v[4];
+      Vec8<T> v[4];
       float nz[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) stats_load(S, p + (long long)u * PL, v[u], nz[u]);
@@ -89,7 +118,7 @@ __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shi
       }
     }
     for (; p < p_end; p += PL) {
-      uint4 v;
+      Vec8<T> v;
       float nz, f[8];
       stats_load(S, p, v, nz);
       unpack8(v, f);
@@ -125,6 +154,7 @@ __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shi
 // X_jc pairs it with the sum of the children's noise — 4x fewer bytes than walking the virtual up-sampled tensor, and the second
 // norm costs no second pass.  Segment 0 of the grid (blockIdx.z) covers x0, segment 1 covers x1.  acc: [N][C][4] doubles
 // {S1, S2, X_0, X_1}; nzacc: [N][2][2] doubles {NZ1_j, NZ2_j}.
+template <typename T>
 __global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift, int c_off, int C, int W_full, int G, int PL, int chunk,
                                                              const float* __restrict__ nz0, const float* __restrict__ nz1,
                                                              double* __restrict__ acc, double* __restrict__ nzacc, int do_noise_sums) {
@@ -142,11 +172,11 @@ __global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift
     const long long p_begin = (long long)blockIdx.x * chunk;
     long long p_end = p_begin + chunk;
     if (p_end > HWs) p_end = HWs;
-    const __nv_bfloat16* base = reinterpret_cast<const __nv_bfloat16*>(xs.ptr) + (long long)n * HWs * xs.pitch + g * 8;
+    const T* base = reinterpret_cast<const T*>(xs.ptr) + (long long)n * HWs * xs.pitch + g * 8;
     const float* n0 = nz0 ? nz0 + (long long)n * HWf : nullptr;
     const float* n1 = nz1 ? nz1 + (long long)n * HWf : nullptr;
     for (long long p = p_begin + pl; p < p_end; p += PL) {
-      const uint4 v = ldg16(base + p * xs.pitch);
+      const Vec8<T> v = ldv8(base + p * xs.pitch);
       float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;  // noise sum / sum of squares over the pixel's footprint, per norm
       if (shift) {
         const int y = (int)(p / xs.w), x = (int)(p - (long long)y * xs.w);
@@ -245,6 +275,7 @@ __global__ void instnorm_finalize_kernel(const double* __restrict__ acc, int NC,
   rstd[i] = (float)(1.0 / sqrt(var + (double)eps));
 }
 
+template <typename T>
 __global__ void instnorm_apply_kernel(View x, const float* __restrict__ mean, const float* __restrict__ rstd,
                                       const float* __restrict__ gamma, const float* __restrict__ beta, View res, int act, View y,
                                       long long total, int G) {
@@ -254,8 +285,8 @@ __global__ void instnorm_apply_kernel(View x, const float* __restrict__ mean, co
   const long long pix = idx / G;
   const int n = (int)(pix / ((long long)x.h * x.w));
   float f[8], r[8];
-  unpack8(ldg16(reinterpret_cast<const __nv_bfloat16*>(x.ptr) + pix * x.pitch + g * 8), f);
-  if (res.ptr) unpack8(ldg16(reinterpret_cast<const __nv_bfloat16*>(res.ptr) + pix * res.pitch + g * 8), r);
+  unpack8(ldv8(reinterpret_cast<const T*>(x.ptr) + pix * x.pitch + g * 8), f);
+  if (res.ptr) unpack8(ldv8(reinterpret_cast<const T*>(res.ptr) + pix * res.pitch + g * 8), r);
   const float* mp = mean + (long long)n * x.c + g * 8;
   const float* rp = rstd + (long long)n * x.c + g * 8;
 #pragma unroll
@@ -270,11 +301,12 @@ __global__ void instnorm_apply_kernel(View x, const float* __restrict__ mean, co
       f[i] = 0.f;
     }
   }
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(y.ptr)) + pix * y.pitch + g * 8) = pack8(f);
+  st8(reinterpret_cast<T*>(const_cast<void*>(y.ptr)) + pix * y.pitch + g * 8, f);
 }
 
 // ------------------------------------------------------------------------------------------------ layout converters
 // thread = (dst pixel, 8-channel group); src fp32 NCHW with nearest resampling.
+template <typename T>
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, int C, int SH, int SW, View dst, int G, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -292,7 +324,7 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, int C, int SH
     const int c = g * 8 + i;
     f[i] = c < C ? __ldg(src + (((long long)n * C + c) * SH + sy) * SW + sx) : 0.f;
   }
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8) = pack8(f);
+  st8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8, f);
 }
 
 // thread = (pixel); loops channels; writes are coalesced per plane.
@@ -313,6 +345,7 @@ __global__ void nhwc_to_nchw_kernel(View src, float* __restrict__ dst, long long
 }
 
 // thread = (dst pixel, sub-pixel 0..3, 8-channel group of src)
+template <typename T>
 __global__ void space_to_depth_kernel(View src, View dst, int G, int Gd, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -321,16 +354,17 @@ __global__ void space_to_depth_kernel(View src, View dst, int G, int Gd, long lo
   const int X = (int)(pix % dst.w);
   const int Y = (int)((pix / dst.w) % dst.h);
   const int n = (int)(pix / ((long long)dst.w * dst.h));
-  uint4 v = make_uint4(0, 0, 0, 0);
+  Vec8<T> v = zero8<T>();
   const int sub = gd / G, g = gd % G;
   if (sub < 4) {
     const int sy = 2 * Y + (sub >> 1), sx = 2 * X + (sub & 1);
     if (sy < src.h && sx < src.w)
-      v = ldg16(reinterpret_cast<const __nv_bfloat16*>(src.ptr) + (((long long)n * src.h + sy) * src.w + sx) * src.pitch + g * 8);
+      v = ldv8(reinterpret_cast<const T*>(src.ptr) + (((long long)n * src.h + sy) * src.w + sx) * src.pitch + g * 8);
   }
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + gd * 8) = v;
+  stv8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + gd * 8, v);
 }
 
+template <typename T>
 __global__ void avgpool3s2_kernel(View src, View dst, int G, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -348,7 +382,7 @@ __global__ void avgpool3s2_kernel(View src, View dst, int G, long long total) {
       const int x = 2 * X + dx;
       if (x < 0 || x >= src.w) continue;
       float f[8];
-      unpack8(ldg16(reinterpret_cast<const __nv_bfloat16*>(src.ptr) + (((long long)n * src.h + y) * src.w + x) * src.pitch + g * 8), f);
+      unpack8(ldv8(reinterpret_cast<const T*>(src.ptr) + (((long long)n * src.h + y) * src.w + x) * src.pitch + g * 8), f);
 #pragma unroll
       for (int i = 0; i < 8; ++i) s[i] += f[i];
       ++cnt;
@@ -357,7 +391,7 @@ __global__ void avgpool3s2_kernel(View src, View dst, int G, long long total) {
   const float inv = 1.f / (float)cnt;
 #pragma unroll
   for (int i = 0; i < 8; ++i) s[i] *= inv;
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8) = pack8(s);
+  st8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8, s);
 }
 
 // F.interpolate(bilinear, x2, align_corners=False): s = max((d+0.5)/2-0.5, 0); i0=floor(s); i1=min(i0+1,n-1)
@@ -371,6 +405,7 @@ __device__ __forceinline__ void up2_taps(int d, int n, int& i0, int& i1, float& 
   w0 = __fsub_rn(1.f, w1);
 }
 
+template <typename T>
 __global__ void bilinear_up2_add_kernel(View a, View b, View dst, int G, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -383,21 +418,21 @@ __global__ void bilinear_up2_add_kernel(View a, View b, View dst, int G, long lo
   float wx0, wx1, wy0, wy1;
   up2_taps(x, a.w, x0, x1, wx0, wx1);
   up2_taps(y, a.h, y0, y1, wy0, wy1);
-  const __nv_bfloat16* ap = reinterpret_cast<const __nv_bfloat16*>(a.ptr) + (long long)n * a.h * a.w * a.pitch + g * 8;
+  const T* ap = reinterpret_cast<const T*>(a.ptr) + (long long)n * a.h * a.w * a.pitch + g * 8;
   float f00[8], f01[8], f10[8], f11[8], o[8];
-  unpack8(ldg16(ap + ((long long)y0 * a.w + x0) * a.pitch), f00);
-  unpack8(ldg16(ap + ((long long)y0 * a.w + x1) * a.pitch), f01);
-  unpack8(ldg16(ap + ((long long)y1 * a.w + x0) * a.pitch), f10);
-  unpack8(ldg16(ap + ((long long)y1 * a.w + x1) * a.pitch), f11);
+  unpack8(ldv8(ap + ((long long)y0 * a.w + x0) * a.pitch), f00);
+  unpack8(ldv8(ap + ((long long)y0 * a.w + x1) * a.pitch), f01);
+  unpack8(ldv8(ap + ((long long)y1 * a.w + x0) * a.pitch), f10);
+  unpack8(ldv8(ap + ((long long)y1 * a.w + x1) * a.pitch), f11);
 #pragma unroll
   for (int i = 0; i < 8; ++i) o[i] = wy0 * (wx0 * f00[i] + wx1 * f01[i]) + wy1 * (wx0 * f10[i] + wx1 * f11[i]);
   if (b.ptr) {
     float fb[8];
-    unpack8(ldg16(reinterpret_cast<const __nv_bfloat16*>(b.ptr) + pix * b.pitch + g * 8), fb);
+    unpack8(ldv8(reinterpret_cast<const T*>(b.ptr) + pix * b.pitch + g * 8), fb);
 #pragma unroll
     for (int i = 0; i < 8; ++i) o[i] += fb[i];
   }
-  *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8) = pack8(o);
+  st8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8, o);
 }
 
 // ------------------------------------------------------------------------------------------------ flow warp
@@ -487,6 +522,21 @@ static int check_bf16_vec(const hrv_tensor* t, const char* what) {
   if (((uintptr_t)t->ptr & 15) || (t->pitch % 8)) return set_error(HRV_EINVAL, "%s: needs 16-byte alignment and pitch %% 8 == 0", what);
   return 0;
 }
+// The entry points that also take fp32 storage: every tensor of one call shares the storage type `dt` of its first one.
+static int storage_of(const hrv_tensor* t) { return (t && t->dtype == HRV_F32) ? HRV_F32 : HRV_BF16; }
+static int check_vec(const hrv_tensor* t, const char* what, int dt) {
+  if (dt == HRV_BF16) return check_bf16_vec(t, what);
+  if (!t || !t->ptr) return set_error(HRV_EINVAL, "%s: null tensor", what);
+  if (t->dtype != HRV_F32) return set_error(HRV_EINVAL, "%s: must be fp32 like the call's other tensors (one storage type per call)", what);
+  if (((uintptr_t)t->ptr & 15) || (t->pitch % 8)) return set_error(HRV_EINVAL, "%s: needs 16-byte alignment and pitch %% 8 == 0", what);
+  return 0;
+}
+// kernel<T><<<...>>>(args) with T = the flavour's 16-bit type or float, after the storage type dt.
+#define HRV_LAUNCH_STORAGE(dt, kernel, grid, block, smem, st, ...)                           \
+  do {                                                                                       \
+    if ((dt) == HRV_F32) kernel<float><<<(grid), (block), (smem), (st)>>>(__VA_ARGS__);      \
+    else kernel<__nv_bfloat16><<<(grid), (block), (smem), (st)>>>(__VA_ARGS__);              \
+  } while (0)
 static int launch_ok(const char* what) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(HRV_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
@@ -501,10 +551,11 @@ using namespace hrv;
 extern "C" int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w,
                                   const float* noise, const float* noise_scale, float eps, float* mean, float* rstd,
                                   void* workspace, size_t workspace_bytes, hrv_stream stream) {
-  int rc = check_bf16_vec(x0, "instnorm_stats x0");
+  const int dt = storage_of(x0);
+  int rc = check_vec(x0, "instnorm_stats x0", dt);
   if (rc) return rc;
   const bool has1 = x1 && x1->ptr;
-  if (has1 && (rc = check_bf16_vec(x1, "instnorm_stats x1"))) return rc;
+  if (has1 && (rc = check_vec(x1, "instnorm_stats x1", dt))) return rc;
   const int C = x0->c + (has1 ? x1->c : 0);
   if ((x0->c % 8) || (C % 8)) return set_error(HRV_EINVAL, "instnorm_stats: channel counts must be multiples of 8");
   if (C / 8 > 256) return set_error(HRV_EUNSUPPORTED, "instnorm_stats: more than 2048 channels");
@@ -524,8 +575,8 @@ extern "C" int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const 
   const long long min_chunk = (long long)PL * 16;
   if (chunk < min_chunk) chunk = min_chunk;
   const unsigned gx = (unsigned)((HW + chunk - 1) / chunk);
-  instnorm_stats_kernel<<<dim3(gx, N), 256, (size_t)PL * C * 2 * sizeof(float), st>>>(mk(x0), x0_shift, mk(has1 ? x1 : nullptr), h, w, G, PL,
-                                                                                 (int)chunk, noise, noise_scale, (double*)workspace);
+  HRV_LAUNCH_STORAGE(dt, instnorm_stats_kernel, dim3(gx, N), 256, (size_t)PL * C * 2 * sizeof(float), st, mk(x0), x0_shift,
+                     mk(has1 ? x1 : nullptr), h, w, G, PL, (int)chunk, noise, noise_scale, (double*)workspace);
   if ((rc = launch_ok("instnorm_stats"))) return rc;
   instnorm_finalize_kernel<<<blocks_for(N * C, 256), 256, 0, st>>>((const double*)workspace, N * C, 1.0 / (double)HW, eps, mean, rstd);
   return launch_ok("instnorm_finalize");
@@ -534,10 +585,11 @@ extern "C" int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const 
 extern "C" int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w, const float* noise0,
                                    const float* noise_scale0, const float* noise1, const float* noise_scale1, float eps, float* mean0,
                                    float* rstd0, float* mean1, float* rstd1, void* workspace, size_t workspace_bytes, hrv_stream stream) {
-  int rc = check_bf16_vec(x0, "instnorm_stats2 x0");
+  const int dt = storage_of(x0);
+  int rc = check_vec(x0, "instnorm_stats2 x0", dt);
   if (rc) return rc;
   const bool has1 = x1 && x1->ptr;
-  if (has1 && (rc = check_bf16_vec(x1, "instnorm_stats2 x1"))) return rc;
+  if (has1 && (rc = check_vec(x1, "instnorm_stats2 x1", dt))) return rc;
   const int C = x0->c + (has1 ? x1->c : 0);
   if ((x0->c % 8) || (C % 8)) return set_error(HRV_EINVAL, "instnorm_stats2: channel counts must be multiples of 8");
   if (x0->c / 8 > 256 || (has1 && x1->c / 8 > 256)) return set_error(HRV_EUNSUPPORTED, "instnorm_stats2: more than 2048 channels per source");
@@ -567,8 +619,8 @@ extern "C" int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const
     const unsigned gx = (unsigned)((HWs + chunk - 1) / chunk);
     // the noise-only sums are taken once, by the segment that walks the full-resolution grid exactly once per pixel: x0's walk covers
     // every full-resolution pixel through its footprint, so segment 0 always does it
-    instnorm_stats2_kernel<<<dim3(gx, N), 256, (size_t)PL * G * 8 * 4 * sizeof(float), st>>>(mk(xs), shift, seg ? x0->c : 0, C, w, G, PL, (int)chunk,
-                                                                                             noise0, noise1, acc, nzacc, seg == 0);
+    HRV_LAUNCH_STORAGE(dt, instnorm_stats2_kernel, dim3(gx, N), 256, (size_t)PL * G * 8 * 4 * sizeof(float), st, mk(xs), shift, seg ? x0->c : 0,
+                       C, w, G, PL, (int)chunk, noise0, noise1, acc, nzacc, seg == 0);
     if ((rc = launch_ok("instnorm_stats2"))) return rc;
   }
   instnorm_finalize2_kernel<<<blocks_for(N * C, 256), 256, 0, st>>>(acc, nzacc, N, C, 1.0 / ((double)h * w), eps, noise0 ? noise_scale0 : nullptr,
@@ -579,14 +631,15 @@ extern "C" int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const
 extern "C" int hrv_norm_apply_affine(const hrv_tensor* x, const float* mean, const float* rstd, const float* gamma, const float* beta,
                                      const hrv_tensor* res, int32_t act, const hrv_tensor* y, hrv_stream stream) {
   int rc;
-  if ((rc = check_bf16_vec(x, "norm_apply x")) || (rc = check_bf16_vec(y, "norm_apply y"))) return rc;
+  const int dt = storage_of(x);
+  if ((rc = check_vec(x, "norm_apply x", dt)) || (rc = check_vec(y, "norm_apply y", dt))) return rc;
   const bool hr = res && res->ptr;
-  if (hr && (rc = check_bf16_vec(res, "norm_apply res"))) return rc;
+  if (hr && (rc = check_vec(res, "norm_apply res", dt))) return rc;
   if (!mean || !rstd) return set_error(HRV_EINVAL, "norm_apply: mean/rstd required");
   const int G = (x->c + 7) / 8;
   const long long total = (long long)x->n * x->h * x->w * G;
-  instnorm_apply_kernel<<<blocks_for(total, 256), 256, 0, (cudaStream_t)stream>>>(mk(x), mean, rstd, gamma, beta, mk(hr ? res : nullptr), act,
-                                                                                 mk(y), total, G);
+  HRV_LAUNCH_STORAGE(dt, instnorm_apply_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, mk(x), mean, rstd, gamma, beta,
+                     mk(hr ? res : nullptr), act, mk(y), total, G);
   return launch_ok("norm_apply");
 }
 
@@ -596,12 +649,13 @@ extern "C" int hrv_instnorm_apply(const hrv_tensor* x, const float* mean, const 
 }
 
 extern "C" int hrv_nchw_to_nhwc(const float* src, int32_t c, int32_t src_h, int32_t src_w, const hrv_tensor* dst, hrv_stream stream) {
-  int rc = check_bf16_vec(dst, "nchw_to_nhwc dst");
+  const int dt = storage_of(dst);
+  int rc = check_vec(dst, "nchw_to_nhwc dst", dt);
   if (rc) return rc;
   const int G = (dst->c + 7) / 8;
   if (G * 8 > dst->pitch) return set_error(HRV_EINVAL, "nchw_to_nhwc: dst pitch too small for padded channels");
   const long long total = (long long)dst->n * dst->h * dst->w * G;
-  nchw_to_nhwc_kernel<<<blocks_for(total, 256), 256, 0, (cudaStream_t)stream>>>(src, c, src_h, src_w, mk(dst), G, total);
+  HRV_LAUNCH_STORAGE(dt, nchw_to_nhwc_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, src, c, src_h, src_w, mk(dst), G, total);
   return launch_ok("nchw_to_nhwc");
 }
 
@@ -614,35 +668,38 @@ extern "C" int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream st
 
 extern "C" int hrv_space_to_depth(const hrv_tensor* src, const hrv_tensor* dst, hrv_stream stream) {
   int rc;
-  if ((rc = check_bf16_vec(src, "s2d src")) || (rc = check_bf16_vec(dst, "s2d dst"))) return rc;
+  const int dt = storage_of(src);
+  if ((rc = check_vec(src, "s2d src", dt)) || (rc = check_vec(dst, "s2d dst", dt))) return rc;
   const int G = (src->c + 7) / 8;
   if (dst->h != (src->h + 1) / 2 || dst->w != (src->w + 1) / 2 || dst->c < 4 * G * 8 || (dst->c % 8))
     return set_error(HRV_EINVAL, "s2d: dst must be ceil(h/2) x ceil(w/2) x (>= 4*roundup8(c))");
   const int Gd = dst->c / 8;
   const long long total = (long long)dst->n * dst->h * dst->w * Gd;
-  space_to_depth_kernel<<<blocks_for(total, 256), 256, 0, (cudaStream_t)stream>>>(mk(src), mk(dst), G, Gd, total);
+  HRV_LAUNCH_STORAGE(dt, space_to_depth_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, mk(src), mk(dst), G, Gd, total);
   return launch_ok("space_to_depth");
 }
 
 extern "C" int hrv_avgpool3s2(const hrv_tensor* src, const hrv_tensor* dst, hrv_stream stream) {
   int rc;
-  if ((rc = check_bf16_vec(src, "avgpool src")) || (rc = check_bf16_vec(dst, "avgpool dst"))) return rc;
+  const int dt = storage_of(src);
+  if ((rc = check_vec(src, "avgpool src", dt)) || (rc = check_vec(dst, "avgpool dst", dt))) return rc;
   if (dst->h != (src->h - 1) / 2 + 1 || dst->w != (src->w - 1) / 2 + 1) return set_error(HRV_EINVAL, "avgpool: dst extent");
   const int G = (src->c + 7) / 8;
   const long long total = (long long)dst->n * dst->h * dst->w * G;
-  avgpool3s2_kernel<<<blocks_for(total, 256), 256, 0, (cudaStream_t)stream>>>(mk(src), mk(dst), G, total);
+  HRV_LAUNCH_STORAGE(dt, avgpool3s2_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, mk(src), mk(dst), G, total);
   return launch_ok("avgpool3s2");
 }
 
 extern "C" int hrv_bilinear_up2_add(const hrv_tensor* a, const hrv_tensor* b, const hrv_tensor* dst, hrv_stream stream) {
   int rc;
-  if ((rc = check_bf16_vec(a, "up2 a")) || (rc = check_bf16_vec(dst, "up2 dst"))) return rc;
+  const int dt = storage_of(a);
+  if ((rc = check_vec(a, "up2 a", dt)) || (rc = check_vec(dst, "up2 dst", dt))) return rc;
   const bool hb = b && b->ptr;
-  if (hb && (rc = check_bf16_vec(b, "up2 b"))) return rc;
+  if (hb && (rc = check_vec(b, "up2 b", dt))) return rc;
   if (dst->h != 2 * a->h || dst->w != 2 * a->w) return set_error(HRV_EINVAL, "up2: dst must be 2x");
   const int G = (a->c + 7) / 8;
   const long long total = (long long)dst->n * dst->h * dst->w * G;
-  bilinear_up2_add_kernel<<<blocks_for(total, 256), 256, 0, (cudaStream_t)stream>>>(mk(a), mk(hb ? b : nullptr), mk(dst), G, total);
+  HRV_LAUNCH_STORAGE(dt, bilinear_up2_add_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, mk(a), mk(hb ? b : nullptr), mk(dst), G, total);
   return launch_ok("bilinear_up2_add");
 }
 
@@ -841,13 +898,16 @@ extern "C" int hrv_flow_warp_bwd(const float* flow_lo, const float* lin_x, const
 
 // ------------------------------------------------------------------------------------------------ weight packing
 namespace hrv {
-// One pass from the fp32 parameter layout (cout,cin,kh,kw) to the bf16 GEMM layout [taps][n_pad][cin_k] (zero padded), with
-// optional 1/sigma scaling, (gamma,beta) row interleave of two parameters and the flip+transpose of the data-gradient convolution.
+// One pass from the fp32 parameter layout (cout,cin,kh,kw) to the GEMM layout [taps][n_pad][cin_k] (zero padded), with optional
+// 1/sigma scaling, (gamma,beta) row interleave of two parameters and the flip+transpose of the data-gradient convolution.
+// kSplit = false: one plane of the flavour's 16-bit type.  kSplit = true (the 3xTF32 convolution of fp32 storage): fp32 planes
+// hi = rna_tf32(v) at [0][taps][n_pad][cin_k] and lo = rna_tf32(v - hi) at [1][taps][n_pad][cin_k].
+template <bool kSplit, typename D>
 __global__ void pack_conv_weight_kernel(const float* __restrict__ w0, const float* __restrict__ w1, int cout, int cin, int kh, int kw,
-                                        int transpose_flip, const float* __restrict__ inv_scale, __nv_bfloat16* __restrict__ dst,
+                                        int transpose_flip, const float* __restrict__ inv_scale, D* __restrict__ dst,
                                         int n_pad, int cin_k, long long plane) {
   // thread = one (row n, K index c) of the GEMM operand; it walks the kh*kw taps, i.e. reads the taps of one (co,ci) pair from
-  // CONTIGUOUS fp32 memory and writes one bf16 per tap plane (coalesced across the threads of a warp, which vary c).
+  // CONTIGUOUS fp32 memory and writes one element per tap plane (coalesced across the threads of a warp, which vary c).
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= plane) return;
   const int c = (int)(idx % cin_k);
@@ -865,7 +925,13 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w0, const floa
   const float sc = inv_scale ? __ldg(inv_scale) : 1.f;
   for (int tap = 0; tap < taps; ++tap) {
     const float v = src ? __ldg(src + (transpose_flip ? taps - 1 - tap : tap)) * sc : 0.f;
-    dst[(long long)tap * plane + idx] = __float2bfloat16(v);
+    if constexpr (kSplit) {
+      const float hi = rna_tf32(v);
+      dst[(long long)tap * plane + idx] = hi;
+      dst[(long long)(taps + tap) * plane + idx] = rna_tf32(v - hi);
+    } else {
+      dst[(long long)tap * plane + idx] = __float2bfloat16(v);
+    }
   }
 }
 }  // namespace hrv
@@ -878,7 +944,21 @@ extern "C" int hrv_pack_conv_weight(const float* w0, const float* w1, int32_t co
   const int rows = transpose_flip ? cin : cout * inter, cols = transpose_flip ? cout * inter : cin;
   if (n_pad < rows || cin_k < cols) return set_error(HRV_EINVAL, "pack_conv_weight: destination too small (%d x %d for %d x %d)", n_pad, cin_k, rows, cols);
   const long long plane = (long long)n_pad * cin_k;
-  pack_conv_weight_kernel<<<blocks_for(plane, 256), 256, 0, (cudaStream_t)stream>>>(w0, w1, cout, cin, kh, kw, transpose_flip, inv_scale,
-                                                                                   (__nv_bfloat16*)dst, n_pad, cin_k, plane);
+  pack_conv_weight_kernel<false><<<blocks_for(plane, 256), 256, 0, (cudaStream_t)stream>>>(w0, w1, cout, cin, kh, kw, transpose_flip, inv_scale,
+                                                                                          (__nv_bfloat16*)dst, n_pad, cin_k, plane);
   return launch_ok("pack_conv_weight");
+}
+
+extern "C" int hrv_pack_conv_weight_tf32x2(const float* w0, const float* w1, int32_t cout, int32_t cin, int32_t kh, int32_t kw,
+                                           int32_t transpose_flip, const float* inv_scale, void* dst, int32_t n_pad, int32_t cin_k,
+                                           hrv_stream stream) {
+  if (!w0 || !dst || cout < 1 || cin < 1 || kh < 1 || kw < 1) return set_error(HRV_EINVAL, "pack_conv_weight_tf32x2: bad arguments");
+  const int inter = w1 ? 2 : 1;
+  const int rows = transpose_flip ? cin : cout * inter, cols = transpose_flip ? cout * inter : cin;
+  if (n_pad < rows || cin_k < cols)
+    return set_error(HRV_EINVAL, "pack_conv_weight_tf32x2: destination too small (%d x %d for %d x %d)", n_pad, cin_k, rows, cols);
+  const long long plane = (long long)n_pad * cin_k;
+  pack_conv_weight_kernel<true><<<blocks_for(plane, 256), 256, 0, (cudaStream_t)stream>>>(w0, w1, cout, cin, kh, kw, transpose_flip, inv_scale,
+                                                                                          (float*)dst, n_pad, cin_k, plane);
+  return launch_ok("pack_conv_weight_tf32x2");
 }

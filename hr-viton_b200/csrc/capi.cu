@@ -31,7 +31,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                      const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle) {
+                      const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle, CUtensorMapDataType type) {
   static EncodeTiledFn fn = nullptr;
   if (!fn) {
     void* sym = nullptr;
@@ -41,7 +41,7 @@ int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* 
       return set_error(HRV_ECUDA, "cuTensorMapEncodeTiled entry point unavailable (%s)", cudaGetErrorString(e));
     fn = (EncodeTiledFn)sym;
   }
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, base, dims, strides_bytes, box, elem_strides,
+  CUresult r = fn(map, type, (cuuint32_t)rank, base, dims, strides_bytes, box, elem_strides,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
     return set_error(HRV_ECUDA, "cuTensorMapEncodeTiled failed: CUresult %d (rank %d dims %llu,%llu box %u,%u)", (int)r, rank,

@@ -255,27 +255,6 @@ __global__ void __launch_bounds__(kThreads, 2) conv_wgmma_kernel(const __grid_co
 
 // ------------------------------------------------------------------------------------------------ host side
 
-static int log2i(int v) {
-  int l = 0;
-  while ((1 << l) < v) ++l;
-  return l;
-}
-
-// Pick the power-of-two tile extent p <= cap for a dimension of size `dim`: least padding, ties -> larger.
-static int pick_pow2(int dim, int cap) {
-  int best = 1;
-  double best_waste = 1e30;
-  for (int p = 1; p <= cap; p <<= 1) {
-    const int tiles = (dim + p - 1) / p;
-    const double waste = (double)tiles * p / dim;
-    if (waste <= best_waste + 0.031) {
-      if (waste < best_waste) best_waste = waste;
-      best = p;
-    }
-  }
-  return best;
-}
-
 template <int BNT>
 static int launch_conv(const ConvArgs& args, int grid, size_t smem, cudaStream_t st) {
   static bool attr_done = false;
@@ -298,6 +277,7 @@ extern "C" int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream) {
   if (!p) return set_error(HRV_EINVAL, "conv: null params");
   const hrv_tensor& in = p->in;
   const hrv_tensor& out = p->out;
+  if (in.dtype == HRV_F32) return conv2d_fwd_tf32x3(p, stream);  // fp32 storage: the 3xTF32 kernel of conv_f32.cu
   if (in.dtype != HRV_BF16) return set_error(HRV_EINVAL, "conv: input must be bf16 NHWC");
   if (((uintptr_t)in.ptr & 15) || (in.pitch % 8) || in.pitch < in.c)
     return set_error(HRV_EINVAL, "conv: input needs 16-byte aligned ptr and pitch %% 8 == 0 (pitch=%d c=%d)", in.pitch, in.c);

@@ -14,9 +14,12 @@ struct GView {
 };
 GView gv(const hrv_tensor* t) { return GView{t->ptr, t->n, t->h, t->w, t->c, t->pitch}; }
 
-int check_vec(const hrv_tensor* t, const char* what) {
+// dt: the storage type every tensor of the call must have (fp32 only where an entry point takes fp32 storage).
+int check_vec(const hrv_tensor* t, const char* what, int dt = HRV_BF16) {
   if (!t || !t->ptr) return set_error(HRV_EINVAL, "%s: null tensor", what);
-  if (t->dtype != HRV_BF16) return set_error(HRV_EINVAL, "%s: must be bf16 NHWC", what);
+  if (t->dtype != dt)
+    return dt == HRV_BF16 ? set_error(HRV_EINVAL, "%s: must be bf16 NHWC", what)
+                          : set_error(HRV_EINVAL, "%s: must be fp32 like the call's other tensors (one storage type per call)", what);
   if (((uintptr_t)t->ptr & 15) || (t->pitch % 8) || t->pitch < t->c) return set_error(HRV_EINVAL, "%s: needs a 16-byte aligned ptr and pitch %% 8 == 0", what);
   return HRV_OK;
 }
@@ -320,6 +323,8 @@ __global__ void __launch_bounds__(256) onehot_u8_kernel(const unsigned char* __r
 // dst[n,y,x, tap*C + ci] = src[n, y+ky-pad, x+kx-pad, ci] (zero outside / beyond taps*C).  A 3x3 convolution over a 7-channel
 // label map (SPADE's mlp_shared, network_generator.py:182-184) becomes ONE K=64 GEMM block per pixel tile instead of nine K=16
 // taps, and its weight gradient a plain 1x1 GEMM.  thread = (pixel, 8-channel group of dst)
+// E = the raw storage element: unsigned short (either 16-bit type, moved as bits) or float (fp32 storage).
+template <typename E>
 __global__ void im2col_kernel(GView src, GView dst, int kh, int kw, int pad, int Gd, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
@@ -327,12 +332,12 @@ __global__ void im2col_kernel(GView src, GView dst, int kh, int kw, int pad, int
   const long long pix = idx / Gd;
   const int x = (int)(pix % dst.w), y = (int)((pix / dst.w) % dst.h), n = (int)(pix / ((long long)dst.w * dst.h));
   const int K = kh * kw * src.c;
-  const unsigned short* s = reinterpret_cast<const unsigned short*>(src.ptr);
-  unsigned short v[8];
+  const E* s = reinterpret_cast<const E*>(src.ptr);
+  E v[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const int j = g * 8 + i;
-    unsigned short o = 0;
+    E o = 0;
     if (j < K) {
       const int tap = j / src.c, ci = j - tap * src.c;
       const int ky = tap / kw, kx = tap - ky * kw;
@@ -341,9 +346,15 @@ __global__ void im2col_kernel(GView src, GView dst, int kh, int kw, int pad, int
     }
     v[i] = o;
   }
-  uint4 o4;
-  o4.x = v[0] | ((unsigned)v[1] << 16); o4.y = v[2] | ((unsigned)v[3] << 16); o4.z = v[4] | ((unsigned)v[5] << 16); o4.w = v[6] | ((unsigned)v[7] << 16);
-  st16(at_w(dst, n, y, x) + g * 8, o4);
+  if constexpr (sizeof(E) == 2) {
+    uint4 o4;
+    o4.x = v[0] | ((unsigned)v[1] << 16); o4.y = v[2] | ((unsigned)v[3] << 16); o4.z = v[4] | ((unsigned)v[5] << 16); o4.w = v[6] | ((unsigned)v[7] << 16);
+    st16(at_w(dst, n, y, x) + g * 8, o4);
+  } else {
+    float4* o = reinterpret_cast<float4*>(reinterpret_cast<float*>(const_cast<void*>(dst.ptr)) + (((long long)n * dst.h + y) * dst.w + x) * dst.pitch + g * 8);
+    o[0] = make_float4(v[0], v[1], v[2], v[3]);
+    o[1] = make_float4(v[4], v[5], v[6], v[7]);
+  }
 }
 
 // 3x3 / 7-channel specialisation (the SPADE label map): thread = pixel; nine 16-byte loads (one per tap, the 8th lane is the
@@ -537,16 +548,20 @@ extern "C" int hrv_flow_warp_nchw(const float* flow_lo, int32_t n, int32_t hl, i
 
 extern "C" int hrv_im2col(const hrv_tensor* src, const hrv_tensor* dst, int32_t kh, int32_t kw, int32_t pad, hrv_stream stream) {
   int rc;
-  if ((rc = check_vec(src, "im2col src")) || (rc = check_vec(dst, "im2col dst"))) return rc;
+  const bool f32 = src && src->dtype == HRV_F32;  // fp32 storage: the generic kernel on 4-byte elements, dst fp32 as well
+  const int dt = f32 ? HRV_F32 : HRV_BF16;
+  if ((rc = check_vec(src, "im2col src", dt)) || (rc = check_vec(dst, "im2col dst", dt))) return rc;
   if (kh < 1 || kw < 1 || dst->n != src->n || dst->h != src->h || dst->w != src->w || dst->c < kh * kw * src->c || (dst->c % 8))
     return set_error(HRV_EINVAL, "im2col: dst must be (n,h,w, >= kh*kw*c, multiple of 8)");
   const int Gd = dst->c / 8;
   const long long total = (long long)dst->n * dst->h * dst->w * Gd;
   const long long npix = (long long)dst->n * dst->h * dst->w;
-  if (kh == 3 && kw == 3 && pad == 1 && src->c == 7 && dst->c == 64) {
+  if (f32) {
+    if (total) im2col_kernel<float><<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(gv(src), gv(dst), kh, kw, pad, Gd, total);
+  } else if (kh == 3 && kw == 3 && pad == 1 && src->c == 7 && dst->c == 64) {
     if (npix) im2col3x3_c7_kernel<<<nblocks(npix, 256), 256, 0, (cudaStream_t)stream>>>(gv(src), gv(dst), npix);
   } else if (total) {
-    im2col_kernel<<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(gv(src), gv(dst), kh, kw, pad, Gd, total);
+    im2col_kernel<unsigned short><<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(gv(src), gv(dst), kh, kw, pad, Gd, total);
   }
   return launched("im2col");
 }

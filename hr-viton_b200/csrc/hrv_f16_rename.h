@@ -18,6 +18,7 @@
 #define hrv_bilinear_up2_bwd hrv_bilinear_up2_bwd_f16
 #define hrv_flow_warp_bwd hrv_flow_warp_bwd_f16
 #define hrv_pack_conv_weight hrv_pack_conv_weight_f16
+#define hrv_pack_conv_weight_tf32x2 hrv_pack_conv_weight_tf32x2_f16
 #define hrv_space_to_depth_bwd hrv_space_to_depth_bwd_f16
 #define hrv_maxpool2_fwd hrv_maxpool2_fwd_f16
 #define hrv_maxpool2_bwd hrv_maxpool2_bwd_f16

@@ -18,7 +18,31 @@ int set_error(int code, const char* fmt, ...);
 int sm_count();
 // cuTensorMapEncodeTiled through cudaGetDriverEntryPoint (no link-time dependency on libcuda).
 int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                      const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle);
+                      const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle,
+                      CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+// hrv_conv2d_fwd on fp32 storage (conv_f32.cu, compiled once): both flavours of hrv_conv2d_fwd hand an fp32 input to it.
+int conv2d_fwd_tf32x3(const hrv_conv_params* p, hrv_stream stream);
+
+// Pixel-tile geometry shared by the convolution kernels.
+inline int log2i(int v) {
+  int l = 0;
+  while ((1 << l) < v) ++l;
+  return l;
+}
+// Pick the power-of-two tile extent p <= cap for a dimension of size `dim`: least padding, ties -> larger.
+inline int pick_pow2(int dim, int cap) {
+  int best = 1;
+  double best_waste = 1e30;
+  for (int p = 1; p <= cap; p <<= 1) {
+    const int tiles = (dim + p - 1) / p;
+    const double waste = (double)tiles * p / dim;
+    if (waste <= best_waste + 0.031) {
+      if (waste < best_waste) best_waste = waste;
+      best = p;
+    }
+  }
+  return best;
+}
 }  // namespace hrv_host
 namespace hrv {
 using namespace hrv_host;

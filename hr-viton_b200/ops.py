@@ -1,5 +1,6 @@
 """NHWC activation views + thin wrappers over the C-ABI.  torch is used here for device memory and streams only."""
 import ctypes
+import os
 from dataclasses import dataclass
 
 import torch
@@ -9,8 +10,9 @@ from .capi import ACT_LRELU, ACT_NONE, ACT_RELU, ACT_TANH, BF16, F32  # noqa: F4
 
 LAUNCHES = [0]  # count of kernel launches issued through the C-ABI (bench.py reads this for `gpu_launches`)
 PARAM_GEN = [0]  # generation of the parameter values: part of every derived-weight cache key (spade._param_key)
-STORAGE = [torch.bfloat16]  # activation storage type of newly created buffers: torch.bfloat16 (default) or torch.float16
+STORAGE = [torch.bfloat16]  # activation storage type of newly created buffers: torch.bfloat16 (default), torch.float16 or torch.float32
 PROFILE = None  # bench.py sets this to a list; every C-ABI call then appends (kind, work, start_event, end_event)
+PRECISIONS = {"bf16": torch.bfloat16, "fp16": torch.float16, "fp32": torch.float32}
 
 
 class _Timed:
@@ -35,17 +37,31 @@ class _Timed:
 
 
 def set_precision(name):
-    """'bf16' (default: bf16 activations, fp32 accumulation — the training configuration) or 'fp16' (IEEE half activations,
+    """'bf16' (default: bf16 activations, fp32 accumulation — the training configuration), 'fp16' (IEEE half activations,
     3 more mantissa bits: the storage type of the reference's own apex-O1 --fp16 runs, train_generator.py:161-169; meets the
-    1e-2 forward tolerance of BASELINE.json).  Invalidates every derived-weight cache."""
-    dt = {"bf16": torch.bfloat16, "fp16": torch.float16}[name]
+    1e-2 forward tolerance of BASELINE.json) or 'fp32' (fp32 activations and 3xTF32 convolutions: the reference's own fp32
+    inference to the 1e-3 tolerance of BASELINE.json; inference only).  Invalidates every derived-weight cache."""
+    if name not in PRECISIONS:
+        raise ValueError("precision must be one of %s, got %r" % ("/".join(PRECISIONS), name))
+    dt = PRECISIONS[name]
     if STORAGE[0] != dt:
         STORAGE[0] = dt
         PARAM_GEN[0] += 1
 
 
 def get_precision():
-    return "fp16" if STORAGE[0] == torch.float16 else "bf16"
+    return {v: k for k, v in PRECISIONS.items()}[STORAGE[0]]
+
+
+def require_trainable_storage(what):
+    """Training entry points call this before any launch: fp32 storage has no backward kernels."""
+    if STORAGE[0] == torch.float32:
+        raise NotImplementedError("fp32 storage is inference-only (%s needs a backward pass): call ops.set_precision('bf16') or "
+                                  "set_precision('fp16') to train" % what)
+
+
+# The reference's inference scripts run unchanged in another precision through the environment (read once, here).
+set_precision(os.environ.get("HRV_PRECISION", "bf16"))
 
 
 def _L(*things):
@@ -115,7 +131,7 @@ def _p(t):
 
 
 def from_nchw(x, c_pad=None, size=None, out=None):
-    """fp32 NCHW (cuda) -> bf16 NHWC Act, optional nearest resize to `size` (F.interpolate nearest)."""
+    """fp32 NCHW (cuda) -> NHWC Act in the storage type, optional nearest resize to `size` (F.interpolate nearest)."""
     assert x.is_cuda and x.dtype == torch.float32
     x = x.contiguous()
     n, c, h, w = x.shape
@@ -170,7 +186,7 @@ def pick_bn_spade(n_gemm):
 
 @dataclass
 class PackedConv:
-    w: torch.Tensor  # bf16 [taps, n_pad, cin_k]
+    w: torch.Tensor  # 16-bit [taps, n_pad, cin_k], or fp32 [2 (hi, lo), taps, n_pad, cin_k] on fp32 storage
     kh: int
     kw: int
     off_y: int
@@ -198,16 +214,26 @@ def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixe
     inter = 2 if interleave is not None else 1
     rows, cols = (cin, cout * inter) if dgrad else (cout * inter, cin)  # GEMM N rows, K columns
     k_eff = cols if cin_total is None else cin_total
-    # Cout <= 128 with more than 32 input channels: 64-channel K blocks (zero padded), the convolution kernel's own block size
-    bk = 64 if (rows <= 128 and k_eff > 32) else pick_bk(k_eff)  # K <= 32 stays on the 32-wide blocks (padding to 64 would double the MMAs)
+    f32 = STORAGE[0] == torch.float32
+    if f32:
+        bk = 32  # the 3xTF32 kernel's K block: 32 fp32 channels = one 128-byte swizzle row
+    else:
+        # Cout <= 128 with more than 32 input channels: 64-channel K blocks (zero padded), the convolution kernel's own block size
+        bk = 64 if (rows <= 128 and k_eff > 32) else pick_bk(k_eff)  # K <= 32 stays on the 32-wide blocks (padding to 64 would double the MMAs)
     cin_k = round_up(k_eff, bk)
     if bn is None:
         bn = pick_bn_spade(rows) if (interleave is not None and not dgrad) else pick_bn(rows)
     n_pad = round_up(rows, bn)
-    wp = torch.empty((kh * kw, n_pad, cin_k), dtype=STORAGE[0], device=w.device)
-    with _Timed("glue", 0.0, label="pack_conv_weight"):
-        capi.check(_L(wp).hrv_pack_conv_weight(w.data_ptr(), _p(interleave), cout, cin, kh, kw, 1 if dgrad else 0, None, wp.data_ptr(),
-                                                   n_pad, cin_k, _stream()), "pack_conv_weight")
+    if f32:  # hi / lo planes of the 3xTF32 split
+        wp = torch.empty((2, kh * kw, n_pad, cin_k), dtype=torch.float32, device=w.device)
+        with _Timed("glue", 0.0, label="pack_conv_weight_tf32x2"):
+            capi.check(capi.lib().hrv_pack_conv_weight_tf32x2(w.data_ptr(), _p(interleave), cout, cin, kh, kw, 1 if dgrad else 0, None,
+                                                              wp.data_ptr(), n_pad, cin_k, _stream()), "pack_conv_weight_tf32x2")
+    else:
+        wp = torch.empty((kh * kw, n_pad, cin_k), dtype=STORAGE[0], device=w.device)
+        with _Timed("glue", 0.0, label="pack_conv_weight"):
+            capi.check(_L(wp).hrv_pack_conv_weight(w.data_ptr(), _p(interleave), cout, cin, kh, kw, 1 if dgrad else 0, None, wp.data_ptr(),
+                                                       n_pad, cin_k, _stream()), "pack_conv_weight")
     fpp = 2.0 * cin * cout * inter * kh * kw if flops_per_pixel is None else flops_per_pixel
     return PackedConv(wp, kh, kw, off[0], off[1], bk, bn, rows, k_eff, fpp)
 

@@ -314,6 +314,7 @@ class SPADEGenerator(BaseNetwork):
         if self.num_upsampling_layers != "most":
             raise NotImplementedError("only num_upsampling_layers='most' (the reference's configuration) is implemented")
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+            ops.require_trainable_storage("SPADEGenerator with grad")
             try:
                 from . import autograd_g
             except ImportError:
@@ -460,6 +461,7 @@ class MultiscaleDiscriminator(BaseNetwork):
     def forward(self, input):
         _need_cuda(input, "MultiscaleDiscriminator")
         if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())):
+            ops.require_trainable_storage("MultiscaleDiscriminator with grad")
             try:
                 from . import autograd_g
             except ImportError:

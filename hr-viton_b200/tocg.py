@@ -104,6 +104,7 @@ class ResBlock(nn.Module):
         _need_cuda(x, "ResBlock")
         if self.training:
             # train-mode BatchNorm (batch statistics, running-stat update) lives in the autograd path (networks.py:188-198)
+            ops.require_trainable_storage("ResBlock in train mode")
             from . import autograd_tocg
             from .autograd_g import FromNCHW
             y = autograd_tocg._resblock(self, FromNCHW.apply(x.float(), None, None))
@@ -176,6 +177,7 @@ class ConditionGenerator(nn.Module):
         if self.training:
             # train mode = batch-statistics BatchNorm (+ running-stat updates) exactly as nn.BatchNorm2d in the reference
             # (train_condition.py:158 calls tocg(input1, input2) in train mode); with grad enabled it also carries the autograd graph
+            ops.require_trainable_storage("ConditionGenerator in train mode")
             from . import autograd_tocg
             return autograd_tocg.tocg_forward_train(self, input1, input2)
         if torch.is_grad_enabled() and (input1.requires_grad or input2.requires_grad):
@@ -372,6 +374,7 @@ class MultiscaleDiscriminator(nn.Module):
         _need_cuda(input, "MultiscaleDiscriminator")
         if torch.is_grad_enabled() and (input.requires_grad or any(p.requires_grad for p in self.parameters())) and not self.getIntermFeat:
             # differentiable path (train_condition.py:208-232: D(fake) back-propagates into tocg, D(real/fake.detach()) into D)
+            ops.require_trainable_storage("MultiscaleDiscriminator with grad")
             from . import autograd_tocg
             return autograd_tocg.tocg_discriminator_forward_train(self, input)
         with torch.no_grad():

@@ -7,6 +7,8 @@ Hot path = the three networks (kernels of this repo).  The per-step tensor glue 
 import torch
 import torch.nn.functional as F
 
+from . import ops
+
 _GRID_CACHE = {}
 LABELS7 = [[0], [2, 4, 7, 8, 9, 10, 11], [3], [1], [5], [6], [12]]  # train_generator.py:261-269
 GROUP_OF_13 = [next(i for i, grp in enumerate(LABELS7) if k in grp) for k in range(13)]
@@ -218,6 +220,7 @@ class Stage2Trainer(_GraphMixin):
 
     def step(self, batch, fine_h, fine_w):
         from . import autograd_g
+        ops.require_trainable_storage("Stage2Trainer.step")
         g_in, parse = make_generator_inputs(self.tocg, batch, fine_h, fine_w, occlusion=self.occlusion)
         im = batch["image"]
         # ---------------- generator update (train_generator.py:279-322)
@@ -299,6 +302,7 @@ class Stage1Trainer(_GraphMixin):
     def step(self, batch):
         from . import autograd_g, autograd_tocg
         from .tocg import make_grid
+        ops.require_trainable_storage("Stage1Trainer.step")
         c_paired, im_c, pcm = batch["cloth"], batch["parse_cloth"], batch["pcm"]
         cm_paired = (batch["cloth_mask"] > 0.5).float()
         input1 = torch.cat([c_paired, cm_paired], 1)

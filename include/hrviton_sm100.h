@@ -16,6 +16,11 @@
  * fp16: same signatures, same kernels compiled against the other 16-bit type, wgmma operand format f16 instead of bf16.
  * fp32 buffers (flows, logits, images, statistics, weight gradients) are identical in both.  Wherever a comment says "bf16" read
  * "the flavour's 16-bit storage type"; hrv_dtype code 0 denotes it.
+ *
+ * fp32 storage (the reference-precision inference mode): the forward entry points marked "fp32 storage" below also take activations
+ * with dtype HRV_F32, in either flavour, and then run the same algorithm on fp32 NHWC tensors.  Every activation tensor of such a
+ * call must be fp32 (mixed storage returns HRV_EINVAL).  hrv_conv2d_fwd on an fp32 input runs a 3xTF32 wgmma kernel over weights
+ * packed by hrv_pack_conv_weight_tf32x2.  There is no fp32 backward pass.
  */
 #ifndef HRVITON_SM100_H_
 #define HRVITON_SM100_H_
@@ -30,7 +35,10 @@ extern "C" {
 typedef void* hrv_stream; /* cudaStream_t */
 
 enum hrv_status { HRV_OK = 0, HRV_EINVAL = -1, HRV_ECUDA = -2, HRV_EUNSUPPORTED = -3 };
-enum hrv_dtype { HRV_BF16 = 0 /* = the flavour's 16-bit type: bf16 in hrv_<op>, fp16 in hrv_<op>_f16 */, HRV_F32 = 1 };
+enum hrv_dtype {
+  HRV_BF16 = 0, /* = the flavour's 16-bit type: bf16 in hrv_<op>, fp16 in hrv_<op>_f16 */
+  HRV_F32 = 1   /* fp32: flows, logits, images, statistics; and activation storage of the fp32 inference mode */
+};
 enum hrv_act { HRV_ACT_NONE = 0, HRV_ACT_RELU = 1, HRV_ACT_LRELU02 = 2, HRV_ACT_TANH = 3 };
 enum hrv_layout { HRV_NHWC = 0, HRV_NCHW = 1 };
 enum hrv_epilogue { HRV_EPI_LINEAR = 0, HRV_EPI_SPADE = 1 };
@@ -66,6 +74,12 @@ typedef struct hrv_tensor {
  *
  * One kernel (pixels as M, 64 or 128 output channels as N, K walked tap by tap in 64-channel blocks) runs every case; results are
  * bit-identical from launch to launch.
+ *
+ * fp32 storage: with in.dtype == HRV_F32 the call runs the 3xTF32 kernel (K walked in 32-channel blocks; every operand split into
+ * hi = rna_tf32(v) and lo = rna_tf32(v - hi), products hi*hi + hi*lo + lo*hi summed in fp32: fp32-class accuracy).  wpack is then
+ * the fp32 [2][kh*kw][n_pad][cin_k] operand of hrv_pack_conv_weight_tf32x2; out, res, x0 and x1 must be fp32 (HRV_EINVAL otherwise),
+ * NHWC outputs with room in their pitch write the pad channels up to the next multiple of 8 as in 16-bit storage, and the training-only
+ * gate res_modes and gamma_out are refused (HRV_EUNSUPPORTED).
  */
 typedef struct hrv_conv_params {
   hrv_tensor in;
@@ -100,7 +114,7 @@ int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream);
  * the (virtual) tensor  cat(up2^x0_shift(x0), x1)  — nn.InstanceNorm2d(affine=False) statistics
  * (network_generator.py:86,110; biased variance, eps inside the sqrt) without materialising the sum,
  * the up-sampling or the concatenation.  h,w = statistics extent.  workspace: 2*N*C doubles, zeroed by
- * the call.  Writes mean[N][C], rstd[N][C]. */
+ * the call.  Writes mean[N][C], rstd[N][C].  fp32 storage: x0/x1 may be fp32 (both). */
 int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w,
                        const float* noise, const float* noise_scale, float eps,
                        float* mean, float* rstd, void* workspace, size_t workspace_bytes, hrv_stream stream);
@@ -108,13 +122,13 @@ int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor*
 /* The same statistics for up to TWO norms that share the input but draw their own noise (norm_s and norm_0 of a SPADEResBlock,
  * network_generator.py:160-170), from ONE pass over the SOURCE tensors: x0 is read at its own (half) resolution, the noise enters
  * through the sums {sum nz, sum nz^2, sum x*nz} (see csrc/aux_kernels.cu).  noise1 / mean1 / rstd1 may be NULL (one norm).
- * workspace: (4*N*C + 4*N) doubles. */
+ * workspace: (4*N*C + 4*N) doubles.  fp32 storage: x0/x1 may be fp32 (both). */
 int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w, const float* noise0,
                         const float* noise_scale0, const float* noise1, const float* noise_scale1, float eps, float* mean0,
                         float* rstd0, float* mean1, float* rstd1, void* workspace, size_t workspace_bytes, hrv_stream stream);
 
 /* y = act((x - mean[n,c]) * rstd[n,c]) elementwise on an NHWC bf16 tensor (InstanceNorm + LeakyReLU of the
- * discriminators, network_generator.py:269-270,427; networks.py:366-386). In place allowed. */
+ * discriminators, network_generator.py:269-270,427; networks.py:366-386). In place allowed.  fp32 storage: x and y fp32. */
 int hrv_instnorm_apply(const hrv_tensor* x, const float* mean, const float* rstd, int32_t act,
                        const hrv_tensor* y, hrv_stream stream);
 
@@ -159,7 +173,7 @@ int hrv_act_bwd_bias(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, con
 
 /* fp32 NCHW -> bf16 NHWC with nearest resampling to (dst.h, dst.w): src index = floor(dst*in/out)
  * (F.interpolate(mode='nearest'), network_generator.py:164,222) and zero fill of dst channels >= C.
- * src: [n][c][src_h][src_w] fp32 contiguous. */
+ * src: [n][c][src_h][src_w] fp32 contiguous.  fp32 storage: dst may be fp32 NHWC. */
 int hrv_nchw_to_nhwc(const float* src, int32_t c, int32_t src_h, int32_t src_w, const hrv_tensor* dst, hrv_stream stream);
 
 /* bf16|f32 NHWC view -> fp32 NCHW contiguous [n][c][h][w]. */
@@ -168,15 +182,15 @@ int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream);
 /* Space-to-depth by 2 with zero fill of odd edges: dst[n,Y,X,(py*2+px)*src.c + ci] = src[n,2Y+py,2X+px,ci];
  * dst.h = ceil(src.h/2), dst.w = ceil(src.w/2), dst.c >= 4*src.c (extra channels zeroed). Turns the
  * stride-2 convolutions (networks.py:185; network_generator.py:263-269; networks.py:360-372) into stride-1
- * 2x2 implicit GEMMs. */
+ * 2x2 implicit GEMMs.  fp32 storage: src and dst fp32. */
 int hrv_space_to_depth(const hrv_tensor* src, const hrv_tensor* dst, hrv_stream stream);
 
 /* F.avg_pool2d(3, stride 2, pad 1, count_include_pad=False) on NHWC bf16 (network_generator.py:302,
- * networks.py:320). dst.h = (src.h-1)/2+1. */
+ * networks.py:320). dst.h = (src.h-1)/2+1.  fp32 storage: src and dst fp32. */
 int hrv_avgpool3s2(const hrv_tensor* src, const hrv_tensor* dst, hrv_stream stream);
 
 /* dst = bilinear_up2(a) (+ b), align_corners=False (F.interpolate / nn.Upsample, networks.py:130,181).
- * a: (n,h,w,c) bf16; b (optional, ptr NULL = none) and dst: (n,2h,2w,c) bf16. */
+ * a: (n,h,w,c) bf16; b (optional, ptr NULL = none) and dst: (n,2h,2w,c) bf16.  fp32 storage: a, b and dst fp32. */
 int hrv_bilinear_up2_add(const hrv_tensor* a, const hrv_tensor* b, const hrv_tensor* dst, hrv_stream stream);
 
 /* The appearance-flow warp (networks.py:133-135,147-152,161-168) in one kernel:
@@ -249,7 +263,8 @@ int hrv_flow_warp_nchw(const float* flow_lo, int32_t n, int32_t hl, int32_t wl, 
 
 /* im2col for tiny-Cin convolutions: dst[n,y,x, (ky*kw+kx)*src.c + ci] = src[n, y+ky-pad, x+kx-pad, ci], zero outside the image
  * and in channels >= kh*kw*src.c.  Lets SPADE's 3x3 mlp_shared convolution over the 7-channel label map
- * (network_generator.py:182-184) run as a single K=64 GEMM block (hrv_conv2d_fwd with kh=kw=1) and its weight gradient as a 1x1. */
+ * (network_generator.py:182-184) run as a single K=64 GEMM block (hrv_conv2d_fwd with kh=kw=1) and its weight gradient as a 1x1.
+ * fp32 storage: src and dst fp32. */
 int hrv_im2col(const hrv_tensor* src, const hrv_tensor* dst, int32_t kh, int32_t kw, int32_t pad, hrv_stream stream);
 
 /* L1 feature loss (VGGLoss, networks.py:244-251): *sum = sum |a - b| over the views (fp64); da = sign(a - b) * (*gscale)
@@ -263,6 +278,12 @@ int hrv_l1_bwd(const hrv_tensor* a, const hrv_tensor* b, const float* gscale, co
  * K = output channels, taps mirrored).  inv_scale (optional, device scalar) multiplies every element (1/sigma of spectral norm). */
 int hrv_pack_conv_weight(const float* w0, const float* w1, int32_t cout, int32_t cin, int32_t kh, int32_t kw,
                          int32_t transpose_flip, const float* inv_scale, void* dst, int32_t n_pad, int32_t cin_k, hrv_stream stream);
+
+/* The weight operand of hrv_conv2d_fwd on fp32 storage, same arguments and element mapping as hrv_pack_conv_weight: dst is fp32
+ * [2][kh*kw][n_pad][cin_k], plane 0 = hi = rna_tf32(v), plane 1 = lo = rna_tf32(v - hi) (rna = round to nearest, ties away). */
+int hrv_pack_conv_weight_tf32x2(const float* w0, const float* w1, int32_t cout, int32_t cin, int32_t kh, int32_t kw,
+                                int32_t transpose_flip, const float* inv_scale, void* dst, int32_t n_pad, int32_t cin_k,
+                                hrv_stream stream);
 
 /* Library / device introspection. */
 const char* hrv_last_error(void);
