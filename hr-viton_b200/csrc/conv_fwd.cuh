@@ -1,0 +1,378 @@
+// conv_fwd.cuh — what the two forward convolution kernels share: conv_wgmma_kernel (conv_igemm.cu, 16-bit storage) and
+// conv_tf32x3_kernel (conv_f32.cu, fp32 storage).  Both are NHWC implicit GEMMs with the same tiling and warp roles:
+//
+//   GEMM view:  M = output pixels (128 per tile = TN x TH x TW box), N = output channels (BNT = 64 or 128 per tile),
+//               K = taps x input channels, walked tap by tap in K blocks of one 128-byte SWIZZLE_128B row per pixel (64 16-bit or
+//               32 fp32 channels).
+//   A operand:  one TMA 4-D box {K block, TW, TH, TN} of the NHWC input per (tap, K block), shifted by the tap offset; TMA zero-fills
+//               out-of-range pixels (= the convolution's zero padding) and channels past the input's or the packed weight's channel
+//               count, so every layer runs on full K blocks whatever block size its weights were packed with.
+//   B operand:  one TMA box {K block, BNT} per weight plane of the packed weights [planes][taps][n_pad][cin_k] (K-major); rows past
+//               n_pad are zero fill.
+//   Pipeline:   warp 8 = TMA producer, warpgroups 0 / 1 = consumers for pixels 0-63 / 64-127 of the tile.  A ring of `stages`
+//               (A + B) stages with full (transaction count) / empty (one arrival per consumer warp) mbarriers.
+//   Epilogues:  straight from the wgmma accumulator fragment.
+//               LINEAR  out = act(acc*scale + shift (+ residual))      (bias / folded BatchNorm / residual / tanh)
+//               SPADE   out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta), gamma/beta = interleaved GEMM columns: a thread's
+//                       accumulator pair (2j, 2j+1) is (gamma, beta) of one channel, so the SPADE modulation never leaves registers
+//                       (network_generator.py:115-121,170-171).
+//               The gate residual modes and gamma_out serve the backward pass and exist on 16-bit storage only.
+//
+// Shared memory of a CTA: 1 KB of mbarriers (full at +0, empty at +128), then `scratch` bytes the kernel owns, then the stage ring.
+#pragma once
+#include "hrv_host.h"
+#include "hrv_ptx.cuh"
+
+namespace hrv {
+
+constexpr int kConvConsumers = 2;                        // consumer warpgroups (64 pixels each)
+constexpr int kConvThreads = 128 * kConvConsumers + 32;  // + one producer warp
+constexpr uint32_t kConvRowBytes = 128;                  // one K block of one pixel / weight row: one SWIZZLE_128B row
+constexpr uint32_t kConvABytes = 128 * kConvRowBytes;    // 128 pixels
+
+// T = activation storage: __nv_bfloat16 (__half in the fp16 flavour) or float.
+template <typename T>
+constexpr bool kStorage16 = sizeof(T) == 2;
+
+template <typename T>
+struct alignas(64) ConvArgs {
+  CUtensorMap tmA;
+  CUtensorMap tmB;
+  int Nimg, Hout, Wout;
+  int tw_log, th_log;
+  int tiles_x, tiles_y, tiles_n;
+  int KH, KW, off_y, off_x, chunks;
+  int stages, n_gemm;
+  int epi, act;
+  const float* scale;
+  const float* shift;
+  void* out;                       // T NHWC; on 16-bit storage also fp32 NHWC / NCHW
+  int out_pitch, out_dtype, out_layout, out_c;
+  int store_c;                     // LINEAR writes channels [0, store_c): out_c, or up to the next multiple of 8 (pad channels)
+  const void* res;                 // T NHWC; on 16-bit storage also fp32 NHWC
+  int res_pitch, res_dtype, res_c;  // an fp32 residual is added to channels [0, res_c)
+  int res_mode;                    // 0 add, 1 ReLU gate, 2 LeakyReLU(0.2) gate (16-bit res only)
+  const T* x0;
+  int x0_c, x0_pitch, x0_shift;
+  const T* x1;
+  int x1_pitch;
+  const float* mean;
+  const float* rstd;
+  const float* noise;
+  const float* noise_scale;
+  int C_mod;
+  T* gamma_out;                    // 16-bit storage only
+  int gamma_pitch;
+};
+
+// Tile of one CTA (N tile, pixel tile (x, y), image group) and the 1024-byte aligned start of its shared memory.
+struct ConvTile {
+  int nt, tx, ty, ti;
+  uint32_t bars;
+};
+
+// Decodes the CTA's tile and initialises the barrier ring; every thread of the CTA calls it.
+template <typename T>
+__device__ __forceinline__ ConvTile conv_prologue(const ConvArgs<T>& a) {
+  extern __shared__ uint8_t smem_raw[];
+  ConvTile t;
+  t.bars = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  t.nt = blockIdx.x % a.tiles_n;
+  int mt = blockIdx.x / a.tiles_n;
+  t.tx = mt % a.tiles_x;
+  mt /= a.tiles_x;
+  t.ty = mt % a.tiles_y;
+  t.ti = mt / a.tiles_y;
+  const int S = a.stages;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(bar_full(t.bars, s), 1);
+      mbar_init(bar_empty(t.bars, s), 4 * kConvConsumers);  // one arrival per consumer warp
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  return t;
+}
+
+// TMA producer (one lane): per K step one A box of KB channels and the B box of PLANES weight planes into the next stage.
+template <int BNT, int KB, int PLANES, typename T>
+__device__ __forceinline__ void conv_produce(const ConvArgs<T>& a, const ConvTile& t, uint32_t stage0) {
+  constexpr uint32_t STAGE = kConvABytes + PLANES * (uint32_t)BNT * kConvRowBytes;
+  tma_prefetch_desc(&a.tmA);
+  tma_prefetch_desc(&a.tmB);
+  const int KT = a.KH * a.KW * a.chunks;
+  const int x0 = (t.tx << a.tw_log) - a.off_x;
+  const int y0 = (t.ty << a.th_log) - a.off_y;
+  const int n0 = t.ti << (7 - a.tw_log - a.th_log);
+  int ky = 0, kx = 0, kc = 0, tap = 0;
+  StageRing ring(stage0, STAGE, a.stages);
+  for (int k = 0; k < KT; ++k) {
+    const uint32_t full = bar_full(t.bars, ring.stage);
+    mbar_wait(bar_empty(t.bars, ring.stage), ring.phase ^ 1u);
+    mbar_arrive_expect_tx(full, STAGE);
+    tma_load_4d(ring.addr, &a.tmA, full, kc * KB, x0 + kx, y0 + ky, n0);
+    if constexpr (PLANES == 1) tma_load_3d(ring.addr + kConvABytes, &a.tmB, full, kc * KB, t.nt * BNT, tap);
+    else tma_load_4d(ring.addr + kConvABytes, &a.tmB, full, kc * KB, t.nt * BNT, tap, 0);  // all planes in one box
+    if (++kc == a.chunks) {
+      kc = 0;
+      ++tap;
+      if (++kx == a.KW) { kx = 0; ++ky; }
+    }
+    ring.next();
+  }
+}
+
+// One output pixel as seen by an epilogue thread.
+struct EpiPix {
+  int x, y, n;
+  bool valid;
+  long long pix;
+};
+
+__device__ __forceinline__ float ld_act(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld_act(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void st_act(float* p, float v) { *p = v; }
+__device__ __forceinline__ void st_act(__nv_bfloat16* p, float v) { *p = __float2bfloat16(v); }
+
+// LINEAR epilogue of two adjacent GEMM columns (c, c+1) of one pixel: out = act(acc*scale + shift (+ res | * act'(res))).
+template <typename T>
+__device__ __forceinline__ void epi_linear2(const ConvArgs<T>& a, const EpiPix& p, int c, float v0, float v1) {
+  if (!p.valid || c >= a.store_c) return;
+  float f[2] = {v0, v1};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int j = c + i;
+    const bool in = j < a.n_gemm;
+    const float sc = in ? (a.scale ? __ldg(a.scale + j) : 1.f) : 0.f;
+    const float sh = (in && a.shift) ? __ldg(a.shift + j) : 0.f;
+    f[i] = fmaf(f[i], sc, sh);
+  }
+  if (a.res) {
+    bool res16 = false;
+    if constexpr (kStorage16<T>) {
+      res16 = a.res_dtype == HRV_BF16;
+      if (res16) {
+        const uint32_t rv = __ldg(reinterpret_cast<const unsigned int*>(static_cast<const T*>(a.res) + p.pix * a.res_pitch + c));
+        const float rf[2] = {bf16_lo(rv), bf16_hi(rv)};
+        if (a.res_mode == 0) {
+          f[0] += rf[0]; f[1] += rf[1];
+        } else {  // activation backward of the layer below, fused: multiply by act'(its saved output)
+          const float slope = a.res_mode == 1 ? 0.f : 0.2f;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) f[i] = rf[i] > 0.f ? f[i] : f[i] * slope;
+        }
+      }
+    }
+    if (!res16) {
+      const float* rp = static_cast<const float*>(a.res) + p.pix * a.res_pitch + c;
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        if (c + i < a.res_c) f[i] += __ldg(rp + i);
+    }
+  }
+  f[0] = apply_act(f[0], a.act);
+  f[1] = apply_act(f[1], a.act);
+  if constexpr (kStorage16<T>) {
+    if (a.out_dtype == HRV_BF16) {  // c even, pitch % 8 == 0: a 4-byte store
+      *reinterpret_cast<uint32_t*>(static_cast<T*>(a.out) + p.pix * a.out_pitch + c) = pack_bf16(f[0], f[1]);
+      return;
+    }
+  }
+  float* const out = static_cast<float*>(a.out);
+  if (a.out_layout == HRV_NHWC) {
+    float* op = out + p.pix * a.out_pitch + c;
+    op[0] = f[0];
+    if (c + 1 < a.store_c) op[1] = f[1];
+  } else {
+    const long long hw = (long long)a.Hout * a.Wout;
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      if (c + i < a.out_c) out[((long long)p.n * a.out_c + c + i) * hw + (long long)p.y * a.Wout + p.x] = f[i];
+  }
+}
+
+// SPADE epilogue of one channel ch of one pixel; g, b = the (gamma, beta) accumulators of columns 2ch, 2ch+1.
+template <typename T>
+__device__ __forceinline__ void epi_spade1(const ConvArgs<T>& a, const EpiPix& p, long long pix0, float nz, int ch, float g, float b) {
+  if (!p.valid || ch >= a.C_mod) return;
+  const float xs = ld_act((ch < a.x0_c) ? (a.x0 + pix0 * a.x0_pitch + ch) : (a.x1 + p.pix * a.x1_pitch + (ch - a.x0_c)));
+  const float mu = __ldg(a.mean + (long long)p.n * a.C_mod + ch);
+  const float rs = __ldg(a.rstd + (long long)p.n * a.C_mod + ch);
+  const float ns = a.noise_scale ? __ldg(a.noise_scale + ch) : 0.f;
+  const float gm = g + (a.shift ? __ldg(a.shift + 2 * ch) : 0.f);
+  const float bt = b + (a.shift ? __ldg(a.shift + 2 * ch + 1) : 0.f);
+  const float xn = (fmaf(nz, ns, xs) - mu) * rs;
+  const float o = apply_act(fmaf(xn, 1.f + gm, bt), a.act);
+  if constexpr (kStorage16<T>) {
+    if (a.gamma_out) st_act(a.gamma_out + p.pix * a.gamma_pitch + ch, gm);  // training: gamma for the backward pass
+  }
+  st_act(static_cast<T*>(a.out) + p.pix * a.out_pitch + ch, o);
+}
+
+// Epilogue of consumer warpgroup wg from its accumulators.  wgmma m64nN fragment: thread (warp w, lane l) holds rows
+// 16 (w % 4) + l / 4 and that + 8, columns 8 j + 2 (l % 4) + {0, 1}.
+template <int BNT, typename T>
+__device__ __forceinline__ void conv_epilogue(const ConvArgs<T>& a, const ConvTile& t, const float (&acc)[BNT / 2]) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
+  const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
+  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int n_base = t.nt * BNT + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = r_base + 8 * h;
+    EpiPix p;
+    p.x = (t.tx << a.tw_log) + (r & tw_mask);
+    p.y = (t.ty << a.th_log) + ((r >> a.tw_log) & th_mask);
+    p.n = (t.ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
+    p.valid = (p.x < a.Wout) && (p.y < a.Hout) && (p.n < a.Nimg);
+    p.pix = ((long long)p.n * a.Hout + p.y) * a.Wout + p.x;
+    if (a.epi == 0) {
+#pragma unroll
+      for (int j = 0; j < BNT / 8; ++j) epi_linear2(a, p, n_base + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    } else {
+      const int sh0 = a.x0_shift;
+      const long long pix0 = ((long long)p.n * (a.Hout >> sh0) + (p.y >> sh0)) * (a.Wout >> sh0) + (p.x >> sh0);
+      const float nz = (p.valid && a.noise) ? __ldg(a.noise + p.pix) : 0.f;
+#pragma unroll
+      for (int j = 0; j < BNT / 8; ++j) epi_spade1(a, p, pix0, nz, (n_base + 8 * j) >> 1, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ host side
+
+// What a kernel supplies to the shared host setup.
+struct ConvBudget {
+  uint32_t smem;     // dynamic shared memory one CTA may use
+  int max_stages;
+  uint32_t scratch;  // bytes between the barriers and the stage ring
+  int kblock;        // K-block width in channels
+  int planes;        // weight planes per stage
+};
+
+// Validates `p` for storage T, picks the tiling, sizes the stage ring, encodes both tensor maps and launches kKernel64 or kKernel128
+// (the kernel's instances for N tiles of 64 / 128 columns).  Errors are prefixed "conv" / "conv(spade)" on 16-bit storage and
+// "conv(fp32)" / "conv(fp32 spade)" on fp32 storage.
+template <typename T, auto kKernel64, auto kKernel128>
+int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* name, hrv_stream stream) {
+  constexpr bool f32 = !kStorage16<T>;
+  constexpr int storage = f32 ? HRV_F32 : HRV_BF16;
+  const char* const pre = f32 ? "conv(fp32)" : "conv";
+  const char* const spre = f32 ? "conv(fp32 spade)" : "conv(spade)";
+  const hrv_tensor& in = p->in;
+  const hrv_tensor& out = p->out;
+  if (((uintptr_t)in.ptr & 15) || (in.pitch % 8) || in.pitch < in.c)
+    return set_error(HRV_EINVAL, "%s: input needs 16-byte aligned ptr and pitch %% 8 == 0 (pitch=%d c=%d)", pre, in.pitch, in.c);
+  if (p->bk != 64 && p->bk != 32 && p->bk != 16) return set_error(HRV_EINVAL, "%s: bk must be 64/32/16", pre);
+  if (p->bn < 16 || p->bn > 256 || (p->bn % 16)) return set_error(HRV_EINVAL, "%s: bn=%d must be a multiple of 16 in [16,256]", pre, p->bn);
+  if (p->kh < 1 || p->kw < 1 || p->n_gemm < 1) return set_error(HRV_EINVAL, "%s: bad kh/kw/n_gemm", pre);
+  if (out.n != in.n) return set_error(HRV_EINVAL, "%s: batch mismatch", pre);
+  if (((uintptr_t)p->wpack & 15)) return set_error(HRV_EINVAL, "%s: wpack must be 16-byte aligned", pre);
+  if (!(out.dtype == storage || (!f32 && out.dtype == HRV_F32)) || !out.ptr || ((uintptr_t)out.ptr & 3))
+    return set_error(HRV_EINVAL, "%s: the output must be non-null and %s", pre, f32 ? "fp32 (one storage type per call)" : "bf16 or fp32");
+  if (p->out_layout != HRV_NHWC && p->out_layout != HRV_NCHW) return set_error(HRV_EINVAL, "%s: out_layout %d", pre, p->out_layout);
+  if (out.dtype == HRV_BF16 && (p->out_layout != HRV_NHWC || ((uintptr_t)out.ptr & 15) || (out.pitch % 8)))
+    return set_error(HRV_EINVAL, "%s: bf16 output must be NHWC, 16-byte aligned, pitch %% 8 == 0", pre);
+  const int res_mode = p->res.ptr ? p->res_mode : 0;
+  if (p->res.ptr) {
+    if (!(p->res.dtype == storage || (!f32 && p->res.dtype == HRV_F32)))
+      return set_error(HRV_EINVAL, "%s: the residual must be %s", pre, f32 ? "fp32 (one storage type per call)" : "bf16 or fp32");
+    if (p->res.dtype == HRV_BF16 && (((uintptr_t)p->res.ptr & 15) || (p->res.pitch % 8)))
+      return set_error(HRV_EINVAL, "%s: bf16 residual must be 16-byte aligned with pitch %% 8 == 0", pre);
+  }
+  if (res_mode < 0 || res_mode > 2) return set_error(HRV_EINVAL, "%s: res_mode %d", pre, res_mode);
+  if (f32 && res_mode)
+    return set_error(HRV_EUNSUPPORTED, "%s: the gate residual modes belong to the backward pass; fp32 storage is inference-only", pre);
+  if (res_mode && (p->res.dtype != HRV_BF16 || out.dtype != HRV_BF16 || p->out_layout != HRV_NHWC || p->epi != HRV_EPI_LINEAR ||
+                   p->act != HRV_ACT_NONE))
+    return set_error(HRV_EINVAL, "%s: gate modes need a bf16 res, a bf16 NHWC output, the LINEAR epilogue and no activation", pre);
+
+  ConvArgs<T> a;
+  memset(&a, 0, sizeof(a));
+  a.Nimg = out.n; a.Hout = out.h; a.Wout = out.w;
+  // N tile: 64 columns for narrow GEMMs, else 128 (a 64 x 128 fp32 accumulator is 64 registers per thread).  Independent of the
+  // packing's bn: the weight map's row extent is the packed n_pad, rows past it are zero fill.
+  const int bnt = p->n_gemm <= 64 ? 64 : 128;
+  const int TW = pick_pow2(out.w, 128);
+  const int TH = pick_pow2(out.h, 128 / TW);
+  const int TN = 128 / (TW * TH);
+  a.tw_log = log2i(TW); a.th_log = log2i(TH);
+  a.tiles_x = (out.w + TW - 1) / TW;
+  a.tiles_y = (out.h + TH - 1) / TH;
+  const int tiles_img = (out.n + TN - 1) / TN;
+  a.tiles_n = (p->n_gemm + bnt - 1) / bnt;
+  a.KH = p->kh; a.KW = p->kw; a.off_y = p->off_y; a.off_x = p->off_x;
+  a.chunks = (in.c + budget.kblock - 1) / budget.kblock;
+  a.n_gemm = p->n_gemm;
+  a.epi = p->epi; a.act = p->act;
+  a.scale = p->scale; a.shift = p->shift;
+  a.out = out.ptr; a.out_pitch = out.pitch; a.out_dtype = out.dtype; a.out_layout = p->out_layout; a.out_c = out.c;
+  // NHWC outputs in the storage type carry pad channels up to the next multiple of 8: written as act(0) (+ res) where the pitch has
+  // room.  Other outputs stop at out_c.
+  const int c8 = (out.c + 7) & ~7;
+  a.store_c = (p->out_layout == HRV_NHWC && out.dtype == storage && out.pitch >= c8) ? c8 : out.c;
+  if (p->res.ptr) {
+    a.res = p->res.ptr; a.res_pitch = p->res.pitch; a.res_dtype = p->res.dtype; a.res_mode = res_mode;
+    a.res_c = (p->res.dtype == storage && p->res.pitch >= a.store_c) ? a.store_c : out.c;
+  }
+
+  if (p->epi == HRV_EPI_SPADE) {
+    const int C = p->x0.c + (p->x1.ptr ? p->x1.c : 0);
+    if (p->n_gemm != 2 * C) return set_error(HRV_EINVAL, "%s: n_gemm=%d must equal 2*(x0.c+x1.c)=%d", spre, p->n_gemm, 2 * C);
+    if (p->x0.dtype != storage || (p->x1.ptr && p->x1.dtype != storage))
+      return set_error(HRV_EINVAL, "%s: x0/x1 must be %s (one storage type per call)", spre, f32 ? "fp32" : "bf16");
+    if (f32 && p->gamma_out.ptr)
+      return set_error(HRV_EUNSUPPORTED, "%s: gamma_out belongs to the backward pass; fp32 storage is inference-only", spre);
+    if ((p->x0.c % 8) || (C % 8) || out.dtype != storage || p->out_layout != HRV_NHWC || !p->mean || !p->rstd || !p->x0.ptr)
+      return set_error(HRV_EINVAL, "%s: channel counts must be multiples of 8, output %s NHWC, mean/rstd/x0 set", spre, f32 ? "fp32" : "bf16");
+    if (((uintptr_t)p->x0.ptr & 15) || (p->x0.pitch % 8) || (p->x1.ptr && (((uintptr_t)p->x1.ptr & 15) || (p->x1.pitch % 8))))
+      return set_error(HRV_EINVAL, "%s: x0/x1 alignment", spre);
+    if (p->x0_shift && ((out.h & 1) || (out.w & 1) || p->x0.h * 2 != out.h || p->x0.w * 2 != out.w))
+      return set_error(HRV_EINVAL, "%s: x0_shift needs x0 at exactly half resolution", spre);
+    if (!p->x0_shift && (p->x0.h != out.h || p->x0.w != out.w)) return set_error(HRV_EINVAL, "%s: x0 extent mismatch", spre);
+    if (out.c != C) return set_error(HRV_EINVAL, "%s: out.c must equal C", spre);
+    a.x0 = (const T*)p->x0.ptr; a.x0_c = p->x0.c; a.x0_pitch = p->x0.pitch; a.x0_shift = p->x0_shift ? 1 : 0;
+    a.x1 = (const T*)p->x1.ptr; a.x1_pitch = p->x1.pitch;
+    a.mean = p->mean; a.rstd = p->rstd; a.noise = p->noise; a.noise_scale = p->noise_scale; a.C_mod = C;
+    if (p->gamma_out.ptr) {
+      if (p->gamma_out.dtype != HRV_BF16 || ((uintptr_t)p->gamma_out.ptr & 15) || (p->gamma_out.pitch % 8) || p->gamma_out.c != C)
+        return set_error(HRV_EINVAL, "%s: gamma_out must be bf16 (n,h,w,C), 16-byte aligned", spre);
+      a.gamma_out = (T*)p->gamma_out.ptr; a.gamma_pitch = p->gamma_out.pitch;
+    }
+  } else if (p->epi != HRV_EPI_LINEAR) {
+    return set_error(HRV_EINVAL, "%s: unknown epilogue %d", pre, p->epi);
+  }
+
+  // ---- pipeline: as many stages as fit in the budget next to the scratch, at most one per K step
+  const uint32_t stage_bytes = kConvABytes + (uint32_t)(budget.planes * bnt) * kConvRowBytes;
+  const int KT = p->kh * p->kw * a.chunks;
+  int stages = (int)((budget.smem - 2048u - budget.scratch) / stage_bytes);
+  if (stages > budget.max_stages) stages = budget.max_stages;
+  if (stages > KT) stages = KT < 2 ? 2 : KT;
+  a.stages = stages;
+  const size_t smem = 2048 + budget.scratch + (size_t)stages * stage_bytes;  // 1 KB alignment slack + 1 KB of barriers
+
+  // ---- tensor maps: the input, and the packed weights [planes][taps][n_pad][cin_k] as laid out for this (bk, bn)
+  int rc = encode_nhwc_map(&a.tmA, in, budget.kblock, TW, TH, TN);
+  if (rc) return rc;
+  const cuuint64_t elem = sizeof(T);
+  const cuuint64_t cin_k = (cuuint64_t)((in.c + p->bk - 1) / p->bk) * p->bk;
+  const cuuint64_t n_pad = (cuuint64_t)((p->n_gemm + p->bn - 1) / p->bn) * p->bn;
+  const cuuint64_t taps = (cuuint64_t)(p->kh * p->kw);
+  const cuuint64_t dims[4] = {cin_k, n_pad, taps, (cuuint64_t)budget.planes};
+  const cuuint64_t strides[3] = {cin_k * elem, n_pad * cin_k * elem, taps * n_pad * cin_k * elem};
+  const cuuint32_t box[4] = {(cuuint32_t)budget.kblock, (cuuint32_t)bnt, 1, (cuuint32_t)budget.planes};
+  const cuuint32_t es[4] = {1, 1, 1, 1};
+  rc = encode_tensor_map(&a.tmB, budget.planes == 1 ? 3 : 4, const_cast<void*>(p->wpack), dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B,
+                         f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+  if (rc) return rc;
+
+  const long long total = (long long)a.tiles_n * a.tiles_x * a.tiles_y * tiles_img;
+  if (total > 0x7FFFFFFFLL) return set_error(HRV_EINVAL, "%s: too many tiles", pre);
+  cudaStream_t st = (cudaStream_t)stream;
+  return bnt == 64 ? launch_dyn_smem<kKernel64>(name, (int)total, kConvThreads, smem, budget.smem, st, a)
+                   : launch_dyn_smem<kKernel128>(name, (int)total, kConvThreads, smem, budget.smem, st, a);
+}
+
+}  // namespace hrv

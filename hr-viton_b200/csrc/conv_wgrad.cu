@@ -53,8 +53,6 @@ template <int BN>
 __global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_constant__ WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  auto bar_full = [&](int s) { return base + 8u * s; };
-  auto bar_empty = [&](int s) { return base + 128u + 8u * s; };
   constexpr uint32_t kBlk = kPX * 128u;                                     // one 64-channel block of kPX pixel rows: 8 KB
   constexpr uint32_t stage_bytes = kBlk * (2u + BN / 64);                  // dY: co blocks 0, 1; X: BN / 64 ci blocks
   const uint32_t stage0 = base + 1024u;
@@ -73,7 +71,7 @@ __global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_
   const int my_chunks = (chunks_total - split + a.splits - 1) / a.splits;  // chunks split, split+splits, ...
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(bar_full(s), 1); mbar_init(bar_empty(s), 8); }  // one arrival per consumer warp
+    for (int s = 0; s < S; ++s) { mbar_init(bar_full(base, s), 1); mbar_init(bar_empty(base, s), 8); }  // one arrival per consumer warp
     fence_mbar_init();
   }
   __syncthreads();
@@ -83,22 +81,21 @@ __global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_
     if (lane == 0) {
       tma_prefetch_desc(&a.tmDY);
       tma_prefetch_desc(&a.tmX);
-      int st = 0;
-      uint32_t ph = 0, sa = stage0;
+      StageRing ring(stage0, stage_bytes, S);
       int c = split;
       for (int i = 0; i < my_chunks; ++i, c += a.splits) {
         const int xs = c % a.xsegs;
         int r = c / a.xsegs;
         const int y = r % a.OH;
         const int n = r / a.OH;
-        mbar_wait(bar_empty(st), ph ^ 1u);
-        mbar_arrive_expect_tx(bar_full(st), stage_bytes);
-        tma_load_4d(sa, &a.tmDY, bar_full(st), m0, xs * kPX, y, n);
-        tma_load_4d(sa + kBlk, &a.tmDY, bar_full(st), m0 + 64, xs * kPX, y, n);
+        const uint32_t full = bar_full(base, ring.stage), sa = ring.addr;
+        mbar_wait(bar_empty(base, ring.stage), ring.phase ^ 1u);
+        mbar_arrive_expect_tx(full, stage_bytes);
+        tma_load_4d(sa, &a.tmDY, full, m0, xs * kPX, y, n);
+        tma_load_4d(sa + kBlk, &a.tmDY, full, m0 + 64, xs * kPX, y, n);
         for (int b = 0; b < BN / 64; ++b)
-          tma_load_4d(sa + (2u + b) * kBlk, &a.tmX, bar_full(st), n0 + 64 * b, xs * kPX - a.pad + kx, y + ky - a.pad, n);
-        sa += stage_bytes;
-        if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
+          tma_load_4d(sa + (2u + b) * kBlk, &a.tmX, full, n0 + 64 * b, xs * kPX - a.pad + kx, y + ky - a.pad, n);
+        ring.next();
       }
     }
     return;
@@ -111,26 +108,24 @@ __global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   {
-    int st = 0, prev = 0;
-    uint32_t ph = 0, sa = stage0;
+    StageRing ring(stage0, stage_bytes, S);
+    int prev = 0;
     for (int i = 0; i < my_chunks; ++i) {
-      mbar_wait(bar_full(st), ph);
+      mbar_wait(bar_full(base, ring.stage), ring.phase);
       wgmma_fence();
-      const uint32_t sdy = sa + (uint32_t)wg * kBlk, sx = sa + 2u * kBlk;
+      const uint32_t sdy = ring.addr + (uint32_t)wg * kBlk, sx = ring.addr + 2u * kBlk;
 #pragma unroll
       for (int kk = 0; kk < kPX / 16; ++kk) {  // 16 pixel rows per instruction
         const uint64_t da = make_wgmma_desc(sdy + kk * 2048u, 1024, 1, kBlk);
         const uint64_t db = make_wgmma_desc(sx + kk * 2048u, 1024, 1, kBlk);
         const uint32_t accf = (uint32_t)((i | kk) != 0);
-        if constexpr (BN == 128) wgmma_n128<1, 1>(acc, da, db, accf);
-        else wgmma_n64<1, 1>(acc, da, db, accf);
+        wgmma_nx<BN, 1, 1>(acc, da, db, accf);
       }
       wgmma_commit();
       wgmma_wait<1>();
-      if (i > 0 && lane == 0) mbar_arrive(bar_empty(prev));
-      prev = st;
-      sa += stage_bytes;
-      if (++st == S) { st = 0; ph ^= 1u; sa = stage0; }
+      if (i > 0 && lane == 0) mbar_arrive(bar_empty(base, prev));
+      prev = ring.stage;
+      ring.next();
     }
     wgmma_wait<0>();
     fence_regs(acc);
@@ -155,18 +150,6 @@ __global__ void __launch_bounds__(kWgThreads, 2) conv_wgrad_kernel(const __grid_
       }
     }
   }
-}
-
-template <int BN>
-static cudaError_t launch_wgrad(const WgradArgs& a, int grid, size_t smem, cudaStream_t st) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kWgSmem);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
-  conv_wgrad_kernel<BN><<<grid, kWgThreads, smem, st>>>(a);
-  return cudaGetLastError();
 }
 
 }  // namespace hrv
@@ -238,34 +221,23 @@ extern "C" int hrv_conv2d_wgrad(const hrv_tensor* x, const hrv_tensor* dy, int32
   int stages = (int)((kWgSmem - 2048u) / stage_bytes);
   if (stages > 16) stages = 16;
   a.stages = stages;
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)dy->c, (cuuint64_t)dy->w, (cuuint64_t)dy->h, (cuuint64_t)dy->n};
-    cuuint64_t strides[3] = {(cuuint64_t)dy->pitch * 2, (cuuint64_t)dy->w * dy->pitch * 2, (cuuint64_t)dy->h * dy->w * dy->pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)kPX, 1, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    int rc = encode_tensor_map(&a.tmDY, 4, dy->ptr, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
-  {
-    cuuint64_t dims[4] = {(cuuint64_t)x->c, (cuuint64_t)x->w, (cuuint64_t)x->h, (cuuint64_t)x->n};
-    cuuint64_t strides[3] = {(cuuint64_t)x->pitch * 2, (cuuint64_t)x->w * x->pitch * 2, (cuuint64_t)x->h * x->w * x->pitch * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)kPX, 1, 1};
-    cuuint32_t es[4] = {1, 1, 1, 1};
-    int rc = encode_tensor_map(&a.tmX, 4, x->ptr, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
+  int rc = encode_nhwc_map(&a.tmDY, *dy, 64, kPX, 1, 1);
+  if (!rc) rc = encode_nhwc_map(&a.tmX, *x, 64, kPX, 1, 1);
+  if (rc) return rc;
   const size_t smem = 2048 + (size_t)stages * stage_bytes;
   const int grid = tiles * splits;
-  cudaError_t e = a.BN == 128 ? launch_wgrad<128>(a, grid, smem, (cudaStream_t)stream) : launch_wgrad<64>(a, grid, smem, (cudaStream_t)stream);
-  if (e != cudaSuccess) return set_error(HRV_ECUDA, "conv_wgrad launch: %s", cudaGetErrorString(e));
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = a.BN == 128 ? launch_dyn_smem<conv_wgrad_kernel<128>>("conv_wgrad", grid, kWgThreads, smem, kWgSmem, st, a)
+                   : launch_dyn_smem<conv_wgrad_kernel<64>>("conv_wgrad", grid, kWgThreads, smem, kWgSmem, st, a);
+  if (rc) return rc;
   if (splits > 1) {
     if ((dw_elems % 4) || ((uintptr_t)dw & 15)) {  // slabs not 16-byte aligned: scalar reduction (tiny layers, e.g. 13 -> 13 channels)
-      wgrad_reduce1_kernel<<<(unsigned)((dw_elems + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float*)workspace, dw, dw_elems, splits);
+      wgrad_reduce1_kernel<<<(unsigned)((dw_elems + 255) / 256), 256, 0, st>>>((const float*)workspace, dw, dw_elems, splits);
     } else {
       const long long n4 = dw_elems / 4;
-      wgrad_reduce_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float*)workspace, dw, n4, n4, splits);
+      wgrad_reduce_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, st>>>((const float*)workspace, dw, n4, n4, splits);
     }
-    e = cudaGetLastError();
+    const cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(HRV_ECUDA, "wgrad_reduce launch: %s", cudaGetErrorString(e));
   }
   return HRV_OK;

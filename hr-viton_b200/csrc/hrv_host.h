@@ -20,6 +20,8 @@ int sm_count();
 int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
                       const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle,
                       CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+// 4-D SWIZZLE_128B map {c, w, h, n} of the NHWC tensor `t` (bf16 / fp16 or fp32 by t.dtype) with box {box_c, box_w, box_h, box_n}.
+int encode_nhwc_map(CUtensorMap* map, const hrv_tensor& t, int box_c, int box_w, int box_h, int box_n);
 // hrv_conv2d_fwd on fp32 storage (conv_f32.cu, compiled once): both flavours of hrv_conv2d_fwd hand an fp32 input to it.
 int conv2d_fwd_tf32x3(const hrv_conv_params* p, hrv_stream stream);
 
@@ -42,6 +44,21 @@ inline int pick_pow2(int dim, int cap) {
     }
   }
   return best;
+}
+
+// Launches `kKernel` with `smem` bytes of dynamic shared memory; the first call raises the kernel's limit to `smem_max`.
+template <auto kKernel, typename Args>
+int launch_dyn_smem(const char* name, int grid, int threads, size_t smem, uint32_t smem_max, cudaStream_t st, const Args& args) {
+  static bool raised = false;
+  if (!raised) {
+    cudaError_t e = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
+    if (e != cudaSuccess) return set_error(HRV_ECUDA, "cudaFuncSetAttribute(%s): %s", name, cudaGetErrorString(e));
+    raised = true;
+  }
+  kKernel<<<grid, threads, smem, st>>>(args);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(HRV_ECUDA, "%s launch: %s", name, cudaGetErrorString(e));
+  return HRV_OK;
 }
 }  // namespace hrv_host
 namespace hrv {

@@ -19,18 +19,6 @@ namespace hrv {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// One lane of a fully converged warp (warp-uniform control flow lets the compiler keep descriptors in uniform
-// registers and issue UTMALDG directly instead of wrapping it in a per-thread election loop).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -59,6 +47,23 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Barriers of a stage ring at shared address `bars`: full barrier of stage s at +8 s, empty barrier at +128 + 8 s.
+__device__ __forceinline__ uint32_t bar_full(uint32_t bars, int s) { return bars + 8u * s; }
+__device__ __forceinline__ uint32_t bar_empty(uint32_t bars, int s) { return bars + 128u + 8u * s; }
+
+// Cursor over a ring of `n` pipeline stages of `bytes` each from shared address `base`: stage index, the parity its mbarriers
+// complete next, stage address.
+struct StageRing {
+  uint32_t base, bytes;
+  int n, stage = 0;
+  uint32_t phase = 0, addr;
+  __device__ __forceinline__ StageRing(uint32_t base_, uint32_t bytes_, int n_) : base(base_), bytes(bytes_), n(n_), addr(base_) {}
+  __device__ __forceinline__ void next() {
+    addr += bytes;
+    if (++stage == n) { stage = 0; phase ^= 1u; addr = base; }
+  }
+};
+
 // ---------------------------------------------------------------- TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -73,12 +78,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
 
@@ -123,6 +122,13 @@ __device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t
       : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
 }
 
+// m64nN for N = 64 or 128.
+template <int N, int TA = 0, int TB = 0>
+__device__ __forceinline__ void wgmma_nx(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (N == 64) wgmma_n64<TA, TB>(d, da, db, scale_d);
+  else wgmma_n128<TA, TB>(d, da, db, scale_d);
+}
+
 // TF32 forms (K = 8 per instruction, 32 bytes of a 128-byte swizzle row, both operands K-major: TF32 operands cannot be
 // transposed).  Used by the fp32 reference-precision convolution (conv_f32.cu).
 __device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
@@ -143,6 +149,12 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uin
       "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(da), "l"(db), "r"(scale_d));
+}
+
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_nx(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (N == 64) wgmma_tf32_n64(d, da, db, scale_d);
+  else wgmma_tf32_n128(d, da, db, scale_d);
 }
 
 // fp32 -> TF32 with round-to-nearest (ties away from zero), returned as fp32 bits with the low 13 mantissa bits cleared.

@@ -396,7 +396,7 @@ PIXN_CASES = [  # n, cin, cout, h, w, k, pad, act, bias, scale, out_pitch
 
 
 @pytest.mark.parametrize("case", PIXN_CASES)
-def test_conv_pixn_matches_classic_kernel(case):
+def test_narrow_conv_reproducible_and_matches_torch(case):
     """Narrow convolutions (Cout <= 128, 64-channel K blocks, every activation, bias / scale, padded output pitch): two launches on
     identical inputs are bit-identical, and the result matches torch's convolution of the bf16-rounded operands."""
     n, cin, cout, h, w, k, pad, act, bias, scale, out_pitch = case
