@@ -791,8 +791,9 @@ __global__ void flow_warp_bwd_kernel(const float* __restrict__ flow_lo, const fl
   const float ixr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)src.w), 1.f), 2.f);
   const float iyr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)src.h), 1.f), 2.f);
   const float ix = fminf(fmaxf(ixr, 0.f), (float)(src.w - 1)), iy = fminf(fmaxf(iyr, 0.f), (float)(src.h - 1));
-  const float mx = (ixr < 0.f || ixr > (float)(src.w - 1)) ? 0.f : 1.f;  // clip_coordinates_set_grad
-  const float my = (iyr < 0.f || iyr > (float)(src.h - 1)) ? 0.f : 1.f;
+  // clip_coordinates_set_grad: a coordinate ON the border counts as clamped too (torch: in <= 0 or in >= size-1 -> zero gradient)
+  const float mx = (ixr <= 0.f || ixr >= (float)(src.w - 1)) ? 0.f : 1.f;
+  const float my = (iyr <= 0.f || iyr >= (float)(src.h - 1)) ? 0.f : 1.f;
   const float fx0 = floorf(ix), fy0 = floorf(iy);
   const int x0 = (int)fx0, y0 = (int)fy0;
   const float tx = ix - fx0, ty = iy - fy0;

@@ -210,7 +210,8 @@ int hrv_bilinear_up2_bwd(const hrv_tensor* dout, const hrv_tensor* da, hrv_strea
 /* Backward of hrv_flow_warp (F.grid_sample backward with border padding, networks.py:135,152, fused with the flow chain):
  *   dsrc32 [n][H][W][roundup8(c)] fp32, caller-zeroed: += d_dst * lerp weight at the 4 taps (atomic scatter; may be NULL);
  *   dflow_up [n][H][W][2] fp32, caller-initialised (zeros, or the gradient arriving directly at the up-sampled flow):
- *            += analytic d/d(flow_up) of the sampled values (zero where the coordinate was clamped);
+ *            += analytic d/d(flow_up) of the sampled values (zero where the coordinate was clamped; a coordinate exactly
+ *               on the border, 0 or size-1, counts as clamped, as in torch's grid_sample backward);
  *   dflow_lo [n][H/2][W/2][2] fp32: written = adjoint of the x2 bilinear flow up-sampling applied to dflow_up (may be NULL). */
 int hrv_flow_warp_bwd(const float* flow_lo, const float* lin_x, const float* lin_y, const hrv_tensor* src, const hrv_tensor* ddst,
                       float* dsrc32, float* dflow_up, float* dflow_lo, hrv_stream stream);
