@@ -21,10 +21,6 @@ constexpr uint32_t kWgBytes = 64 * kConvRowBytes;                // one consumer
 constexpr uint32_t kScratch = 2 * kConvConsumers * kWgBytes;     // lo tiles, two per consumer (ping-pong)
 constexpr ConvBudget kBudget32 = {227u * 1024u, 8, kScratch, 32, 2};  // one CTA per SM
 
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-
 // hi/lo split of one warpgroup's 64 rows (8 KB): thread t handles four 16-byte vectors.
 __device__ __forceinline__ void split_rows(uint32_t hi_rows, uint32_t lo_rows, int t) {
 #pragma unroll
@@ -101,7 +97,7 @@ __global__ void __launch_bounds__(kConvThreads, 1) conv_tf32x3_kernel(const __gr
       ring.next();
     }
   }
-  conv_epilogue<BNT>(a, tile, acc);
+  conv_epilogue<BNT>(a, tile, acc, stage0);
 }
 
 }  // namespace hrv

@@ -11,14 +11,15 @@
 //               n_pad are zero fill.
 //   Pipeline:   warp 8 = TMA producer, warpgroups 0 / 1 = consumers for pixels 0-63 / 64-127 of the tile.  A ring of `stages`
 //               (A + B) stages with full (transaction count) / empty (one arrival per consumer warp) mbarriers.
-//   Epilogues:  straight from the wgmma accumulator fragment.
+//   Epilogues:  staged: the accumulators go through an fp32 tile in the idle stage ring and leave in row order, as 16-byte vectors.
 //               LINEAR  out = act(acc*scale + shift (+ residual))      (bias / folded BatchNorm / residual / tanh)
-//               SPADE   out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta), gamma/beta = interleaved GEMM columns: a thread's
-//                       accumulator pair (2j, 2j+1) is (gamma, beta) of one channel, so the SPADE modulation never leaves registers
+//               SPADE   out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta), gamma/beta = interleaved GEMM columns (2k, 2k+1)
+//                       of channel k, so one 8-channel group of the modulation is 16 adjacent tile columns
 //                       (network_generator.py:115-121,170-171).
 //               The gate residual modes and gamma_out serve the backward pass and exist on 16-bit storage only.
 //
-// Shared memory of a CTA: 1 KB of mbarriers (full at +0, empty at +128), then `scratch` bytes the kernel owns, then the stage ring.
+// Shared memory of a CTA: 1 KB of mbarriers (full at +0, empty at +128), then `scratch` bytes the kernel owns, then the stage ring
+// (at least the 128 x BNT fp32 epilogue tile).
 #pragma once
 #include "hrv_host.h"
 #include "hrv_ptx.cuh"
@@ -49,6 +50,7 @@ struct alignas(64) ConvArgs {
   void* out;                       // T NHWC; on 16-bit storage also fp32 NHWC / NCHW
   int out_pitch, out_dtype, out_layout, out_c;
   int store_c;                     // LINEAR writes channels [0, store_c): out_c, or up to the next multiple of 8 (pad channels)
+  int out_vec;                     // out is the storage type, NHWC, 16-byte aligned, pitch and store_c multiples of 8: 8-channel stores
   const void* res;                 // T NHWC; on 16-bit storage also fp32 NHWC
   int res_pitch, res_dtype, res_c;  // an fp32 residual is added to channels [0, res_c)
   int res_mode;                    // 0 add, 1 ReLU gate, 2 LeakyReLU(0.2) gate (16-bit res only)
@@ -123,121 +125,238 @@ __device__ __forceinline__ void conv_produce(const ConvArgs<T>& a, const ConvTil
   }
 }
 
-// One output pixel as seen by an epilogue thread.
+// ------------------------------------------------------------------------------------------------ epilogue
+// The epilogue runs after the main loop and is staged through the stage ring, which is idle by then (the producer issued exactly KT
+// loads and the consumers waited on all of them):
+//   1. each consumer thread writes its wgmma fragment into an fp32 [128 pixels][BNT] tile at the start of the ring;
+//   2. the 256 consumer threads walk the tile in row order.  A thread owns one 8-channel group (8 LINEAR columns, or 16 interleaved
+//      SPADE gamma/beta columns) and visits every (256 / threads per pixel)-th pixel, so x, the residual, out and gamma_out move as
+//      16-byte vectors of consecutive channels and the per-channel constants are loaded once.  fp32 outputs that are not the storage
+//      type (flows, discriminator logits, NCHW heads) keep one element per store, with lanes along pixels so that NCHW rows coalesce.
+// Tile layout: XOR swizzle, no padding.  Row r is BNT floats; its 16-byte chunk q is stored at chunk q ^ (r & 7).  A fragment store
+// (8 rows x 32 bytes per warp) then hits every bank twice (2 wavefronts, the minimum for 256 bytes), and a row-order 16-byte load
+// (32 / G rows x G groups per warp, G a power of two) hits every bank four times (4 wavefronts, the minimum for 512 bytes).
+
+constexpr uint32_t kEpiBar = 3;  // named barrier of the 256 consumer threads (conv_f32.cu uses 1 and 2 in its main loop)
+
+__host__ __device__ constexpr uint32_t conv_tile_bytes(int bnt) { return 128u * (uint32_t)bnt * 4u; }
+
+// Byte offset of element (pixel r, tile column c) in the staged tile.
+template <int BNT>
+__device__ __forceinline__ uint32_t tile_off(int r, int c) {
+  return (uint32_t)r * (BNT * 4u) + ((((uint32_t)c >> 2) ^ ((uint32_t)r & 7u)) << 4) + (((uint32_t)c & 3u) << 2);
+}
+
+// One output pixel: row r of the tile.
 struct EpiPix {
   int x, y, n;
   bool valid;
   long long pix;
 };
 
-__device__ __forceinline__ float ld_act(const float* p) { return __ldg(p); }
-__device__ __forceinline__ float ld_act(const __nv_bfloat16* p) { return __bfloat162float(*p); }
-__device__ __forceinline__ void st_act(float* p, float v) { *p = v; }
-__device__ __forceinline__ void st_act(__nv_bfloat16* p, float v) { *p = __float2bfloat16(v); }
-
-// LINEAR epilogue of two adjacent GEMM columns (c, c+1) of one pixel: out = act(acc*scale + shift (+ res | * act'(res))).
 template <typename T>
-__device__ __forceinline__ void epi_linear2(const ConvArgs<T>& a, const EpiPix& p, int c, float v0, float v1) {
-  if (!p.valid || c >= a.store_c) return;
-  float f[2] = {v0, v1};
+__device__ __forceinline__ EpiPix epi_pix(const ConvArgs<T>& a, const ConvTile& t, int r) {
+  EpiPix p;
+  p.x = (t.tx << a.tw_log) + (r & ((1 << a.tw_log) - 1));
+  p.y = (t.ty << a.th_log) + ((r >> a.tw_log) & ((1 << a.th_log) - 1));
+  p.n = (t.ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
+  p.valid = (p.x < a.Wout) && (p.y < a.Hout) && (p.n < a.Nimg);
+  p.pix = ((long long)p.n * a.Hout + p.y) * a.Wout + p.x;
+  return p;
+}
+
+// Eight consecutive activations <-> fp32 (16-byte aligned).
+__device__ __forceinline__ void ld8(const __nv_bfloat16* p, float (&v)[8]) {
+  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int j = c + i;
-    const bool in = j < a.n_gemm;
-    const float sc = in ? (a.scale ? __ldg(a.scale + j) : 1.f) : 0.f;
-    const float sh = (in && a.shift) ? __ldg(a.shift + j) : 0.f;
-    f[i] = fmaf(f[i], sc, sh);
-  }
-  if (a.res) {
-    bool res16 = false;
-    if constexpr (kStorage16<T>) {
-      res16 = a.res_dtype == HRV_BF16;
-      if (res16) {
-        const uint32_t rv = __ldg(reinterpret_cast<const unsigned int*>(static_cast<const T*>(a.res) + p.pix * a.res_pitch + c));
-        const float rf[2] = {bf16_lo(rv), bf16_hi(rv)};
-        if (a.res_mode == 0) {
-          f[0] += rf[0]; f[1] += rf[1];
-        } else {  // activation backward of the layer below, fused: multiply by act'(its saved output)
-          const float slope = a.res_mode == 1 ? 0.f : 0.2f;
+  for (int i = 0; i < 4; ++i) { v[2 * i] = bf16_lo(w[i]); v[2 * i + 1] = bf16_hi(w[i]); }
+}
+__device__ __forceinline__ void ld8(const float* p, float (&v)[8]) {
+  const float4 u = __ldg(reinterpret_cast<const float4*>(p)), w = __ldg(reinterpret_cast<const float4*>(p) + 1);
+  v[0] = u.x; v[1] = u.y; v[2] = u.z; v[3] = u.w; v[4] = w.x; v[5] = w.y; v[6] = w.z; v[7] = w.w;
+}
+__device__ __forceinline__ void st8(__nv_bfloat16* p, const float (&v)[8]) {
+  *reinterpret_cast<uint4*>(p) = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
+}
+__device__ __forceinline__ void st8(float* p, const float (&v)[8]) {
+  reinterpret_cast<float4*>(p)[0] = make_float4(v[0], v[1], v[2], v[3]);
+  reinterpret_cast<float4*>(p)[1] = make_float4(v[4], v[5], v[6], v[7]);
+}
+
+// LINEAR scale / shift of GEMM column j; columns past n_gemm (pad channels) become act(0) (+ res).
+template <typename T>
+__device__ __forceinline__ void lin_coef(const ConvArgs<T>& a, int j, float& sc, float& sh) {
+  const bool in = j < a.n_gemm;
+  sc = in ? (a.scale ? __ldg(a.scale + j) : 1.f) : 0.f;
+  sh = (in && a.shift) ? __ldg(a.shift + j) : 0.f;
+}
+
+// Threads per pixel of the row pass: `groups` 8-channel groups rounded up to a power of two (returned as log2).
+__device__ __forceinline__ int groups_log(int groups) { return groups <= 1 ? 0 : 32 - __clz(groups - 1); }
+
+// LINEAR into a storage-type NHWC output (a.out_vec): out = act(acc*scale + shift (+ res | * act'(res))), 8 channels per access.
+template <int BNT, typename T>
+__device__ __forceinline__ void epi_linear_rows(const ConvArgs<T>& a, const ConvTile& t, uint32_t tile, int tid) {
+  const int col0 = t.nt * BNT;
+  const int groups = (min(BNT, a.store_c - col0) + 7) >> 3;  // store_c % 8 == 0 here
+  if (groups <= 0) return;
+  const int gl = groups_log(groups);
+  const int g = tid & ((1 << gl) - 1);
+  if (g >= groups) return;
+  const int c = col0 + 8 * g;
+  float sc[8], sh[8];
 #pragma unroll
-          for (int i = 0; i < 2; ++i) f[i] = rf[i] > 0.f ? f[i] : f[i] * slope;
+  for (int i = 0; i < 8; ++i) lin_coef(a, c + i, sc[i], sh[i]);
+  for (int r = tid >> gl; r < 128; r += 256 >> gl) {
+    const EpiPix p = epi_pix(a, t, r);
+    if (!p.valid) continue;
+    float f[8];
+    ld_shared_v4(tile + tile_off<BNT>(r, 8 * g), f);
+    ld_shared_v4(tile + tile_off<BNT>(r, 8 * g + 4), f + 4);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) f[i] = fmaf(f[i], sc[i], sh[i]);
+    if (a.res) {
+      bool res_st = false;
+      if constexpr (kStorage16<T>) {
+        res_st = a.res_dtype == HRV_BF16;
+        if (res_st) {
+          float rf[8];
+          ld8(static_cast<const T*>(a.res) + p.pix * a.res_pitch + c, rf);
+          if (a.res_mode == 0) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) f[i] += rf[i];
+          } else {  // activation backward of the layer below, fused: multiply by act'(its saved output)
+            const float slope = a.res_mode == 1 ? 0.f : 0.2f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) f[i] = rf[i] > 0.f ? f[i] : f[i] * slope;
+          }
         }
       }
-    }
-    if (!res16) {
-      const float* rp = static_cast<const float*>(a.res) + p.pix * a.res_pitch + c;
+      if (!res_st) {
+        const float* rp = static_cast<const float*>(a.res) + p.pix * a.res_pitch + c;
 #pragma unroll
-      for (int i = 0; i < 2; ++i)
-        if (c + i < a.res_c) f[i] += __ldg(rp + i);
+        for (int i = 0; i < 8; ++i)
+          if (c + i < a.res_c) f[i] += __ldg(rp + i);
+      }
     }
-  }
-  f[0] = apply_act(f[0], a.act);
-  f[1] = apply_act(f[1], a.act);
-  if constexpr (kStorage16<T>) {
-    if (a.out_dtype == HRV_BF16) {  // c even, pitch % 8 == 0: a 4-byte store
-      *reinterpret_cast<uint32_t*>(static_cast<T*>(a.out) + p.pix * a.out_pitch + c) = pack_bf16(f[0], f[1]);
-      return;
-    }
-  }
-  float* const out = static_cast<float*>(a.out);
-  if (a.out_layout == HRV_NHWC) {
-    float* op = out + p.pix * a.out_pitch + c;
-    op[0] = f[0];
-    if (c + 1 < a.store_c) op[1] = f[1];
-  } else {
-    const long long hw = (long long)a.Hout * a.Wout;
 #pragma unroll
-    for (int i = 0; i < 2; ++i)
-      if (c + i < a.out_c) out[((long long)p.n * a.out_c + c + i) * hw + (long long)p.y * a.Wout + p.x] = f[i];
+    for (int i = 0; i < 8; ++i) f[i] = apply_act(f[i], a.act);
+    st8(static_cast<T*>(a.out) + p.pix * a.out_pitch + c, f);
   }
 }
 
-// SPADE epilogue of one channel ch of one pixel; g, b = the (gamma, beta) accumulators of columns 2ch, 2ch+1.
-template <typename T>
-__device__ __forceinline__ void epi_spade1(const ConvArgs<T>& a, const EpiPix& p, long long pix0, float nz, int ch, float g, float b) {
-  if (!p.valid || ch >= a.C_mod) return;
-  const float xs = ld_act((ch < a.x0_c) ? (a.x0 + pix0 * a.x0_pitch + ch) : (a.x1 + p.pix * a.x1_pitch + (ch - a.x0_c)));
-  const float mu = __ldg(a.mean + (long long)p.n * a.C_mod + ch);
-  const float rs = __ldg(a.rstd + (long long)p.n * a.C_mod + ch);
-  const float ns = a.noise_scale ? __ldg(a.noise_scale + ch) : 0.f;
-  const float gm = g + (a.shift ? __ldg(a.shift + 2 * ch) : 0.f);
-  const float bt = b + (a.shift ? __ldg(a.shift + 2 * ch + 1) : 0.f);
-  const float xn = (fmaf(nz, ns, xs) - mu) * rs;
-  const float o = apply_act(fmaf(xn, 1.f + gm, bt), a.act);
-  if constexpr (kStorage16<T>) {
-    if (a.gamma_out) st_act(a.gamma_out + p.pix * a.gamma_pitch + ch, gm);  // training: gamma for the backward pass
-  }
-  st_act(static_cast<T*>(a.out) + p.pix * a.out_pitch + ch, o);
-}
-
-// Epilogue of consumer warpgroup wg from its accumulators.  wgmma m64nN fragment: thread (warp w, lane l) holds rows
-// 16 (w % 4) + l / 4 and that + 8, columns 8 j + 2 (l % 4) + {0, 1}.
+// LINEAR into an fp32 output that is not the storage type (or not 16-byte aligned): one element per store, lanes along pixels.
 template <int BNT, typename T>
-__device__ __forceinline__ void conv_epilogue(const ConvArgs<T>& a, const ConvTile& t, const float (&acc)[BNT / 2]) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2;
-  const int tw_mask = (1 << a.tw_log) - 1, th_mask = (1 << a.th_log) - 1;
-  const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int n_base = t.nt * BNT + 2 * (lane & 3);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = r_base + 8 * h;
-    EpiPix p;
-    p.x = (t.tx << a.tw_log) + (r & tw_mask);
-    p.y = (t.ty << a.th_log) + ((r >> a.tw_log) & th_mask);
-    p.n = (t.ti << (7 - a.tw_log - a.th_log)) + (r >> (a.tw_log + a.th_log));
-    p.valid = (p.x < a.Wout) && (p.y < a.Hout) && (p.n < a.Nimg);
-    p.pix = ((long long)p.n * a.Hout + p.y) * a.Wout + p.x;
-    if (a.epi == 0) {
-#pragma unroll
-      for (int j = 0; j < BNT / 8; ++j) epi_linear2(a, p, n_base + 8 * j, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-    } else {
-      const int sh0 = a.x0_shift;
-      const long long pix0 = ((long long)p.n * (a.Hout >> sh0) + (p.y >> sh0)) * (a.Wout >> sh0) + (p.x >> sh0);
-      const float nz = (p.valid && a.noise) ? __ldg(a.noise + p.pix) : 0.f;
-#pragma unroll
-      for (int j = 0; j < BNT / 8; ++j) epi_spade1(a, p, pix0, nz, (n_base + 8 * j) >> 1, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+__device__ __forceinline__ void epi_linear_f32(const ConvArgs<T>& a, const ConvTile& t, uint32_t tile, int tid) {
+  const int col0 = t.nt * BNT;
+  const int ncols = min(BNT, a.store_c - col0);
+  const int r = tid & 127;
+  const EpiPix p = epi_pix(a, t, r);
+  if (!p.valid) return;
+  float* const out = static_cast<float*>(a.out);
+  const long long hw = (long long)a.Hout * a.Wout;
+  for (int cl = tid >> 7; cl < ncols; cl += 2) {
+    const int c = col0 + cl;
+    float sc, sh;
+    lin_coef(a, c, sc, sh);
+    float f = fmaf(ld_shared_f32(tile + tile_off<BNT>(r, cl)), sc, sh);
+    if (a.res) {
+      bool res_st = false;
+      if constexpr (kStorage16<T>) {
+        res_st = a.res_dtype == HRV_BF16;
+        if (res_st) {
+          const float rf = __bfloat162float(static_cast<const T*>(a.res)[p.pix * a.res_pitch + c]);
+          if (a.res_mode == 0) f += rf;
+          else f = rf > 0.f ? f : f * (a.res_mode == 1 ? 0.f : 0.2f);
+        }
+      }
+      if (!res_st && c < a.res_c) f += __ldg(static_cast<const float*>(a.res) + p.pix * a.res_pitch + c);
     }
+    f = apply_act(f, a.act);
+    if (a.out_layout == HRV_NHWC) out[p.pix * a.out_pitch + c] = f;
+    else out[((long long)p.n * a.out_c + c) * hw + (long long)p.y * a.Wout + p.x] = f;
   }
+}
+
+// SPADE: out = act((x + noise*ns - mean)*rstd*(1+gamma) + beta); tile columns (2k, 2k+1) are (gamma, beta) of channel k.
+template <int BNT, typename T>
+__device__ __forceinline__ void epi_spade_rows(const ConvArgs<T>& a, const ConvTile& t, uint32_t tile, int tid) {
+  const int ch0 = t.nt * (BNT / 2);
+  const int groups = min(BNT / 2, a.C_mod - ch0) >> 3;  // C_mod % 8 == 0
+  if (groups <= 0) return;
+  const int gl = groups_log(groups);
+  const int g = tid & ((1 << gl) - 1);
+  if (g >= groups) return;
+  const int ch = ch0 + 8 * g;
+  float ns[8], gs[8], bs[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    ns[i] = a.noise_scale ? __ldg(a.noise_scale + ch + i) : 0.f;
+    gs[i] = a.shift ? __ldg(a.shift + 2 * (ch + i)) : 0.f;
+    bs[i] = a.shift ? __ldg(a.shift + 2 * (ch + i) + 1) : 0.f;
+  }
+  const bool in_x0 = ch < a.x0_c;  // x0_c % 8 == 0: a group never straddles x0 / x1
+  const int sh0 = a.x0_shift;
+  int n_cur = -1;
+  float mu[8], rs[8];
+  for (int r = tid >> gl; r < 128; r += 256 >> gl) {
+    const EpiPix p = epi_pix(a, t, r);
+    if (!p.valid) continue;
+    if (p.n != n_cur) {  // a tile spans several images at small resolutions
+      n_cur = p.n;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        mu[i] = __ldg(a.mean + (long long)p.n * a.C_mod + ch + i);
+        rs[i] = __ldg(a.rstd + (long long)p.n * a.C_mod + ch + i);
+      }
+    }
+    float xs[8];
+    if (in_x0) {
+      const long long pix0 = ((long long)p.n * (a.Hout >> sh0) + (p.y >> sh0)) * (a.Wout >> sh0) + (p.x >> sh0);
+      ld8(a.x0 + pix0 * a.x0_pitch + ch, xs);
+    } else {
+      ld8(a.x1 + p.pix * a.x1_pitch + (ch - a.x0_c), xs);
+    }
+    const float nz = a.noise ? __ldg(a.noise + p.pix) : 0.f;
+    float v[16];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) ld_shared_v4(tile + tile_off<BNT>(r, 16 * g + 4 * q), v + 4 * q);
+    float o[8], gm[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      gm[i] = v[2 * i] + gs[i];
+      const float bt = v[2 * i + 1] + bs[i];
+      const float xn = (fmaf(nz, ns[i], xs[i]) - mu[i]) * rs[i];
+      o[i] = apply_act(fmaf(xn, 1.f + gm[i], bt), a.act);
+    }
+    if constexpr (kStorage16<T>) {
+      if (a.gamma_out) st8(a.gamma_out + p.pix * a.gamma_pitch + ch, gm);  // training: gamma for the backward pass
+    }
+    st8(static_cast<T*>(a.out) + p.pix * a.out_pitch + ch, o);
+  }
+}
+
+// Epilogue of the 256 consumer threads after their main loops (each warpgroup has run wgmma_wait<0>); `tile` = start of the stage
+// ring.  wgmma m64nN fragment: thread (warp w, lane l) holds rows 16 (w % 4) + l / 4 and that + 8 of its warpgroup's 64, columns
+// 8 j + 2 (l % 4) + {0, 1}.
+template <int BNT, typename T>
+__device__ __forceinline__ void conv_epilogue(const ConvArgs<T>& a, const ConvTile& t, const float (&acc)[BNT / 2], uint32_t tile) {
+  const int tid = threadIdx.x;  // 0..255
+  const int warp = tid >> 5, lane = tid & 31;
+  named_bar_sync(kEpiBar, 4 * 32 * kConvConsumers);  // both warpgroups' MMAs are done reading the ring
+  fence_proxy_async();
+  const int r0 = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BNT / 8; ++j)
+      st_shared_v2(tile + tile_off<BNT>(r0 + 8 * h, 8 * j + c0), acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  named_bar_sync(kEpiBar, 4 * 32 * kConvConsumers);
+  if (a.epi == HRV_EPI_SPADE) epi_spade_rows<BNT>(a, t, tile, tid);
+  else if (a.out_vec) epi_linear_rows<BNT>(a, t, tile, tid);
+  else epi_linear_f32<BNT>(a, t, tile, tid);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -312,6 +431,8 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
   // room.  Other outputs stop at out_c.
   const int c8 = (out.c + 7) & ~7;
   a.store_c = (p->out_layout == HRV_NHWC && out.dtype == storage && out.pitch >= c8) ? c8 : out.c;
+  // Always true for 16-bit outputs (their alignment is validated above).  Other outputs are written one element per store.
+  a.out_vec = p->out_layout == HRV_NHWC && out.dtype == storage && !((uintptr_t)out.ptr & 15) && !(out.pitch % 8) && !(a.store_c % 8);
   if (p->res.ptr) {
     a.res = p->res.ptr; a.res_pitch = p->res.pitch; a.res_dtype = p->res.dtype; a.res_mode = res_mode;
     a.res_c = (p->res.dtype == storage && p->res.pitch >= a.store_c) ? a.store_c : out.c;
@@ -328,6 +449,7 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
       return set_error(HRV_EINVAL, "%s: channel counts must be multiples of 8, output %s NHWC, mean/rstd/x0 set", spre, f32 ? "fp32" : "bf16");
     if (((uintptr_t)p->x0.ptr & 15) || (p->x0.pitch % 8) || (p->x1.ptr && (((uintptr_t)p->x1.ptr & 15) || (p->x1.pitch % 8))))
       return set_error(HRV_EINVAL, "%s: x0/x1 alignment", spre);
+    if (!a.out_vec) return set_error(HRV_EINVAL, "%s: the output needs a 16-byte aligned ptr and pitch %% 8 == 0", spre);
     if (p->x0_shift && ((out.h & 1) || (out.w & 1) || p->x0.h * 2 != out.h || p->x0.w * 2 != out.w))
       return set_error(HRV_EINVAL, "%s: x0_shift needs x0 at exactly half resolution", spre);
     if (!p->x0_shift && (p->x0.h != out.h || p->x0.w != out.w)) return set_error(HRV_EINVAL, "%s: x0 extent mismatch", spre);
@@ -344,14 +466,17 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
     return set_error(HRV_EINVAL, "%s: unknown epilogue %d", pre, p->epi);
   }
 
-  // ---- pipeline: as many stages as fit in the budget next to the scratch, at most one per K step
+  // ---- pipeline: as many stages as fit in the budget next to the scratch, at most one per K step; the ring also holds the
+  //      epilogue tile
   const uint32_t stage_bytes = kConvABytes + (uint32_t)(budget.planes * bnt) * kConvRowBytes;
   const int KT = p->kh * p->kw * a.chunks;
   int stages = (int)((budget.smem - 2048u - budget.scratch) / stage_bytes);
   if (stages > budget.max_stages) stages = budget.max_stages;
   if (stages > KT) stages = KT < 2 ? 2 : KT;
   a.stages = stages;
-  const size_t smem = 2048 + budget.scratch + (size_t)stages * stage_bytes;  // 1 KB alignment slack + 1 KB of barriers
+  const size_t ring_stages = (size_t)stages * stage_bytes;
+  const size_t ring = ring_stages > conv_tile_bytes(bnt) ? ring_stages : conv_tile_bytes(bnt);
+  const size_t smem = 2048 + budget.scratch + ring;  // 1 KB alignment slack + 1 KB of barriers
 
   // ---- tensor maps: the input, and the packed weights [planes][taps][n_pad][cin_k] as laid out for this (bk, bn)
   int rc = encode_nhwc_map(&a.tmA, in, budget.kblock, TW, TH, TN);

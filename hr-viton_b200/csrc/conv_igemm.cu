@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(kConvThreads, 2) conv_wgmma_kernel(const __gri
     wgmma_wait<0>();
     fence_regs(acc);
   }
-  conv_epilogue<BNT>(a, t, acc);
+  conv_epilogue<BNT>(a, t, acc, stage0);
 }
 
 }  // namespace hrv

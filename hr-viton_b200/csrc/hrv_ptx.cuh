@@ -172,6 +172,22 @@ __device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t sbo
          ((uint64_t)layout_type << 62);
 }
 
+// ---------------------------------------------------------------- shared memory, named barriers
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ void ld_shared_v4(uint32_t addr, float* v) {
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ float ld_shared_f32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+
 // ---------------------------------------------------------------- misc
 #ifdef HRV_F16
 __device__ __forceinline__ float bf16_lo(uint32_t u) { return __half2float(__ushort_as_half((unsigned short)(u & 0xFFFFu))); }
