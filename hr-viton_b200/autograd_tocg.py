@@ -102,6 +102,26 @@ class FlowWarpFn(torch.autograd.Function):
         return (dsrc.buf if dsrc is not None else None), dflo
 
 
+class FlowWarpNchwFn(torch.autograd.Function):
+    """(warped, warped_mask) = hrv_flow_warp_nchw(src, mask, flow_lo) at any scale: F.interpolate(size, bilinear) of the flow, normalise by
+    div_xy, + base grid, grid_sample(border) of the planar fp32 cloth and its mask (train_condition.py's --interflowloss warps).
+    backward = hrv_flow_warp_nchw_bwd: the gradient reaches flow_lo only (cloth and mask are data)."""
+
+    @staticmethod
+    def forward(ctx, flow_lo, src, mask, size, div_xy):
+        flow_lo = flow_lo.contiguous()
+        out, _, mask_out = ops.flow_warp_nchw(flow_lo, src, size, div_xy, mask=mask)
+        ctx.save_for_backward(flow_lo, src, mask)
+        ctx.size, ctx.div_xy = size, div_xy
+        return out, mask_out
+
+    @staticmethod
+    def backward(ctx, d_out, d_mask):
+        flow_lo, src, mask = ctx.saved_tensors
+        dflo = ops.flow_warp_nchw_bwd(flow_lo, src, ctx.size, ctx.div_xy, d_out, mask=mask, d_mask=d_mask) if ctx.needs_input_grad[0] else None
+        return dflo, None, None, None, None
+
+
 def _resblock(rb, x_buf):
     """ResBlock.forward in training mode (networks.py:171-198)."""
     if rb.kind == "down":

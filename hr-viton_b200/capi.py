@@ -14,7 +14,11 @@ RES_ADD, RES_GATE_RELU, RES_GATE_LRELU = 0, 1, 2
 
 EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_instnorm_apply", "hrv_norm_apply_affine", "hrv_norm_bwd_reduce", "hrv_norm_bwd_apply", "hrv_act_bwd_bias", "hrv_conv2d_wgrad", "hrv_conv2d_wgrad_workspace_bytes", "hrv_nchw_to_nhwc", "hrv_nhwc_to_nchw",
            "hrv_space_to_depth", "hrv_avgpool3s2", "hrv_bilinear_up2_add", "hrv_flow_warp", "hrv_bilinear_up2_bwd", "hrv_flow_warp_bwd", "hrv_pack_conv_weight", "hrv_pack_conv_weight_tf32x2", "hrv_space_to_depth_bwd", "hrv_maxpool2_fwd", "hrv_maxpool2_bwd",
-           "hrv_avgpool3s2_bwd", "hrv_parse_blur_argmax", "hrv_gaussian_blur", "hrv_flow_warp_nchw", "hrv_onehot_u8", "hrv_im2col", "hrv_l1_sum", "hrv_l1_bwd", "hrv_last_error",
+           "hrv_avgpool3s2_bwd", "hrv_parse_blur_argmax", "hrv_gaussian_blur", "hrv_flow_warp_nchw", "hrv_onehot_u8", "hrv_im2col", "hrv_l1_sum", "hrv_l1_bwd",
+           "hrv_instnorm_stats_workspace_bytes", "hrv_instnorm_stats2_workspace_bytes", "hrv_norm_bwd_reduce_workspace_bytes",
+           "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
+           "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
+           "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 
 
@@ -64,15 +68,15 @@ def lib(dtype=None):
         raise RuntimeError("hrviton_b200: %s is missing — run `python __graft_entry__.py build` (no CPU fallback exists)" % LIB_PATH)
     L = ctypes.CDLL(LIB_PATH)
     L.hrv_last_error.restype = ctypes.c_char_p
-    vp, i32, f32 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_float
+    vp, i32, f32, sz = ctypes.c_void_p, ctypes.c_int32, ctypes.c_float, ctypes.c_size_t
     TP = ctypes.POINTER(Tensor)
     L.hrv_conv2d_fwd.argtypes = [ctypes.POINTER(ConvParams), vp]
     L.hrv_instnorm_stats.argtypes = [TP, i32, TP, i32, i32, vp, vp, f32, vp, vp, vp, ctypes.c_size_t, vp]
     L.hrv_instnorm_stats2.argtypes = [TP, i32, TP, i32, i32, vp, vp, vp, vp, f32, vp, vp, vp, vp, vp, ctypes.c_size_t, vp]
     L.hrv_instnorm_apply.argtypes = [TP, vp, vp, i32, TP, vp]
-    L.hrv_norm_bwd_reduce.argtypes = [TP, TP, TP, TP, i32, TP, i32, i32, vp, vp, vp, vp, vp, i32, TP, TP, vp, vp]
+    L.hrv_norm_bwd_reduce.argtypes = [TP, TP, TP, TP, i32, TP, i32, i32, vp, vp, vp, vp, vp, i32, TP, TP, vp, vp, sz, vp]
     L.hrv_norm_apply_affine.argtypes = [TP, vp, vp, vp, vp, TP, i32, TP, vp]
-    L.hrv_norm_bwd_apply.argtypes = [TP, TP, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, TP, vp, vp]
+    L.hrv_norm_bwd_apply.argtypes = [TP, TP, i32, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, TP, vp, vp, sz, vp]
     L.hrv_act_bwd_bias.argtypes = [TP, TP, i32, TP, vp, vp]
     L.hrv_conv2d_wgrad.argtypes = [TP, TP, i32, i32, i32, vp, vp, ctypes.c_size_t, vp]
     L.hrv_conv2d_wgrad_workspace_bytes.argtypes = [TP, TP, i32, i32]
@@ -92,17 +96,28 @@ def lib(dtype=None):
     L.hrv_gaussian_blur.argtypes = [vp, i32, i32, i32, i32, f32, vp, vp]
     L.hrv_flow_warp_nchw.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, vp, i32, vp]
     L.hrv_im2col.argtypes = [TP, TP, i32, i32, i32, vp]
-    L.hrv_l1_sum.argtypes = [TP, TP, vp, vp]
+    L.hrv_l1_sum.argtypes = [TP, TP, vp, vp, sz, vp]
     L.hrv_l1_bwd.argtypes = [TP, TP, vp, TP, i32, vp]
     L.hrv_pack_conv_weight.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp]
     L.hrv_pack_conv_weight_tf32x2.argtypes = L.hrv_pack_conv_weight.argtypes
     L.hrv_flow_warp_bwd.argtypes = [vp, vp, vp, TP, TP, vp, vp, vp, vp]
+    L.hrv_flow_warp_bwd_ordered.argtypes = [vp, vp, vp, TP, TP, vp, vp, vp, vp, sz, vp]
+    L.hrv_flow_warp_bwd_ordered_workspace_bytes.argtypes = [TP, TP]
+    L.hrv_act_bwd_bias_ordered.argtypes = [TP, TP, i32, TP, vp, vp, sz, vp]
+    L.hrv_act_bwd_bias_ordered_workspace_bytes.argtypes = [TP]
+    L.hrv_instnorm_stats_workspace_bytes.argtypes = [TP, TP, i32, i32]
+    L.hrv_instnorm_stats2_workspace_bytes.argtypes = [TP, TP]
+    L.hrv_norm_bwd_reduce_workspace_bytes.argtypes = [TP, TP, i32, i32]
+    L.hrv_norm_bwd_apply_workspace_bytes.argtypes = [TP]
+    L.hrv_l1_sum_workspace_bytes.argtypes = [TP]
+    L.hrv_flow_warp_nchw_bwd.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, vp, sz, vp]
+    L.hrv_flow_warp_nchw_bwd_workspace_bytes.argtypes = [i32, i32, i32, i32]
     for name in FLAVOURED:
         twin = getattr(L, name + "_f16")
         twin.argtypes = getattr(L, name).argtypes
     for name in EXPORTS + EXPORTS_F16:
         fn = getattr(L, name)
-        if name.startswith("hrv_conv2d_wgrad_workspace_bytes"):
+        if "_workspace_bytes" in name:
             fn.restype = ctypes.c_size_t
         elif name != "hrv_last_error":
             fn.restype = ctypes.c_int

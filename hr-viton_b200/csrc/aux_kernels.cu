@@ -2,6 +2,8 @@
 // InstanceNorm statistics (with the SPADE noise, virtual up-sampling and concat), InstanceNorm apply, layout
 // converters with nearest resampling, space-to-depth, 3x3/s2 average pool, bilinear x2 (+add), and the fused
 // appearance-flow warp.  Citations: see include/hrviton_sm100.h.
+#include <cub/device/device_radix_sort.cuh>
+
 #include "hrv_host.h"
 #include "hrv_ptx.cuh"
 
@@ -58,7 +60,8 @@ template <> __device__ __forceinline__ Vec8<float> zero8<float>() { return Vec8<
 // ------------------------------------------------------------------------------------------------ IN statistics
 // grid (chunks, N); thread = (pixel lane pl, channel group g of 8).  Each thread accumulates fp32 partial sums over its
 // pixels (4 independent 16-byte loads in flight), partials meet in shared memory (one slot per thread, no atomics),
-// then one fp64 global atomic per channel per block.
+// then every block writes its fp64 per-channel sums into its own slab [n][blockIdx.x][C][2]; slab_sum adds the slabs in a fixed
+// order, so the statistics do not depend on which block finishes first.
 template <typename T>
 struct StatsSrc {
   const T* p0;
@@ -77,7 +80,7 @@ __device__ __forceinline__ void stats_load(const StatsSrc<T>& S, long long p, Ve
 template <typename T>
 __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shift, View x1, int H, int W, int G, int PL,
                                                             int chunk, const float* __restrict__ noise,
-                                                            const float* __restrict__ ns, double* __restrict__ acc) {
+                                                            const float* __restrict__ ns, double* __restrict__ slab) {
   extern __shared__ float shf[];  // [PL][C][2]
   const int n = blockIdx.y;
   const int C = G * 8;
@@ -140,8 +143,9 @@ __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shi
       S1 += (double)shf[((long long)l * C + c) * 2];
       S2 += (double)shf[((long long)l * C + c) * 2 + 1];
     }
-    atomicAdd(&acc[((long long)n * C + c) * 2], S1);
-    atomicAdd(&acc[((long long)n * C + c) * 2 + 1], S2);
+    double* o = slab + (((long long)n * gridDim.x + blockIdx.x) * C + c) * 2;
+    o[0] = S1;
+    o[1] = S2;
   }
 }
 
@@ -152,12 +156,13 @@ __global__ void __launch_bounds__(256) instnorm_stats_kernel(View x0, int x0_shi
 //   sum_P (x_c[P] + nz_j[P] ns_jc)^2 = S2_c + 2 ns_jc X_jc + ns_jc^2 NZ2_j   S2_c = sum x_c^2, X_jc = sum x_c nz_j, NZ2_j = sum nz_j^2
 // x0 is read at ITS OWN resolution: with x0_shift = 1 every source pixel stands for its 2x2 children, so S1/S2 count it four times and
 // X_jc pairs it with the sum of the children's noise — 4x fewer bytes than walking the virtual up-sampled tensor, and the second
-// norm costs no second pass.  Segment 0 of the grid (blockIdx.z) covers x0, segment 1 covers x1.  acc: [N][C][4] doubles
-// {S1, S2, X_0, X_1}; nzacc: [N][2][2] doubles {NZ1_j, NZ2_j}.
+// norm costs no second pass.  One launch per segment: segment 0 covers x0, segment 1 covers x1.  Every block writes its sums into
+// its own slab, added in a fixed order by slab_sum: slab [N][gridDim.x][Cs][4] doubles {S1, S2, X_0, X_1} -> acc [N][C][4];
+// nzslab [N][gridDim.x][4] doubles {NZ1_0, NZ2_0, NZ1_1, NZ2_1} (segment 0 only) -> nzacc [N][4].
 template <typename T>
-__global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift, int c_off, int C, int W_full, int G, int PL, int chunk,
+__global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift, int W_full, int G, int PL, int chunk,
                                                              const float* __restrict__ nz0, const float* __restrict__ nz1,
-                                                             double* __restrict__ acc, double* __restrict__ nzacc, int do_noise_sums) {
+                                                             double* __restrict__ slab, double* __restrict__ nzslab, int do_noise_sums) {
   extern __shared__ float shf[];  // [PL][G*8][4]
   __shared__ float nzred[8][4];
   const int n = blockIdx.y;
@@ -218,13 +223,9 @@ __global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift
       const float* e = shf + ((long long)l * Cs + c) * 4;
       t[0] += (double)e[0]; t[1] += (double)e[1]; t[2] += (double)e[2]; t[3] += (double)e[3];
     }
-    double* a = acc + ((long long)n * C + c_off + c) * 4;
-    atomicAdd(a, t[0] * mult);
-    atomicAdd(a + 1, t[1] * mult);
-    atomicAdd(a + 2, t[2]);
-    atomicAdd(a + 3, t[3]);
+    reinterpret_cast<double4*>(slab)[(size_t)(n * gridDim.x + blockIdx.x) * Cs + c] = make_double4(t[0] * mult, t[1] * mult, t[2], t[3]);
   }
-  if (do_noise_sums) {  // NZ1/NZ2 of both norms: only the g == 0 threads hold contributions; warp reduce, then one atomic per block
+  if (do_noise_sums) {  // NZ1/NZ2 of both norms: only the g == 0 threads hold contributions; warp reduce, then one slab entry per block
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       float v = nsum[k];
@@ -236,7 +237,7 @@ __global__ void __launch_bounds__(256) instnorm_stats2_kernel(View xs, int shift
     if (threadIdx.x < 4) {
       double t = 0.0;
       for (int wv = 0; wv < 8; ++wv) t += (double)nzred[wv][threadIdx.x];
-      atomicAdd(nzacc + (long long)n * 4 + threadIdx.x, t);
+      nzslab[(size_t)(n * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = t;
     }
   }
 }
@@ -436,20 +437,18 @@ __global__ void bilinear_up2_add_kernel(View a, View b, View dst, int G, long lo
 }
 
 // ------------------------------------------------------------------------------------------------ flow warp
-// thread = (dst pixel, 8-channel group).  The coordinate chain uses explicitly rounded fp32 operations (no FMA
-// contraction) in the exact order of oracle/hrviton_oracle.py:np_flow_warp_coords so that the gather indices
-// are bit-exact.
-__global__ void flow_warp_kernel(const float* __restrict__ flow_lo, const float* __restrict__ lin_x, const float* __restrict__ lin_y,
-                                 View src, View dst, float* __restrict__ flow_up, int* __restrict__ idx_out, float sx, float sy,
-                                 int G, long long total) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= total) return;
-  const int g = (int)(idx % G);
-  const long long pix = idx / G;
-  const int W = dst.w, H = dst.h;
-  const int x = (int)(pix % W);
-  const int y = (int)((pix / W) % H);
-  const int n = (int)(pix / ((long long)W * H));
+// The sampling coordinates of destination pixel (x, y) of image n, shared by the forward and the ordered backward passes so they
+// cannot drift apart.  The chain uses explicitly rounded fp32 operations (no FMA contraction) in the exact order of
+// oracle/hrviton_oracle.py:np_flow_warp_coords so that the gather indices are bit-exact.
+struct WarpTaps {
+  float fx, fy;    // the up-sampled flow
+  float ixr, iyr;  // source coordinates before the border clamp
+  int x0, y0, x1, y1;
+  float tx, ty, wx0, wx1, wy0, wy1;  // wx1 / wy1 are zero where the second tap falls outside the image
+  bool vx, vy;     // the second tap lies inside the image
+};
+__device__ __forceinline__ WarpTaps warp_taps(const float* __restrict__ flow_lo, const float* __restrict__ lin_x, const float* __restrict__ lin_y,
+                                              int n, int x, int y, int H, int W, int Hs, int Ws, float sx, float sy) {
   const int hl = H >> 1, wl = W >> 1;
   int xa, xb, ya, yb;
   float wxa, wxb, wya, wyb;
@@ -463,26 +462,51 @@ __global__ void flow_warp_kernel(const float* __restrict__ flow_lo, const float*
   const float ux1 = __fadd_rn(__fmul_rn(f10.x, wxa), __fmul_rn(f11.x, wxb));
   const float uy0 = __fadd_rn(__fmul_rn(f00.y, wxa), __fmul_rn(f01.y, wxb));
   const float uy1 = __fadd_rn(__fmul_rn(f10.y, wxa), __fmul_rn(f11.y, wxb));
-  const float fx = __fadd_rn(__fmul_rn(ux0, wya), __fmul_rn(ux1, wyb));
-  const float fy = __fadd_rn(__fmul_rn(uy0, wya), __fmul_rn(uy1, wyb));
-  const float gx = __fadd_rn(__fdiv_rn(fx, sx), __ldg(lin_x + x));
-  const float gy = __fadd_rn(__fdiv_rn(fy, sy), __ldg(lin_y + y));
-  float ix = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)src.w), 1.f), 2.f);
-  float iy = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)src.h), 1.f), 2.f);
-  ix = fminf(fmaxf(ix, 0.f), (float)(src.w - 1));
-  iy = fminf(fmaxf(iy, 0.f), (float)(src.h - 1));
+  WarpTaps t;
+  t.fx = __fadd_rn(__fmul_rn(ux0, wya), __fmul_rn(ux1, wyb));
+  t.fy = __fadd_rn(__fmul_rn(uy0, wya), __fmul_rn(uy1, wyb));
+  const float gx = __fadd_rn(__fdiv_rn(t.fx, sx), __ldg(lin_x + x));
+  const float gy = __fadd_rn(__fdiv_rn(t.fy, sy), __ldg(lin_y + y));
+  t.ixr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)Ws), 1.f), 2.f);
+  t.iyr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)Hs), 1.f), 2.f);
+  const float ix = fminf(fmaxf(t.ixr, 0.f), (float)(Ws - 1));
+  const float iy = fminf(fmaxf(t.iyr, 0.f), (float)(Hs - 1));
   const float fx0 = floorf(ix), fy0 = floorf(iy);
-  const int x0 = (int)fx0, y0 = (int)fy0;
-  const float tx = __fsub_rn(ix, fx0), ty = __fsub_rn(iy, fy0);
+  t.x0 = (int)fx0;
+  t.y0 = (int)fy0;
+  t.tx = __fsub_rn(ix, fx0);
+  t.ty = __fsub_rn(iy, fy0);
+  t.vx = t.x0 + 1 <= Ws - 1;
+  t.vy = t.y0 + 1 <= Hs - 1;
+  t.x1 = t.vx ? t.x0 + 1 : t.x0;
+  t.y1 = t.vy ? t.y0 + 1 : t.y0;
+  t.wx1 = t.vx ? t.tx : 0.f;
+  t.wy1 = t.vy ? t.ty : 0.f;
+  t.wx0 = __fsub_rn(1.f, t.tx);
+  t.wy0 = __fsub_rn(1.f, t.ty);
+  return t;
+}
+
+// thread = (dst pixel, 8-channel group).
+__global__ void flow_warp_kernel(const float* __restrict__ flow_lo, const float* __restrict__ lin_x, const float* __restrict__ lin_y,
+                                 View src, View dst, float* __restrict__ flow_up, int* __restrict__ idx_out, float sx, float sy,
+                                 int G, long long total) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int g = (int)(idx % G);
+  const long long pix = idx / G;
+  const int W = dst.w, H = dst.h;
+  const int x = (int)(pix % W);
+  const int y = (int)((pix / W) % H);
+  const int n = (int)(pix / ((long long)W * H));
+  const WarpTaps t = warp_taps(flow_lo, lin_x, lin_y, n, x, y, H, W, src.h, src.w, sx, sy);
+  const int x0 = t.x0, y0 = t.y0, x1 = t.x1, y1 = t.y1;
   if (g == 0) {
-    if (flow_up) reinterpret_cast<float2*>(flow_up)[pix] = make_float2(fx, fy);
+    if (flow_up) reinterpret_cast<float2*>(flow_up)[pix] = make_float2(t.fx, t.fy);
     if (idx_out) reinterpret_cast<int2*>(idx_out)[pix] = make_int2(x0, y0);
   }
   if (g * 8 >= ((src.c + 7) & ~7)) return;
-  const int x1 = min(x0 + 1, src.w - 1), y1 = min(y0 + 1, src.h - 1);
-  const float wx1 = (x0 + 1 <= src.w - 1) ? tx : 0.f, wy1 = (y0 + 1 <= src.h - 1) ? ty : 0.f;
-  const float wx0 = 1.f - tx, wy0 = 1.f - ty;
-  const float w00 = wy0 * wx0, w01 = wy0 * wx1, w10 = wy1 * wx0, w11 = wy1 * wx1;
+  const float w00 = t.wy0 * t.wx0, w01 = t.wy0 * t.wx1, w10 = t.wy1 * t.wx0, w11 = t.wy1 * t.wx1;
   float o[8];
   const long long ib = (long long)n * src.h * src.w;
   if (src.dtype == 0) {
@@ -543,10 +567,31 @@ static int launch_ok(const char* what) {
   return HRV_OK;
 }
 static inline unsigned blocks_for(long long total, int bs) { return (unsigned)((total + bs - 1) / bs); }
+static inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// Grid of the statistics kernels: blocks per image over HW pixels, PL pixel lanes per block.  Depends on the shapes and the SM
+// count only, so the per-block slabs, and the order they are added in, are fixed for a given device and shape.
+static unsigned stats_blocks(long long HW, int N, int PL, long long& chunk) {
+  long long target_blocks = (long long)sm_count() * 8 / (N > 0 ? N : 1);
+  if (target_blocks < 1) target_blocks = 1;
+  chunk = (HW + target_blocks - 1) / target_blocks;
+  const long long min_chunk = (long long)PL * 16;
+  if (chunk < min_chunk) chunk = min_chunk;
+  return (unsigned)((HW + chunk - 1) / chunk);
+}
 
 }  // namespace hrv
 
 using namespace hrv;
+
+extern "C" size_t hrv_instnorm_stats_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1, int32_t h, int32_t w) {
+  if (!x0) return 0;
+  const int C = x0->c + ((x1 && x1->ptr) ? x1->c : 0);
+  const int N = x0->n, G = (C + 7) / 8, PL = G > 0 && G <= 256 ? 256 / G : 1;
+  long long chunk;
+  const unsigned gx = stats_blocks((long long)h * w, N, PL, chunk);
+  return ((size_t)N * C * 2 + (size_t)N * gx * C * 2) * sizeof(double);
+}
 
 extern "C" int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w,
                                   const float* noise, const float* noise_scale, float eps, float* mean, float* rstd,
@@ -562,24 +607,51 @@ extern "C" int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const 
   if ((x0->h << x0_shift) != h || (x0->w << x0_shift) != w) return set_error(HRV_EINVAL, "instnorm_stats: x0 extent mismatch");
   if (has1 && (x1->h != h || x1->w != w || x1->n != x0->n)) return set_error(HRV_EINVAL, "instnorm_stats: x1 extent mismatch");
   const int N = x0->n;
-  const size_t need = (size_t)N * C * 2 * sizeof(double);
+  const size_t need = hrv_instnorm_stats_workspace_bytes(x0, x1, h, w);
   if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "instnorm_stats: workspace too small (%zu < %zu)", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(workspace, 0, need, st);
   const int G = C / 8;
   const int PL = 256 / G;
   const long long HW = (long long)h * w;
-  long long target_blocks = (long long)sm_count() * 8 / (N > 0 ? N : 1);
-  if (target_blocks < 1) target_blocks = 1;
-  long long chunk = (HW + target_blocks - 1) / target_blocks;
-  const long long min_chunk = (long long)PL * 16;
-  if (chunk < min_chunk) chunk = min_chunk;
-  const unsigned gx = (unsigned)((HW + chunk - 1) / chunk);
+  long long chunk;
+  const unsigned gx = stats_blocks(HW, N, PL, chunk);
+  double* acc = (double*)workspace;  // [N][C][2] raw sums, then the blocks' slabs
+  double* slab = acc + (size_t)N * C * 2;
   HRV_LAUNCH_STORAGE(dt, instnorm_stats_kernel, dim3(gx, N), 256, (size_t)PL * C * 2 * sizeof(float), st, mk(x0), x0_shift,
-                     mk(has1 ? x1 : nullptr), h, w, G, PL, (int)chunk, noise, noise_scale, (double*)workspace);
+                     mk(has1 ? x1 : nullptr), h, w, G, PL, (int)chunk, noise, noise_scale, slab);
   if ((rc = launch_ok("instnorm_stats"))) return rc;
-  instnorm_finalize_kernel<<<blocks_for(N * C, 256), 256, 0, st>>>((const double*)workspace, N * C, 1.0 / (double)HW, eps, mean, rstd);
+  if ((rc = slab_sum(slab, N, (int)gx, C * 2, acc, C * 2, st, "instnorm_stats sum"))) return rc;
+  instnorm_finalize_kernel<<<blocks_for(N * C, 256), 256, 0, st>>>(acc, N * C, 1.0 / (double)HW, eps, mean, rstd);
   return launch_ok("instnorm_finalize");
+}
+
+// Workspace of hrv_instnorm_stats2: the sums acc and nzacc, segment 0 (x0) slabs, segment 1 (x1) slabs, segment 0's noise-sum slabs.
+static void stats2_plan(const hrv_tensor* x0, const hrv_tensor* x1, unsigned gx[2], long long chunk[2], size_t off[3], size_t& total) {
+  const int N = x0->n;
+  const bool has1 = x1 && x1->ptr;
+  const int C = x0->c + (has1 ? x1->c : 0);
+  size_t o = ((size_t)N * C * 4 + (size_t)N * 4) * sizeof(double);  // acc [N][C][4], nzacc [N][4]
+  for (int seg = 0; seg < 2; ++seg) {
+    gx[seg] = 0;
+    chunk[seg] = 0;
+    off[seg] = o;
+    if (seg == 1 && !has1) continue;
+    const hrv_tensor* xs = seg ? x1 : x0;
+    const int G = xs->c / 8, PL = G > 0 && G <= 256 ? 256 / G : 1;
+    gx[seg] = stats_blocks((long long)xs->h * xs->w, N, PL, chunk[seg]);
+    o += (size_t)N * gx[seg] * xs->c * 4 * sizeof(double);
+  }
+  off[2] = o;
+  total = o + (size_t)N * gx[0] * 4 * sizeof(double);
+}
+
+extern "C" size_t hrv_instnorm_stats2_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1) {
+  if (!x0) return 0;
+  unsigned gx[2];
+  long long chunk[2];
+  size_t off[3], total;
+  stats2_plan(x0, x1, gx, chunk, off, total);
+  return total;
 }
 
 extern "C" int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w, const float* noise0,
@@ -600,29 +672,29 @@ extern "C" int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const
   if (!mean0 || !rstd0 || ((mean1 == nullptr) != (rstd1 == nullptr))) return set_error(HRV_EINVAL, "instnorm_stats2: outputs");
   if ((noise0 && !noise_scale0) || (noise1 && !noise_scale1)) return set_error(HRV_EINVAL, "instnorm_stats2: noise without noise_scale");
   const int N = x0->n;
-  const size_t need = ((size_t)N * C * 4 + (size_t)N * 4) * sizeof(double);
+  unsigned gx[2];
+  long long chunk[2];
+  size_t off[3], need;
+  stats2_plan(x0, x1, gx, chunk, off, need);
   if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "instnorm_stats2: workspace too small (%zu < %zu)", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(workspace, 0, need, st);
-  double* acc = (double*)workspace;
-  double* nzacc = acc + (size_t)N * C * 4;
+  char* ws = (char*)workspace;
+  double* nzslab = (double*)(ws + off[2]);
   for (int seg = 0; seg < (has1 ? 2 : 1); ++seg) {
     const hrv_tensor* xs = seg ? x1 : x0;
     const int shift = seg ? 0 : x0_shift;
     const int G = xs->c / 8, PL = 256 / G;
-    const long long HWs = (long long)xs->h * xs->w;
-    long long target_blocks = (long long)sm_count() * 8 / (N > 0 ? N : 1);
-    if (target_blocks < 1) target_blocks = 1;
-    long long chunk = (HWs + target_blocks - 1) / target_blocks;
-    const long long min_chunk = (long long)PL * 16;
-    if (chunk < min_chunk) chunk = min_chunk;
-    const unsigned gx = (unsigned)((HWs + chunk - 1) / chunk);
     // the noise-only sums are taken once, by the segment that walks the full-resolution grid exactly once per pixel: x0's walk covers
     // every full-resolution pixel through its footprint, so segment 0 always does it
-    HRV_LAUNCH_STORAGE(dt, instnorm_stats2_kernel, dim3(gx, N), 256, (size_t)PL * G * 8 * 4 * sizeof(float), st, mk(xs), shift, seg ? x0->c : 0,
-                       C, w, G, PL, (int)chunk, noise0, noise1, acc, nzacc, seg == 0);
+    HRV_LAUNCH_STORAGE(dt, instnorm_stats2_kernel, dim3(gx[seg], N), 256, (size_t)PL * G * 8 * 4 * sizeof(float), st, mk(xs), shift,
+                       w, G, PL, (int)chunk[seg], noise0, noise1, (double*)(ws + off[seg]), nzslab, seg == 0);
     if ((rc = launch_ok("instnorm_stats2"))) return rc;
   }
+  double* acc = (double*)ws;
+  double* nzacc = acc + (size_t)N * C * 4;
+  if ((rc = slab_sum((const double*)(ws + off[0]), N, (int)gx[0], x0->c * 4, acc, C * 4, st, "instnorm_stats2 sum"))) return rc;
+  if (has1 && (rc = slab_sum((const double*)(ws + off[1]), N, (int)gx[1], x1->c * 4, acc + (size_t)x0->c * 4, C * 4, st, "instnorm_stats2 sum"))) return rc;
+  if ((rc = slab_sum(nzslab, N, (int)gx[0], 4, nzacc, 4, st, "instnorm_stats2 noise sum"))) return rc;
   instnorm_finalize2_kernel<<<blocks_for(N * C, 256), 256, 0, st>>>(acc, nzacc, N, C, 1.0 / ((double)h * w), eps, noise0 ? noise_scale0 : nullptr,
                                                                    noise1 ? noise_scale1 : nullptr, mean0, rstd0, mean1, rstd1);
   return launch_ok("instnorm_finalize2");
@@ -864,6 +936,140 @@ __global__ void flow_up2_bwd_kernel(const float* __restrict__ dup, float* __rest
   reinterpret_cast<float2*>(dlo)[idx] = make_float2(ax, ay);
 }
 
+// ---- ordered backward of flow_warp_kernel: d_src as a gather in a fixed order, d_flow_up without atomics.
+// Pass 1, thread = (dst pixel p, 8-channel group g): recomputes the taps (warp_taps) and writes the group's share of the coordinate
+// gradient to part[p][g]; the g == 0 thread also writes one sort entry per tap: key = source pixel index within the batch (the
+// sentinel S = N*Hs*Ws for a zero-weight tap, so it sorts last), value = 4*p + tap, weight wts[4*p + tap].
+__global__ void flow_warp_bwd_entries_kernel(const float* __restrict__ flow_lo, const float* __restrict__ lin_x, const float* __restrict__ lin_y,
+                                             View src, View ddst, float sx, float sy, int G, long long total, unsigned* __restrict__ keys,
+                                             unsigned* __restrict__ vals, float* __restrict__ wts, float2* __restrict__ part) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int g = (int)(idx % G);
+  const long long pix = idx / G;
+  const int W = ddst.w, H = ddst.h;
+  const int x = (int)(pix % W);
+  const int y = (int)((pix / W) % H);
+  const int n = (int)(pix / ((long long)W * H));
+  const WarpTaps t = warp_taps(flow_lo, lin_x, lin_y, n, x, y, H, W, src.h, src.w, sx, sy);
+  const long long ib = (long long)n * src.h * src.w;
+  if (keys && g == 0) {
+    const unsigned sentinel = (unsigned)((long long)src.n * src.h * src.w);
+    const long long tap_pix[4] = {ib + (long long)t.y0 * src.w + t.x0, ib + (long long)t.y0 * src.w + t.x1,
+                                  ib + (long long)t.y1 * src.w + t.x0, ib + (long long)t.y1 * src.w + t.x1};
+    const float w[4] = {t.wy0 * t.wx0, t.wy0 * t.wx1, t.wy1 * t.wx0, t.wy1 * t.wx1};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const long long e = 4 * pix + k;
+      keys[e] = w[k] != 0.f ? (unsigned)tap_pix[k] : sentinel;
+      vals[e] = (unsigned)e;
+      wts[e] = w[k];
+    }
+  }
+  if (!part) return;
+  const float mx = (t.ixr <= 0.f || t.ixr >= (float)(src.w - 1)) ? 0.f : 1.f;
+  const float my = (t.iyr <= 0.f || t.iyr >= (float)(src.h - 1)) ? 0.f : 1.f;
+  float d[8], a[8], b[8], c[8], e[8];
+  unpack8(ldg16(reinterpret_cast<const __nv_bfloat16*>(ddst.ptr) + pix * ddst.pitch + g * 8), d);
+  const __nv_bfloat16* sp = reinterpret_cast<const __nv_bfloat16*>(src.ptr) + g * 8;
+  unpack8(ldg16(sp + (ib + (long long)t.y0 * src.w + t.x0) * src.pitch), a);
+  unpack8(ldg16(sp + (ib + (long long)t.y0 * src.w + t.x1) * src.pitch), b);
+  unpack8(ldg16(sp + (ib + (long long)t.y1 * src.w + t.x0) * src.pitch), c);
+  unpack8(ldg16(sp + (ib + (long long)t.y1 * src.w + t.x1) * src.pitch), e);
+  float dix = 0.f, diy = 0.f;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    // value = a*wy0*wx0 + b*wy0*wx1 + c*wy1*wx0 + e*wy1*wx1 ; taps outside the image carry zero weight AND zero derivative
+    const float bb = t.vx ? b[k] : 0.f, cc = t.vy ? c[k] : 0.f, ee = (t.vx && t.vy) ? e[k] : 0.f;
+    dix += d[k] * ((bb - a[k]) * t.wy0 + (ee - cc) * t.wy1);
+    diy += d[k] * ((cc - a[k]) * t.wx0 + (ee - bb) * t.wx1);
+  }
+  // d ix / d gx = src.w/2 ; d gx / d flow_up.x = 1/sx
+  part[pix * G + g] = make_float2(dix * mx * (0.5f * (float)src.w) / sx, diy * my * (0.5f * (float)src.h) / sy);
+}
+
+// Pass 2, thread = dst pixel: dflow_up += the groups' partials, added in ascending group order.
+__global__ void flow_warp_bwd_dflow_kernel(const float2* __restrict__ part, float2* __restrict__ dflow_up, int G, long long npix) {
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= npix) return;
+  float2 v = dflow_up[pix];
+  for (int g = 0; g < G; ++g) {
+    const float2 q = __ldg(part + pix * G + g);
+    v.x = __fadd_rn(v.x, q.x);
+    v.y = __fadd_rn(v.y, q.y);
+  }
+  dflow_up[pix] = v;
+}
+
+// Pass 3 (after the stable radix sort by key), thread = source pixel s in [0, S]: begin[s] = first sorted entry with key >= s.
+__global__ void flow_warp_bwd_bounds_kernel(const unsigned* __restrict__ keys, long long m, unsigned* __restrict__ begin, long long S) {
+  const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s > S) return;
+  long long lo = 0, hi = m;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if ((long long)__ldg(keys + mid) < s) lo = mid + 1;
+    else hi = mid;
+  }
+  begin[s] = (unsigned)lo;
+}
+
+// Pass 4, thread = (source pixel s, 8-channel group g): dsrc32[s] = sum of d_dst[p] * w over s's entries in ascending
+// (dst pixel, tap) order — the stable sort kept that order.  __fmul_rn / __fadd_rn forbid FMA contraction, so the result equals a
+// sequential fp32 sum in that order bit for bit.
+__global__ void flow_warp_bwd_gather_kernel(View ddst, const unsigned* __restrict__ begin, const unsigned* __restrict__ vals,
+                                            const float* __restrict__ wts, float* __restrict__ dsrc32, int G, long long total) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int g = (int)(idx % G);
+  const long long s = idx / G;
+  const unsigned b = __ldg(begin + s), e = __ldg(begin + s + 1);
+  float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  const __nv_bfloat16* dp = reinterpret_cast<const __nv_bfloat16*>(ddst.ptr) + g * 8;
+  for (unsigned i = b; i < e; ++i) {
+    const unsigned v = __ldg(vals + i);
+    const float w = __ldg(wts + v);
+    float d[8];
+    unpack8(ldg16(dp + (long long)(v >> 2) * ddst.pitch), d);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], __fmul_rn(d[k], w));
+  }
+  float4* o = reinterpret_cast<float4*>(dsrc32 + s * (long long)G * 8 + g * 8);
+  o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+  o[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+}
+
+// Workspace of hrv_flow_warp_bwd_ordered, 256-byte aligned pieces.
+struct WarpBwdPlan {
+  long long m, S, npix;
+  int G, end_bit;
+  size_t keys_in, keys_out, vals_in, vals_out, wts, begin, part, temp, temp_bytes, total;
+};
+static int warp_bwd_plan(const hrv_tensor* src, const hrv_tensor* ddst, WarpBwdPlan& p) {
+  p.npix = (long long)ddst->n * ddst->h * ddst->w;
+  p.m = 4 * p.npix;
+  p.S = (long long)src->n * src->h * src->w;
+  p.G = (src->c + 7) / 8;
+  p.end_bit = log2i((int)(p.S + 1));
+  if (p.end_bit < 1) p.end_bit = 1;
+  p.temp_bytes = 0;
+  cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, p.temp_bytes, (const unsigned*)nullptr, (unsigned*)nullptr, (const unsigned*)nullptr,
+                                                  (unsigned*)nullptr, (int)p.m, 0, p.end_bit);
+  if (e != cudaSuccess) return set_error(HRV_ECUDA, "flow_warp_bwd_ordered: sort size query: %s", cudaGetErrorString(e));
+  size_t o = 0;
+  const size_t ent = align256((size_t)p.m * 4);
+  p.keys_in = o; o += ent;
+  p.keys_out = o; o += ent;
+  p.vals_in = o; o += ent;
+  p.vals_out = o; o += ent;
+  p.wts = o; o += ent;
+  p.begin = o; o += align256((size_t)(p.S + 1) * 4);
+  p.part = o; o += align256((size_t)p.npix * p.G * sizeof(float2));
+  p.temp = o; o += align256(p.temp_bytes);
+  p.total = o;
+  return HRV_OK;
+}
+
 }  // namespace hrv
 
 extern "C" int hrv_bilinear_up2_bwd(const hrv_tensor* dout, const hrv_tensor* da, hrv_stream stream) {
@@ -889,6 +1095,62 @@ extern "C" int hrv_flow_warp_bwd(const float* flow_lo, const float* lin_x, const
   cudaStream_t st = (cudaStream_t)stream;
   flow_warp_bwd_kernel<<<blocks_for(total, 256), 256, 0, st>>>(flow_lo, lin_x, lin_y, mk(src), mk(ddst), dsrc32, dflow_up, sx, sy, G, total);
   if ((rc = launch_ok("flow_warp_bwd"))) return rc;
+  if (dflow_lo) {
+    const long long tl = (long long)ddst->n * (ddst->h / 2) * (ddst->w / 2);
+    flow_up2_bwd_kernel<<<blocks_for(tl, 256), 256, 0, st>>>(dflow_up, dflow_lo, ddst->n, ddst->h / 2, ddst->w / 2);
+    return launch_ok("flow_up2_bwd");
+  }
+  return HRV_OK;
+}
+
+extern "C" size_t hrv_flow_warp_bwd_ordered_workspace_bytes(const hrv_tensor* src, const hrv_tensor* ddst) {
+  if (!src || !ddst) return 0;
+  WarpBwdPlan p;
+  return warp_bwd_plan(src, ddst, p) ? 0 : p.total;
+}
+
+extern "C" int hrv_flow_warp_bwd_ordered(const float* flow_lo, const float* lin_x, const float* lin_y, const hrv_tensor* src,
+                                         const hrv_tensor* ddst, float* dsrc32, float* dflow_up, float* dflow_lo, void* workspace,
+                                         size_t workspace_bytes, hrv_stream stream) {
+  int rc;
+  if (!flow_lo || !lin_x || !lin_y) return set_error(HRV_EINVAL, "flow_warp_bwd_ordered: null argument");
+  if ((rc = check_bf16_vec(src, "flow_warp_bwd_ordered src")) || (rc = check_bf16_vec(ddst, "flow_warp_bwd_ordered ddst"))) return rc;
+  if ((ddst->h & 1) || (ddst->w & 1) || src->n != ddst->n || src->c != ddst->c) return set_error(HRV_EINVAL, "flow_warp_bwd_ordered: shape mismatch");
+  if (dflow_lo && !dflow_up) return set_error(HRV_EINVAL, "flow_warp_bwd_ordered: dflow_lo needs the dflow_up buffer");
+  if (((uintptr_t)dsrc32 & 15)) return set_error(HRV_EINVAL, "flow_warp_bwd_ordered: dsrc32 needs 16-byte alignment");
+  WarpBwdPlan p;
+  if ((rc = warp_bwd_plan(src, ddst, p))) return rc;
+  if (p.m >= (1LL << 32) || p.S >= (1LL << 31)) return set_error(HRV_EUNSUPPORTED, "flow_warp_bwd_ordered: more than 2^30 destination pixels");
+  if (!workspace || workspace_bytes < p.total)
+    return set_error(HRV_EINVAL, "flow_warp_bwd_ordered: workspace too small (%zu < %zu)", workspace_bytes, p.total);
+  if (!dsrc32 && !dflow_up) return HRV_OK;
+  char* ws = (char*)workspace;
+  unsigned* keys_in = (unsigned*)(ws + p.keys_in);
+  unsigned* keys_out = (unsigned*)(ws + p.keys_out);
+  unsigned* vals_in = (unsigned*)(ws + p.vals_in);
+  unsigned* vals_out = (unsigned*)(ws + p.vals_out);
+  float* wts = (float*)(ws + p.wts);
+  unsigned* begin = (unsigned*)(ws + p.begin);
+  float2* part = (float2*)(ws + p.part);
+  const float sx = (float)((ddst->w / 2.0 - 1.0) / 2.0), sy = (float)((ddst->h / 2.0 - 1.0) / 2.0);
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long total = p.npix * p.G;
+  flow_warp_bwd_entries_kernel<<<blocks_for(total, 256), 256, 0, st>>>(flow_lo, lin_x, lin_y, mk(src), mk(ddst), sx, sy, p.G, total,
+                                                                       dsrc32 ? keys_in : nullptr, vals_in, wts, dflow_up ? part : nullptr);
+  if ((rc = launch_ok("flow_warp_bwd_entries"))) return rc;
+  if (dflow_up) {
+    flow_warp_bwd_dflow_kernel<<<blocks_for(p.npix, 256), 256, 0, st>>>(part, (float2*)dflow_up, p.G, p.npix);
+    if ((rc = launch_ok("flow_warp_bwd_dflow"))) return rc;
+  }
+  if (dsrc32) {
+    size_t tb = p.temp_bytes;
+    cudaError_t e = cub::DeviceRadixSort::SortPairs(ws + p.temp, tb, keys_in, keys_out, vals_in, vals_out, (int)p.m, 0, p.end_bit, st);
+    if (e != cudaSuccess) return set_error(HRV_ECUDA, "flow_warp_bwd_ordered sort: %s", cudaGetErrorString(e));
+    flow_warp_bwd_bounds_kernel<<<blocks_for(p.S + 1, 256), 256, 0, st>>>(keys_out, p.m, begin, p.S);
+    if ((rc = launch_ok("flow_warp_bwd_bounds"))) return rc;
+    flow_warp_bwd_gather_kernel<<<blocks_for(p.S * p.G, 256), 256, 0, st>>>(mk(ddst), begin, vals_out, wts, dsrc32, p.G, p.S * p.G);
+    if ((rc = launch_ok("flow_warp_bwd_gather"))) return rc;
+  }
   if (dflow_lo) {
     const long long tl = (long long)ddst->n * (ddst->h / 2) * (ddst->w / 2);
     flow_up2_bwd_kernel<<<blocks_for(tl, 256), 256, 0, st>>>(dflow_up, dflow_lo, ddst->n, ddst->h / 2, ddst->w / 2);

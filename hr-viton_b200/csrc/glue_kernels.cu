@@ -307,6 +307,123 @@ __global__ void __launch_bounds__(256) flow_warp_nchw_kernel(const float* __rest
   }
 }
 
+// ---------------------------------------------------------------------------------------------- hi-res flow warp backward
+// d flow_lo of flow_warp_nchw_kernel (without overlap / composite), in three gathers with fixed summation orders:
+//   1. thread = hi-res pixel: the analytic coordinate gradient of grid_sample (bilinear, border; a coordinate clamped or exactly on
+//      the border gets none), summing the C channels and then the mask in that order, times d ix / d flow = (size/2) / div;
+//   2. thread = (n, hi-res row y, lo-res column X): R[y][X] = sum over hi-res columns x (ascending) of wx(x, X) * dhi[y][x];
+//   3. thread = (n, Y, X): dflow_lo[Y][X] = sum over hi-res rows y (ascending) of wy(y, Y) * R[y][X]
+// — 2 and 3 are the adjoint of F.interpolate(size, bilinear, align_corners=False), row then column.
+__device__ __forceinline__ void resize_taps(float sc, int d, int n_lo, int& i0, int& i1, float& l, float& h) {
+  const float f = fmaxf(__fsub_rn(__fmul_rn(sc, __fadd_rn((float)d, 0.5f)), 0.5f), 0.f);
+  i0 = (int)f;
+  i1 = min(i0 + 1, n_lo - 1);
+  l = __fsub_rn(f, (float)i0);
+  h = __fsub_rn(1.f, l);
+}
+__global__ void __launch_bounds__(256) flow_warp_nchw_bwd_coord_kernel(const float* __restrict__ flow_lo, int hl, int wl, const float* __restrict__ lin_x,
+                                                                      const float* __restrict__ lin_y, const float* __restrict__ src, int C, int Hs, int Ws,
+                                                                      const float* __restrict__ d_dst, int H, int W, float div_x, float div_y,
+                                                                      float sc_y, float sc_x, const float* __restrict__ mask_src,
+                                                                      const float* __restrict__ d_mask, float2* __restrict__ dhi, long long npix) {
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= npix) return;
+  const int x = (int)(pix % W), y = (int)((pix / W) % H), n = (int)(pix / ((long long)W * H));
+  int y0, y1, x0, x1;
+  float ly, hy, lx, hx;
+  resize_taps(sc_y, y, hl, y0, y1, ly, hy);
+  resize_taps(sc_x, x, wl, x0, x1, lx, hx);
+  const float2* fl = reinterpret_cast<const float2*>(flow_lo) + (long long)n * hl * wl;
+  const float2 f00 = __ldg(fl + (long long)y0 * wl + x0), f01 = __ldg(fl + (long long)y0 * wl + x1);
+  const float2 f10 = __ldg(fl + (long long)y1 * wl + x0), f11 = __ldg(fl + (long long)y1 * wl + x1);
+  const float ux = __fadd_rn(__fmul_rn(hy, __fadd_rn(__fmul_rn(hx, f00.x), __fmul_rn(lx, f01.x))), __fmul_rn(ly, __fadd_rn(__fmul_rn(hx, f10.x), __fmul_rn(lx, f11.x))));
+  const float uy = __fadd_rn(__fmul_rn(hy, __fadd_rn(__fmul_rn(hx, f00.y), __fmul_rn(lx, f01.y))), __fmul_rn(ly, __fadd_rn(__fmul_rn(hx, f10.y), __fmul_rn(lx, f11.y))));
+  const float gx = __fadd_rn(__fdiv_rn(ux, div_x), __ldg(lin_x + x));
+  const float gy = __fadd_rn(__fdiv_rn(uy, div_y), __ldg(lin_y + y));
+  const float ixr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gx, 1.f), (float)Ws), 1.f), 2.f);
+  const float iyr = __fdiv_rn(__fsub_rn(__fmul_rn(__fadd_rn(gy, 1.f), (float)Hs), 1.f), 2.f);
+  const float ix = fminf(fmaxf(ixr, 0.f), (float)(Ws - 1)), iy = fminf(fmaxf(iyr, 0.f), (float)(Hs - 1));
+  const float mx = (ixr <= 0.f || ixr >= (float)(Ws - 1)) ? 0.f : 1.f;
+  const float my = (iyr <= 0.f || iyr >= (float)(Hs - 1)) ? 0.f : 1.f;
+  const float bx = floorf(ix), by = floorf(iy);
+  const int sx0 = (int)bx, sy0 = (int)by;
+  const float tx = __fsub_rn(ix, bx), ty = __fsub_rn(iy, by);
+  const bool vx = sx0 + 1 <= Ws - 1, vy = sy0 + 1 <= Hs - 1;
+  const int sx1 = vx ? sx0 + 1 : sx0, sy1 = vy ? sy0 + 1 : sy0;
+  const float wx0 = 1.f - tx, wy0 = 1.f - ty, wx1 = vx ? tx : 0.f, wy1 = vy ? ty : 0.f;
+  const long long plane_s = (long long)Hs * Ws, plane_d = (long long)H * W;
+  const long long o00 = (long long)sy0 * Ws + sx0, o01 = (long long)sy0 * Ws + sx1, o10 = (long long)sy1 * Ws + sx0, o11 = (long long)sy1 * Ws + sx1;
+  const long long dpix = (long long)y * W + x;
+  float dix = 0.f, diy = 0.f;
+  // value = a*wy0*wx0 + b*wy0*wx1 + c*wy1*wx0 + e*wy1*wx1 ; taps outside the image carry zero weight AND zero derivative
+  for (int ch = 0; ch <= C; ++ch) {
+    const float* sp;
+    float d;
+    if (ch < C) {
+      if (!d_dst) continue;
+      sp = src + ((long long)n * C + ch) * plane_s;
+      d = __ldg(d_dst + ((long long)n * C + ch) * plane_d + dpix);
+    } else {
+      if (!d_mask) break;
+      sp = mask_src + (long long)n * plane_s;
+      d = __ldg(d_mask + (long long)n * plane_d + dpix);
+    }
+    const float a = __ldg(sp + o00), b = vx ? __ldg(sp + o01) : 0.f, c = vy ? __ldg(sp + o10) : 0.f, e = (vx && vy) ? __ldg(sp + o11) : 0.f;
+    dix = __fadd_rn(dix, __fmul_rn(d, __fadd_rn(__fmul_rn(__fsub_rn(b, a), wy0), __fmul_rn(__fsub_rn(e, c), wy1))));
+    diy = __fadd_rn(diy, __fmul_rn(d, __fadd_rn(__fmul_rn(__fsub_rn(c, a), wx0), __fmul_rn(__fsub_rn(e, b), wx1))));
+  }
+  dhi[pix] = make_float2(dix * mx * (0.5f * (float)Ws) / div_x, diy * my * (0.5f * (float)Hs) / div_y);
+}
+
+// First hi-res index d whose lower resize tap i0(d) is >= target (i0 is non-decreasing in d).
+__device__ __forceinline__ int first_hi(float sc, int target, int n_hi, int n_lo) {
+  int d = max(0, (int)(((float)target + 0.5f) / sc - 0.5f) - 2);
+  int i0, i1;
+  float l, h;
+  while (d > 0) {
+    resize_taps(sc, d - 1, n_lo, i0, i1, l, h);
+    if (i0 < target) break;
+    --d;
+  }
+  while (d < n_hi) {
+    resize_taps(sc, d, n_lo, i0, i1, l, h);
+    if (i0 >= target) break;
+    ++d;
+  }
+  return d;
+}
+
+// Adjoint of the resize along one axis, as a gather onto lo-res index L: sum over hi-res d (ascending) whose taps i0 / i1 are L.
+// in: element (d) at in[d * stride]; float2 values.
+__device__ __forceinline__ float2 resize_adjoint(const float2* __restrict__ in, long long stride, float sc, int L, int n_hi, int n_lo) {
+  float2 acc = make_float2(0.f, 0.f);
+  for (int d = first_hi(sc, L - 1, n_hi, n_lo); d < n_hi; ++d) {
+    int i0, i1;
+    float l, h;
+    resize_taps(sc, d, n_lo, i0, i1, l, h);
+    if (i0 > L) break;
+    const float2 v = in[(long long)d * stride];
+    if (i0 == L) { acc.x = __fadd_rn(acc.x, __fmul_rn(h, v.x)); acc.y = __fadd_rn(acc.y, __fmul_rn(h, v.y)); }
+    if (i1 == L) { acc.x = __fadd_rn(acc.x, __fmul_rn(l, v.x)); acc.y = __fadd_rn(acc.y, __fmul_rn(l, v.y)); }
+  }
+  return acc;
+}
+__global__ void __launch_bounds__(256) resize_adjoint_rows_kernel(const float2* __restrict__ dhi, int H, int W, int wl, float sc_x,
+                                                                 float2* __restrict__ rows, long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int X = (int)(i % wl);
+  const long long ny = i / wl;  // n * H + y
+  rows[i] = resize_adjoint(dhi + ny * W, 1, sc_x, X, W, wl);
+}
+__global__ void __launch_bounds__(256) resize_adjoint_cols_kernel(const float2* __restrict__ rows, int H, int hl, int wl, float sc_y,
+                                                                 float2* __restrict__ dlo, long long total) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int X = (int)(i % wl), Y = (int)((i / wl) % hl), n = (int)(i / ((long long)wl * hl));
+  dlo[i] = resize_adjoint(rows + (long long)n * H * wl + X, wl, sc_y, Y, H, hl);
+}
+
 // ---------------------------------------------------------------------------------------------- label map -> one-hot planes
 // Input feeding (SURVEY.md 8f N4; cp_dataset.py:150-172 builds the 13-channel one-hot parse map on the CPU and ships it as fp32):
 // the host ships ONE byte per pixel, this kernel expands it on the device.  out[n,c,p] = (label[n,p] == c).  thread = pixel.
@@ -389,8 +506,9 @@ __global__ void __launch_bounds__(256) im2col3x3_c7_kernel(GView src, GView dst,
 }
 
 // ---------------------------------------------------------------------------------------------- L1 feature loss
-// sum |a - b| over the (n,h,w,c) views (fp64 accumulator), and its gradient da = sign(a - b) * (*gscale).
-__global__ void __launch_bounds__(256) l1_fwd_kernel(GView a, GView b, int G, long long total, double* __restrict__ out) {
+// sum |a - b| over the (n,h,w,c) views (every block writes its fp64 partial to slab[blockIdx.x]; l1_finish_kernel adds them in
+// a fixed order), and its gradient da = sign(a - b) * (*gscale).
+__global__ void __launch_bounds__(256) l1_fwd_kernel(GView a, GView b, int G, long long total, double* __restrict__ slab) {
   float acc = 0.f;
   for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long long)gridDim.x * blockDim.x) {
     const int g = (int)(idx % G);
@@ -411,8 +529,24 @@ __global__ void __launch_bounds__(256) l1_fwd_kernel(GView a, GView b, int G, lo
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int i = 0; i < 8; ++i) t += (double)red[i];
-    atomicAdd(out, t);
+    slab[blockIdx.x] = t;
   }
+}
+// One block of 256 threads: thread t adds the slabs of its contiguous range [t*k, (t+1)*k) in order, then a fixed shared-memory
+// tree combines the 256 partials — the same order on every launch, without one thread walking thousands of slabs serially.
+__global__ void __launch_bounds__(256) l1_finish_kernel(const double* __restrict__ slab, int nb, double* __restrict__ out) {
+  __shared__ double part[256];
+  const int k = (nb + 255) / 256, b = threadIdx.x * k, e = min(b + k, nb);
+  double t = 0.0;
+#pragma unroll 4
+  for (int i = b; i < e; ++i) t += slab[i];
+  part[threadIdx.x] = t;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if (threadIdx.x < s) part[threadIdx.x] += part[threadIdx.x + s];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *out = part[0];
 }
 __global__ void l1_bwd_kernel(GView a, GView b, GView da, int G, long long total, const float* __restrict__ gscale, int relu_gate) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -546,6 +680,37 @@ extern "C" int hrv_flow_warp_nchw(const float* flow_lo, int32_t n, int32_t hl, i
   return launched("flow_warp_nchw");
 }
 
+extern "C" size_t hrv_flow_warp_nchw_bwd_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t wl) {
+  if (n < 1 || h < 1 || w < 1 || wl < 1) return 0;
+  return ((size_t)n * h * w + (size_t)n * h * wl) * sizeof(float2);
+}
+
+extern "C" int hrv_flow_warp_nchw_bwd(const float* flow_lo, int32_t n, int32_t hl, int32_t wl, const float* lin_x, const float* lin_y,
+                                      const float* src, int32_t c, int32_t hs, int32_t ws, const float* d_dst, int32_t h, int32_t w,
+                                      float div_x, float div_y, const float* mask_src, const float* d_mask, float* d_flow_lo,
+                                      void* workspace, size_t workspace_bytes, hrv_stream stream) {
+  if (!flow_lo || !lin_x || !lin_y || !d_flow_lo || n < 1 || hl < 1 || wl < 1 || c < 0 || hs < 1 || ws < 1 || h < 1 || w < 1)
+    return set_error(HRV_EINVAL, "flow_warp_nchw_bwd: bad arguments");
+  if ((d_dst && (!src || c < 1)) || (d_mask && !mask_src) || (!d_dst && !d_mask))
+    return set_error(HRV_EINVAL, "flow_warp_nchw_bwd: d_dst needs src, d_mask needs mask_src, and one of them is required");
+  const size_t need = hrv_flow_warp_nchw_bwd_workspace_bytes(n, h, w, wl);
+  if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "flow_warp_nchw_bwd: workspace too small (%zu < %zu)", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  float2* dhi = (float2*)workspace;
+  float2* rows = dhi + (size_t)n * h * w;
+  const float sc_y = (float)hl / (float)h, sc_x = (float)wl / (float)w;
+  const long long npix = (long long)n * h * w;
+  flow_warp_nchw_bwd_coord_kernel<<<nblocks(npix, 256), 256, 0, st>>>(flow_lo, hl, wl, lin_x, lin_y, d_dst ? src : nullptr, d_dst ? c : 0, hs, ws,
+                                                                      d_dst, h, w, div_x, div_y, sc_y, sc_x, mask_src, d_mask, dhi, npix);
+  int rc;
+  if ((rc = launched("flow_warp_nchw_bwd"))) return rc;
+  const long long nr = (long long)n * h * wl, nl = (long long)n * hl * wl;
+  resize_adjoint_rows_kernel<<<nblocks(nr, 256), 256, 0, st>>>(dhi, h, w, wl, sc_x, rows, nr);
+  if ((rc = launched("resize_adjoint_rows"))) return rc;
+  resize_adjoint_cols_kernel<<<nblocks(nl, 256), 256, 0, st>>>(rows, h, hl, wl, sc_y, (float2*)d_flow_lo, nl);
+  return launched("resize_adjoint_cols");
+}
+
 extern "C" int hrv_im2col(const hrv_tensor* src, const hrv_tensor* dst, int32_t kh, int32_t kw, int32_t pad, hrv_stream stream) {
   int rc;
   const bool f32 = src && src->dtype == HRV_F32;  // fp32 storage: the generic kernel on 4-byte elements, dst fp32 as well
@@ -573,20 +738,28 @@ static int l1_check(const hrv_tensor* a, const hrv_tensor* b) {
   return HRV_OK;
 }
 
-extern "C" int hrv_l1_sum(const hrv_tensor* a, const hrv_tensor* b, double* sum, hrv_stream stream) {
+static long long l1_blocks(const hrv_tensor* a) {
+  const long long total = (long long)a->n * a->h * a->w * ((a->c + 7) / 8);
+  const long long want = (total + 255) / 256, cap = (long long)sm_count() * 16;
+  return want < cap ? want : cap;
+}
+
+extern "C" size_t hrv_l1_sum_workspace_bytes(const hrv_tensor* a) { return a ? (size_t)l1_blocks(a) * sizeof(double) : 0; }
+
+extern "C" int hrv_l1_sum(const hrv_tensor* a, const hrv_tensor* b, double* sum, void* workspace, size_t workspace_bytes, hrv_stream stream) {
   int rc;
   if ((rc = l1_check(a, b))) return rc;
   if (!sum) return set_error(HRV_EINVAL, "l1_sum: null accumulator");
+  const long long nb = l1_blocks(a);
+  if (nb && (!workspace || workspace_bytes < (size_t)nb * sizeof(double)))
+    return set_error(HRV_EINVAL, "l1_sum: workspace too small (%zu < %zu)", workspace_bytes, (size_t)nb * sizeof(double));
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(sum, 0, sizeof(double), st);
   const int G = (a->c + 7) / 8;
   const long long total = (long long)a->n * a->h * a->w * G;
-  if (total) {
-    long long want = (total + 255) / 256;
-    const long long cap = (long long)sm_count() * 16;
-    l1_fwd_kernel<<<(unsigned)(want < cap ? want : cap), 256, 0, st>>>(gv(a), gv(b), G, total, sum);
-  }
-  return launched("l1_sum");
+  if (nb) l1_fwd_kernel<<<(unsigned)nb, 256, 0, st>>>(gv(a), gv(b), G, total, (double*)workspace);
+  if ((rc = launched("l1_sum"))) return rc;
+  l1_finish_kernel<<<1, 256, 0, st>>>((const double*)workspace, (int)nb, sum);
+  return launched("l1_sum finish");
 }
 
 extern "C" int hrv_l1_bwd(const hrv_tensor* a, const hrv_tensor* b, const float* gscale, const hrv_tensor* da, int32_t relu_gate, hrv_stream stream) {

@@ -63,4 +63,7 @@ int launch_dyn_smem(const char* name, int grid, int threads, size_t smem, uint32
 }  // namespace hrv_host
 namespace hrv {
 using namespace hrv_host;
+// out[o * out_stride + j] = sum over r < rows of slab[(o * rows + r) * cols + j] (fp64), in a fixed order that does not depend on
+// timing: the finishing pass of the per-block slabs that replace cross-block atomics (csrc/norm_bwd.cu).
+int slab_sum(const double* slab, int outer, int rows, int cols, double* out, int out_stride, cudaStream_t st, const char* what);
 }

@@ -1,7 +1,8 @@
 // norm_bwd.cu — fused backward of the SPADE modulation + InstanceNorm (and of plain InstanceNorm+activation).
 //
 // Forward (network_generator.py:101-122,170-171):  xn = (xs + noise*ns - mean) * rstd ;  v = xn*(1+gamma) + beta ; h = act(v)
-// Backward, two HBM-bound passes (NHWC bf16, 8 channels per thread, fp32 math, fp64 cross-block accumulation):
+// Backward, two HBM-bound passes (NHWC bf16, 8 channels per thread, fp32 math, fp64 per-block sums written to per-block slabs and
+// added in a fixed order by a finishing kernel, so every sum is reproducible run to run):
 //   pass 1 (reduce):  dv = dh*act'(h);  dgamma = dv*xn;  dbeta = dv;  dxn = dv*(1+gamma)
 //                     writes d(gamma|beta) interleaved (the dY of the gamma/beta GEMM) and dxn; accumulates per (n,c):
 //                     S1 = sum dxn, S2 = sum dxn*xn, Sg = sum dgamma, Sb = sum dbeta
@@ -52,7 +53,7 @@ struct BwdArgs {
   const float* mean;
   const float* rstd;
   const float* chan_scale;  // optional per-channel affine weight (BatchNorm): dxn = dv * chan_scale[c]
-  double* acc;  // [N][C][4]
+  double* slab;  // [N][gridDim.x][C][4]
 };
 
 // grid (chunks, N); thread = (pixel lane, channel group)
@@ -121,7 +122,7 @@ __global__ void __launch_bounds__(256) spade_bwd_reduce_kernel(BwdArgs a) {
   for (int j = threadIdx.x; j < C * 4; j += blockDim.x) {
     double t = 0.0;
     for (int l = 0; l < a.PL; ++l) t += (double)shf[(long long)l * C * 4 + j];
-    atomicAdd(&a.acc[(long long)n * C * 4 + j], t);
+    a.slab[((long long)n * gridDim.x + blockIdx.x) * C * 4 + j] = t;
   }
 }
 
@@ -134,7 +135,7 @@ struct ApplyArgs {
   const float* rstd;
   const float* m1;   // [N][C] = S1/HW
   const float* m2;   // [N][C] = S2/HW
-  double* dns;       // [C] accumulated sum dxs*noise (may be null)
+  double* dns_slab;  // [N][gridDim.x][Gs*8] per-block sums of dxs*noise (may be null)
 };
 
 // grid (chunks over src pixels, N); thread = (pixel lane, channel group of src)
@@ -198,13 +199,40 @@ __global__ void __launch_bounds__(256) spade_bwd_apply_kernel(ApplyArgs a) {
     for (int i = 0; i < 8; ++i) dst[i] = dn[i];
   }
   __syncthreads();
-  if (a.dns) {
+  if (a.dns_slab) {
     for (int j = threadIdx.x; j < Cs; j += blockDim.x) {
       double t = 0.0;
       for (int l = 0; l < a.PL; ++l) t += (double)shf[(long long)l * Cs + j];
-      atomicAdd(&a.dns[a.c_off + j], t);
+      a.dns_slab[((long long)n * gridDim.x + blockIdx.x) * Cs + j] = t;
     }
   }
+}
+
+// Finishing pass of the slabs: out[o * out_stride + j] = sum over slab rows r = 0..rows-1 of slab[(o * rows + r) * cols + j].
+// block = 32 columns x 32 row groups, grid = (column chunks, o): thread (j, g) adds rows g, g+32, g+64, ... in that order (coalesced
+// across j), then a fixed shared-memory tree combines the 32 groups.  The order is the same on every launch, and no thread walks
+// the up to ~1000 slabs of a small-image reduction serially.
+__global__ void __launch_bounds__(1024) slab_sum_kernel(const double* __restrict__ slab, int rows, int cols, double* __restrict__ out, int out_stride) {
+  __shared__ double part[32][33];
+  const int j = blockIdx.x * 32 + threadIdx.x, g = threadIdx.y, o = blockIdx.y;
+  double t = 0.0;
+  if (j < cols) {
+    const double* p = slab + (long long)o * rows * cols + j;
+#pragma unroll 4
+    for (int r = g; r < rows; r += 32) t += p[(long long)r * cols];
+  }
+  part[g][threadIdx.x] = t;
+  __syncthreads();
+  for (int s = 16; s > 0; s >>= 1) {
+    if (g < s) part[g][threadIdx.x] += part[g + s][threadIdx.x];
+    __syncthreads();
+  }
+  if (g == 0 && j < cols) out[(long long)o * out_stride + j] = part[0][threadIdx.x];
+}
+int slab_sum(const double* slab, int outer, int rows, int cols, double* out, int out_stride, cudaStream_t st, const char* what) {
+  slab_sum_kernel<<<dim3((unsigned)((cols + 31) / 32), (unsigned)outer), dim3(32, 32), 0, st>>>(slab, rows, cols, out, out_stride);
+  cudaError_t e = cudaGetLastError();
+  return e == cudaSuccess ? HRV_OK : set_error(HRV_ECUDA, "%s launch: %s", what, cudaGetErrorString(e));
 }
 
 static int chk(const hrv_tensor* t, const char* what, bool optional = false) {
@@ -228,10 +256,20 @@ static void plan(long long HW, int N, int G, int& PL, int& chunk, unsigned& gx) 
 
 using namespace hrv;
 
+extern "C" size_t hrv_norm_bwd_reduce_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1, int32_t H, int32_t W) {
+  if (!x0) return 0;
+  const int C = x0->c + ((x1 && x1->ptr) ? x1->c : 0), G = (C + 7) / 8;
+  int PL, chunk;
+  unsigned gx;
+  plan((long long)H * W, x0->n, G > 0 ? G : 1, PL, chunk, gx);
+  return (size_t)x0->n * gx * G * 8 * 4 * sizeof(double);
+}
+
 extern "C" int hrv_norm_bwd_reduce(const hrv_tensor* dh, const hrv_tensor* h, const hrv_tensor* gamma, const hrv_tensor* x0,
                                    int32_t x0_shift, const hrv_tensor* x1, int32_t H, int32_t W, const float* noise,
                                    const float* noise_scale, const float* mean, const float* rstd, const float* chan_scale, int32_t act,
-                                   const hrv_tensor* dgb, const hrv_tensor* dxn, double* sums, hrv_stream stream) {
+                                   const hrv_tensor* dgb, const hrv_tensor* dxn, double* sums, void* workspace, size_t workspace_bytes,
+                                   hrv_stream stream) {
   int rc;
   if ((rc = chk(dh, "norm_bwd dh")) || (rc = chk(x0, "norm_bwd x0")) || (rc = chk(dxn, "norm_bwd dxn")) || (rc = chk(h, "norm_bwd h", act == 0)) ||
       (rc = chk(gamma, "norm_bwd gamma", true)) || (rc = chk(x1, "norm_bwd x1", true)) || (rc = chk(dgb, "norm_bwd dgb", true)))
@@ -245,20 +283,31 @@ extern "C" int hrv_norm_bwd_reduce(const hrv_tensor* dh, const hrv_tensor* h, co
   BwdArgs a;
   a.dh = mkview(dh); a.h = mkview(h); a.gamma = mkview(gamma); a.x0 = mkview(x0); a.x1 = mkview(has1 ? x1 : nullptr); a.dgb = mkview(dgb); a.dxn = mkview(dxn);
   a.x0_shift = x0_shift; a.H = H; a.W = W; a.G = C / 8; a.act = act;
-  a.noise = noise; a.ns = noise_scale; a.mean = mean; a.rstd = rstd; a.chan_scale = chan_scale; a.acc = sums;
+  a.noise = noise; a.ns = noise_scale; a.mean = mean; a.rstd = rstd; a.chan_scale = chan_scale; a.slab = (double*)workspace;
   unsigned gx;
   plan((long long)H * W, N, a.G, a.PL, a.chunk, gx);
+  const size_t need = hrv_norm_bwd_reduce_workspace_bytes(x0, x1, H, W);
+  if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "norm_bwd_reduce: workspace too small (%zu < %zu)", workspace_bytes, need);
   cudaStream_t st = (cudaStream_t)stream;
-  cudaMemsetAsync(sums, 0, (size_t)N * C * 4 * sizeof(double), st);
   spade_bwd_reduce_kernel<<<dim3(gx, N), 256, (size_t)a.PL * C * 4 * sizeof(float), st>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(HRV_ECUDA, "norm_bwd_reduce launch: %s", cudaGetErrorString(e));
-  return HRV_OK;
+  return slab_sum(a.slab, N, (int)gx, C * 4, sums, C * 4, st, "norm_bwd_reduce sum");
+}
+
+extern "C" size_t hrv_norm_bwd_apply_workspace_bytes(const hrv_tensor* src) {
+  if (!src) return 0;
+  const int G = (src->c + 7) / 8;
+  int PL, chunk;
+  unsigned gx;
+  plan((long long)src->h * src->w, src->n, G > 0 ? G : 1, PL, chunk, gx);
+  return (size_t)src->n * gx * G * 8 * sizeof(double);
 }
 
 extern "C" int hrv_norm_bwd_apply(const hrv_tensor* dxn, const hrv_tensor* src, int32_t shift, int32_t c_off, int32_t C, int32_t H,
                                   int32_t W, const float* noise, const float* noise_scale, const float* mean, const float* rstd,
-                                  const float* m1, const float* m2, const hrv_tensor* dx, double* dns, hrv_stream stream) {
+                                  const float* m1, const float* m2, const hrv_tensor* dx, double* dns, void* workspace,
+                                  size_t workspace_bytes, hrv_stream stream) {
   int rc;
   if ((rc = chk(dxn, "norm_bwd_apply dxn")) || (rc = chk(src, "norm_bwd_apply src")) || (rc = chk(dx, "norm_bwd_apply dx"))) return rc;
   if ((src->c % 8) || (c_off % 8) || c_off + src->c > C) return set_error(HRV_EINVAL, "norm_bwd_apply: bad channel slice");
@@ -267,22 +316,31 @@ extern "C" int hrv_norm_bwd_apply(const hrv_tensor* dxn, const hrv_tensor* src, 
   ApplyArgs a;
   a.dxn = mkview(dxn); a.src = mkview(src); a.dx = mkview(dx);
   a.shift = shift; a.H = H; a.W = W; a.G = src->c / 8; a.c_off = c_off; a.C = C;
-  a.noise = noise; a.ns = noise_scale; a.mean = mean; a.rstd = rstd; a.m1 = m1; a.m2 = m2; a.dns = dns;
+  a.noise = noise; a.ns = noise_scale; a.mean = mean; a.rstd = rstd; a.m1 = m1; a.m2 = m2; a.dns_slab = dns ? (double*)workspace : nullptr;
   unsigned gx;
   plan((long long)src->h * src->w, src->n, a.G, a.PL, a.chunk, gx);
+  if (dns) {
+    const size_t need = hrv_norm_bwd_apply_workspace_bytes(src);
+    if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "norm_bwd_apply: workspace too small (%zu < %zu)", workspace_bytes, need);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
   if (a.shift)
-    spade_bwd_apply_kernel<2><<<dim3(gx, src->n), 256, (size_t)a.PL * a.G * 8 * sizeof(float), (cudaStream_t)stream>>>(a);
+    spade_bwd_apply_kernel<2><<<dim3(gx, src->n), 256, (size_t)a.PL * a.G * 8 * sizeof(float), st>>>(a);
   else
-    spade_bwd_apply_kernel<1><<<dim3(gx, src->n), 256, (size_t)a.PL * a.G * 8 * sizeof(float), (cudaStream_t)stream>>>(a);
+    spade_bwd_apply_kernel<1><<<dim3(gx, src->n), 256, (size_t)a.PL * a.G * 8 * sizeof(float), st>>>(a);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(HRV_ECUDA, "norm_bwd_apply launch: %s", cudaGetErrorString(e));
-  return HRV_OK;
+  // one slab row per (n, block): every image's blocks and all images meet in one fixed-order sum
+  return dns ? slab_sum(a.dns_slab, 1, src->n * (int)gx, a.G * 8, dns + c_off, 0, st, "norm_bwd_apply sum") : HRV_OK;
 }
 
 // ------------------------------------------------------------------------------------------------ activation backward + bias gradient
 namespace hrv {
-// dv = dy * act'(y) (bf16, NHWC) and bias_grad[c] += sum over all pixels of dv — one pass instead of where() + float() + sum().
-__global__ void __launch_bounds__(256) act_bwd_bias_kernel(NView dy, NView y, NView dv, int act, int G, int PL, int chunk,
+// dv = dy * act'(y) (bf16, NHWC) and bias_grad[c] = sum over all pixels of dv — one pass instead of where() + float() + sum().
+// kSlab = false: the block sums meet in bsum through fp64 atomics (hrv_act_bwd_bias, order-dependent); kSlab = true: every block
+// writes its sums to row blockIdx.x of the slab bsum[gridDim.x][C], added in a fixed order afterwards (hrv_act_bwd_bias_ordered).
+template <bool kSlab>
+__global__ void __launch_bounds__(256, 1) act_bwd_bias_kernel(NView dy, NView y, NView dv, int act, int G, int PL, int chunk,
                                                           long long npix, double* __restrict__ bsum) {
   extern __shared__ float shf[];  // [PL][C]
   const int C = G * 8;
@@ -339,7 +397,8 @@ __global__ void __launch_bounds__(256) act_bwd_bias_kernel(NView dy, NView y, NV
     for (int j = threadIdx.x; j < C; j += blockDim.x) {
       double t = 0.0;
       for (int l = 0; l < PL; ++l) t += (double)shf[(long long)l * C + j];
-      atomicAdd(&bsum[j], t);
+      if constexpr (kSlab) bsum[(long long)blockIdx.x * C + j] = t;
+      else atomicAdd(&bsum[j], t);
     }
   }
 }
@@ -357,8 +416,39 @@ extern "C" int hrv_act_bwd_bias(const hrv_tensor* dy, const hrv_tensor* y, int32
   plan(npix, 1, G, PL, chunk, gx);
   cudaStream_t st = (cudaStream_t)stream;
   if (bias_sum) cudaMemsetAsync(bias_sum, 0, (size_t)G * 8 * sizeof(double), st);
-  act_bwd_bias_kernel<<<gx, 256, (size_t)PL * G * 8 * sizeof(float), st>>>(mkview(dy), mkview(y), mkview(dv), act, G, PL, chunk, npix, bias_sum);
+  act_bwd_bias_kernel<false><<<gx, 256, (size_t)PL * G * 8 * sizeof(float), st>>>(mkview(dy), mkview(y), mkview(dv), act, G, PL, chunk, npix, bias_sum);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error(HRV_ECUDA, "act_bwd_bias launch: %s", cudaGetErrorString(e));
   return HRV_OK;
+}
+
+extern "C" size_t hrv_act_bwd_bias_ordered_workspace_bytes(const hrv_tensor* dy) {
+  if (!dy) return 0;
+  const int G = (dy->c + 7) / 8;
+  int PL, chunk;
+  unsigned gx;
+  plan((long long)dy->n * dy->h * dy->w, 1, G > 0 ? G : 1, PL, chunk, gx);
+  return (size_t)gx * G * 8 * sizeof(double);
+}
+
+extern "C" int hrv_act_bwd_bias_ordered(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, const hrv_tensor* dv, double* bias_sum,
+                                        void* workspace, size_t workspace_bytes, hrv_stream stream) {
+  int rc;
+  if ((rc = chk(dy, "act_bwd dy")) || (rc = chk(y, "act_bwd y", act == 0)) || (rc = chk(dv, "act_bwd dv", true))) return rc;
+  const int G = (dy->c + 7) / 8;
+  if (G > 256) return set_error(HRV_EUNSUPPORTED, "act_bwd: more than 2048 channels");
+  const long long npix = (long long)dy->n * dy->h * dy->w;
+  int PL, chunk;
+  unsigned gx;
+  plan(npix, 1, G, PL, chunk, gx);
+  if (bias_sum) {
+    const size_t need = hrv_act_bwd_bias_ordered_workspace_bytes(dy);
+    if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "act_bwd_bias_ordered: workspace too small (%zu < %zu)", workspace_bytes, need);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  double* slab = bias_sum ? (double*)workspace : nullptr;
+  act_bwd_bias_kernel<true><<<gx, 256, (size_t)PL * G * 8 * sizeof(float), st>>>(mkview(dy), mkview(y), mkview(dv), act, G, PL, chunk, npix, slab);
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return set_error(HRV_ECUDA, "act_bwd_bias_ordered launch: %s", cudaGetErrorString(e));
+  return bias_sum ? slab_sum(slab, 1, (int)gx, G * 8, bias_sum, 0, st, "act_bwd_bias_ordered sum") : HRV_OK;
 }

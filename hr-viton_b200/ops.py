@@ -333,12 +333,13 @@ def instnorm_stats(x0, x0_shift, x1, h, w, noise, noise_scale, eps=1e-5):
     c = x0.c + (x1.c if x1 is not None else 0)
     mean = torch.empty((n, c), dtype=torch.float32, device=x0.buf.device)
     rstd = torch.empty_like(mean)
-    ws = _workspace(n * c * 16, x0.buf.device)
     t0 = x0.ct()
     t1 = x1.ct() if x1 is not None else _NULL
+    L = _L(x0)
+    ws = _workspace(int(L.hrv_instnorm_stats_workspace_bytes(ctypes.byref(t0), ctypes.byref(t1), h, w)), x0.buf.device)
     nbytes = n * h * w * (2.0 * c + (4.0 if noise is not None else 0.0))  # one bf16 read of every element (+ noise)
-    with _Timed("instnorm_stats", nbytes, launches=3, label="c%d n%d %dx%d shift%d" % (c, n, h, w, x0_shift)):
-        capi.check(_L(x0).hrv_instnorm_stats(ctypes.byref(t0), x0_shift, ctypes.byref(t1), h, w, _p(noise), _p(noise_scale),
+    with _Timed("instnorm_stats", nbytes, launches=2, label="c%d n%d %dx%d shift%d" % (c, n, h, w, x0_shift)):
+        capi.check(L.hrv_instnorm_stats(ctypes.byref(t0), x0_shift, ctypes.byref(t1), h, w, _p(noise), _p(noise_scale),
                                                  eps, mean.data_ptr(), rstd.data_ptr(), ws.data_ptr(), ws.numel(), _stream()),
                    "instnorm_stats")
     return mean, rstd
@@ -353,13 +354,14 @@ def instnorm_stats2(x0, x0_shift, x1, h, w, noises, noise_scales, eps=1e-5):
     assert k in (1, 2) and len(noise_scales) == k
     dev = x0.buf.device
     outs = [(torch.empty((n, c), dtype=torch.float32, device=dev), torch.empty((n, c), dtype=torch.float32, device=dev)) for _ in range(k)]
-    ws = _workspace((n * c * 4 + n * 4) * 8, dev)
     t0 = x0.ct()
     t1 = x1.ct() if x1 is not None else _NULL
+    L = _L(x0)
+    ws = _workspace(int(L.hrv_instnorm_stats2_workspace_bytes(ctypes.byref(t0), ctypes.byref(t1))), dev)
     src_bytes = 2.0 * n * (x0.h * x0.w * x0.c + (h * w * x1.c if x1 is not None else 0)) + 4.0 * n * h * w * sum(z is not None for z in noises)
     nz1, ns1, m1, r1 = (noises[1], noise_scales[1], outs[1][0], outs[1][1]) if k == 2 else (None, None, None, None)
-    with _Timed("instnorm_stats", src_bytes, launches=3 + (1 if x1 is not None else 0), label="c%d n%d %dx%d shift%d norms%d" % (c, n, h, w, x0_shift, k)):
-        capi.check(_L(x0).hrv_instnorm_stats2(ctypes.byref(t0), x0_shift, ctypes.byref(t1), h, w, _p(noises[0]), _p(noise_scales[0]), _p(nz1), _p(ns1),
+    with _Timed("instnorm_stats", src_bytes, launches=2 + (1 if x1 is not None else 0), label="c%d n%d %dx%d shift%d norms%d" % (c, n, h, w, x0_shift, k)):
+        capi.check(L.hrv_instnorm_stats2(ctypes.byref(t0), x0_shift, ctypes.byref(t1), h, w, _p(noises[0]), _p(noise_scales[0]), _p(nz1), _p(ns1),
                                               eps, outs[0][0].data_ptr(), outs[0][1].data_ptr(), _p(m1), _p(r1), ws.data_ptr(), ws.numel(), _stream()),
                    "instnorm_stats2")
     return outs
@@ -428,11 +430,14 @@ def im2col(x, kh, kw, pad, k_pad=None):
 
 
 def l1_sum(a, b):
-    """sum |a - b| as a 1-element fp64 cuda tensor."""
+    """sum |a - b| as a 1-element fp64 cuda tensor (per-block partials added in a fixed order: reproducible)."""
     out = torch.empty(1, dtype=torch.float64, device=a.buf.device)
     ta, tb = a.ct(), b.ct()
-    with _Timed("glue", 0.0, label="l1_sum"):
-        capi.check(_L(a).hrv_l1_sum(ctypes.byref(ta), ctypes.byref(tb), out.data_ptr(), _stream()), "l1_sum")
+    L = _L(a)
+    nws = int(L.hrv_l1_sum_workspace_bytes(ctypes.byref(ta)))
+    ws = torch.empty(max(nws, 8), dtype=torch.uint8, device=a.buf.device)
+    with _Timed("glue", 0.0, launches=2, label="l1_sum"):
+        capi.check(L.hrv_l1_sum(ctypes.byref(ta), ctypes.byref(tb), out.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "l1_sum")
     return out
 
 
@@ -519,6 +524,29 @@ def flow_warp_nchw(flow_lo, src, size, div_xy, want_grid=False, mask=None, overl
     return (out, grid, mask_out) if mask is not None else (out, grid)
 
 
+def flow_warp_nchw_bwd(flow_lo, src, size, div_xy, d_dst, mask=None, d_mask=None):
+    """d flow_lo (N,hl,wl,2) fp32 of flow_warp_nchw (without overlap / composite) from the gradients of the warped cloth d_dst
+    (N,C,H,W) and, optionally, of the warped mask d_mask (N,1,H,W): hrv_flow_warp_nchw_bwd, fixed summation order throughout."""
+    flow_lo, src = flow_lo.contiguous(), src.contiguous()
+    n, hl, wl, _ = flow_lo.shape
+    _, c, hs, ws_ = src.shape
+    H, W = size
+    dev = src.device
+    d_dst = d_dst.float().contiguous() if d_dst is not None else None
+    if d_mask is not None:
+        mask, d_mask = mask.float().contiguous(), d_mask.float().contiguous()
+    dflo = torch.empty((n, hl, wl, 2), dtype=torch.float32, device=dev)
+    L = capi.lib()
+    nws = int(L.hrv_flow_warp_nchw_bwd_workspace_bytes(n, H, W, wl))
+    ws = torch.empty(nws, dtype=torch.uint8, device=dev)
+    with _Timed("glue", 0.0, launches=3, label="flow_warp_nchw_bwd"):
+        capi.check(L.hrv_flow_warp_nchw_bwd(flow_lo.data_ptr(), n, hl, wl, linspace_table(W, dev).data_ptr(), linspace_table(H, dev).data_ptr(),
+                                            src.data_ptr(), c, hs, ws_, _p(d_dst), H, W, float(div_xy[0]), float(div_xy[1]),
+                                            _p(mask if d_mask is not None else None), _p(d_mask), dflo.data_ptr(), ws.data_ptr(), nws, _stream()),
+                   "flow_warp_nchw_bwd")
+    return dflo
+
+
 def avgpool3s2(x):
     out = Act.empty(x.n, (x.h - 1) // 2 + 1, (x.w - 1) // 2 + 1, x.c, pitch=x.pitch if x.c0 == 0 else None)
     tx, ty = x.ct(), out.ct()
@@ -578,10 +606,17 @@ def norm_bwd(dh, h, gamma, x0, x0_shift, x1, noise, noise_scale, mean, rstd, act
     tg = gamma.ct() if gamma is not None else _NULL
     tx1 = x1.ct() if x1 is not None else _NULL
     tdgb = dgb.ct() if dgb is not None else _NULL
+    L = _L(dh)
+    nws = int(L.hrv_norm_bwd_reduce_workspace_bytes(ctypes.byref(tx0), ctypes.byref(tx1), H, W))
+    if noise_scale is not None:
+        nws = max(nws, int(L.hrv_norm_bwd_apply_workspace_bytes(ctypes.byref(tx0))),
+                  int(L.hrv_norm_bwd_apply_workspace_bytes(ctypes.byref(tx1))) if x1 is not None else 0)
+    ws = torch.empty(nws, dtype=torch.uint8, device=dev)  # per-block slabs, added in a fixed order (reproducible sums)
     with _Timed("norm_bwd", n * H * W * C * 2.0 * (4 + (1 if gamma is not None else 0) + (2 if want_dgb else 0)), launches=2):
-        capi.check(_L(dh).hrv_norm_bwd_reduce(ctypes.byref(tdh), ctypes.byref(th), ctypes.byref(tg), ctypes.byref(tx0), x0_shift,
-                                                  ctypes.byref(tx1), H, W, _p(noise), _p(noise_scale), mean.data_ptr(), rstd.data_ptr(),
-                                                  _p(chan_scale), act, ctypes.byref(tdgb), ctypes.byref(tdxn), sums.data_ptr(), _stream()), "norm_bwd_reduce")
+        capi.check(L.hrv_norm_bwd_reduce(ctypes.byref(tdh), ctypes.byref(th), ctypes.byref(tg), ctypes.byref(tx0), x0_shift,
+                                         ctypes.byref(tx1), H, W, _p(noise), _p(noise_scale), mean.data_ptr(), rstd.data_ptr(),
+                                         _p(chan_scale), act, ctypes.byref(tdgb), ctypes.byref(tdxn), sums.data_ptr(), ws.data_ptr(), nws,
+                                         _stream()), "norm_bwd_reduce")
     if batch_stats:  # BatchNorm: the two means run over (N,H,W)
         tot = sums.sum(0, keepdim=True) / float(n * H * W)
         m1 = tot[:, :, 0].expand(n, C).float().contiguous()
@@ -590,21 +625,21 @@ def norm_bwd(dh, h, gamma, x0, x0_shift, x1, noise, noise_scale, mean, rstd, act
         inv = 1.0 / float(H * W)
         m1 = (sums[:, :, 0] * inv).float().contiguous()
         m2 = (sums[:, :, 1] * inv).float().contiguous()
-    dns = torch.zeros(C, dtype=torch.float64, device=dev) if noise_scale is not None else None
+    dns = torch.empty(C, dtype=torch.float64, device=dev) if noise_scale is not None else None
     dx0 = Act.empty(n, x0.h, x0.w, c0)
     tdx0 = dx0.ct()
-    with _Timed("norm_bwd", n * H * W * c0 * 2.0 * 2, launches=1):
-        capi.check(_L(dh).hrv_norm_bwd_apply(ctypes.byref(tdxn), ctypes.byref(tx0), x0_shift, 0, C, H, W, _p(noise), _p(noise_scale),
-                                                 mean.data_ptr(), rstd.data_ptr(), m1.data_ptr(), m2.data_ptr(), ctypes.byref(tdx0),
-                                                 _p(dns), _stream()), "norm_bwd_apply(x0)")
+    with _Timed("norm_bwd", n * H * W * c0 * 2.0 * 2, launches=2 if dns is not None else 1):
+        capi.check(L.hrv_norm_bwd_apply(ctypes.byref(tdxn), ctypes.byref(tx0), x0_shift, 0, C, H, W, _p(noise), _p(noise_scale),
+                                        mean.data_ptr(), rstd.data_ptr(), m1.data_ptr(), m2.data_ptr(), ctypes.byref(tdx0),
+                                        _p(dns), ws.data_ptr(), nws, _stream()), "norm_bwd_apply(x0)")
     dx1 = None
     if x1 is not None:
         dx1 = Act.empty(n, H, W, c1)
         tdx1 = dx1.ct()
-        with _Timed("norm_bwd", n * H * W * c1 * 2.0 * 3, launches=1):
-            capi.check(_L(dh).hrv_norm_bwd_apply(ctypes.byref(tdxn), ctypes.byref(tx1), 0, c0, C, H, W, _p(noise), _p(noise_scale),
-                                                     mean.data_ptr(), rstd.data_ptr(), m1.data_ptr(), m2.data_ptr(), ctypes.byref(tdx1),
-                                                     _p(dns), _stream()), "norm_bwd_apply(x1)")
+        with _Timed("norm_bwd", n * H * W * c1 * 2.0 * 3, launches=2 if dns is not None else 1):
+            capi.check(L.hrv_norm_bwd_apply(ctypes.byref(tdxn), ctypes.byref(tx1), 0, c0, C, H, W, _p(noise), _p(noise_scale),
+                                            mean.data_ptr(), rstd.data_ptr(), m1.data_ptr(), m2.data_ptr(), ctypes.byref(tdx1),
+                                            _p(dns), ws.data_ptr(), nws, _stream()), "norm_bwd_apply(x1)")
     return dgb, dx0, dx1, (dns.float() if dns is not None else None), sums[:, :, 2].sum(0).float(), sums[:, :, 3].sum(0).float()
 
 
@@ -618,8 +653,12 @@ def act_bwd_bias(dy, y, act, want_dv=True, want_bias=True):
     tdy = dy.ct()
     ty = y.ct() if (y is not None and act != ACT_NONE) else _NULL
     tdv = dv.ct() if dv is not None else _NULL
-    with _Timed("act_bwd", dy.n * dy.h * dy.w * dy.c * 2.0 * (3 if dv is not None else 1)):
-        capi.check(_L(dy).hrv_act_bwd_bias(ctypes.byref(tdy), ctypes.byref(ty), act, ctypes.byref(tdv), _p(bsum), _stream()), "act_bwd_bias")
+    L = _L(dy)
+    nws = int(L.hrv_act_bwd_bias_ordered_workspace_bytes(ctypes.byref(tdy))) if bsum is not None else 0
+    ws = torch.empty(nws, dtype=torch.uint8, device=dy.buf.device) if nws else None  # per-block slabs, added in a fixed order
+    with _Timed("act_bwd", dy.n * dy.h * dy.w * dy.c * 2.0 * (3 if dv is not None else 1), launches=2 if bsum is not None else 1):
+        capi.check(L.hrv_act_bwd_bias_ordered(ctypes.byref(tdy), ctypes.byref(ty), act, ctypes.byref(tdv), _p(bsum), _p(ws), nws, _stream()),
+                   "act_bwd_bias_ordered")
     return (dv if dv is not None else dy), (bsum[:dy.c].float() if bsum is not None else None)
 
 
@@ -640,12 +679,13 @@ def batchnorm_stats(x, eps=1e-5):
     """Train-mode BatchNorm2d statistics over (N,H,W) from ONE pass of the statistics kernel (per-image fp64 partial sums combined
     here on [N][C] scalars) — the "single-kernel reduce" standing in for SyncBatchNorm.  Returns (mean[C], biased var[C]) fp32."""
     n, c = x.n, x.c
-    ws = _workspace(n * c * 16, x.buf.device)
     mean_nc = torch.empty((n, c), dtype=torch.float32, device=x.buf.device)
     rstd_nc = torch.empty_like(mean_nc)
     t0 = x.ct()
-    with _Timed("instnorm_stats", n * x.h * x.w * 2.0 * c, launches=3, label="bn c%d n%d %dx%d" % (c, n, x.h, x.w)):
-        capi.check(_L(x).hrv_instnorm_stats(ctypes.byref(t0), 0, ctypes.byref(_NULL), x.h, x.w, None, None, eps, mean_nc.data_ptr(),
+    L = _L(x)
+    ws = _workspace(int(L.hrv_instnorm_stats_workspace_bytes(ctypes.byref(t0), ctypes.byref(_NULL), x.h, x.w)), x.buf.device)
+    with _Timed("instnorm_stats", n * x.h * x.w * 2.0 * c, launches=2, label="bn c%d n%d %dx%d" % (c, n, x.h, x.w)):
+        capi.check(L.hrv_instnorm_stats(ctypes.byref(t0), 0, ctypes.byref(_NULL), x.h, x.w, None, None, eps, mean_nc.data_ptr(),
                                                  rstd_nc.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "batchnorm_stats")
     sums = ws[: n * c * 16].view(torch.float64).view(n, c, 2).sum(0)  # raw sum / sum of squares left in the workspace
     cnt = float(n * x.h * x.w)
@@ -673,18 +713,21 @@ def bilinear_up2_bwd(dout):
 
 
 def flow_warp_bwd(flow_lo, src, ddst, dflow_up_in, want_dsrc=True):
-    """Returns (dsrc bf16 Act | None, dflow_lo fp32 (N,h,w,2))."""
+    """Returns (dsrc bf16 Act | None, dflow_lo fp32 (N,h,w,2)) from the ordered (bit-reproducible) backward."""
     n, hl, wl, _ = flow_lo.shape
     H, W = 2 * hl, 2 * wl
     dev = flow_lo.device
     c8 = round_up(src.c, 8)
-    dsrc32 = torch.zeros((n, src.h, src.w, c8), dtype=torch.float32, device=dev) if want_dsrc else None
+    dsrc32 = torch.empty((n, src.h, src.w, c8), dtype=torch.float32, device=dev) if want_dsrc else None
     dfu = dflow_up_in.float().contiguous().clone() if dflow_up_in is not None else torch.zeros((n, H, W, 2), dtype=torch.float32, device=dev)
     dflo = torch.empty((n, hl, wl, 2), dtype=torch.float32, device=dev)
     ts, td = src.ct(), ddst.ct()
-    with _Timed("flow_warp_bwd", n * H * W * src.c * 2.0 * 3, launches=2):
-        capi.check(_L(src, ddst).hrv_flow_warp_bwd(flow_lo.data_ptr(), linspace_table(W, dev).data_ptr(), linspace_table(H, dev).data_ptr(),
-                                                ctypes.byref(ts), ctypes.byref(td), _p(dsrc32), dfu.data_ptr(), dflo.data_ptr(), _stream()),
-                   "flow_warp_bwd")
+    L = _L(src, ddst)
+    nws = int(L.hrv_flow_warp_bwd_ordered_workspace_bytes(ctypes.byref(ts), ctypes.byref(td)))
+    ws = torch.empty(nws, dtype=torch.uint8, device=dev)
+    with _Timed("flow_warp_bwd", n * H * W * src.c * 2.0 * 3, launches=6 if want_dsrc else 3):
+        capi.check(L.hrv_flow_warp_bwd_ordered(flow_lo.data_ptr(), linspace_table(W, dev).data_ptr(), linspace_table(H, dev).data_ptr(),
+                                               ctypes.byref(ts), ctypes.byref(td), _p(dsrc32), dfu.data_ptr(), dflo.data_ptr(), ws.data_ptr(), nws,
+                                               _stream()), "flow_warp_bwd_ordered")
     dsrc = Act(dsrc32.to(src.buf.dtype)) if want_dsrc else None
     return dsrc, dflo

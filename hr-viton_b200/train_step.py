@@ -301,7 +301,6 @@ class Stage1Trainer(_GraphMixin):
 
     def step(self, batch):
         from . import autograd_g, autograd_tocg
-        from .tocg import make_grid
         ops.require_trainable_storage("Stage1Trainer.step")
         c_paired, im_c, pcm = batch["cloth"], batch["parse_cloth"], batch["pcm"]
         cm_paired = (batch["cloth_mask"] > 0.5).float()
@@ -321,21 +320,15 @@ class Stage1Trainer(_GraphMixin):
             loss_tv = loss_tv + (flow[:, 1:] - flow[:, :-1]).abs().mean() + (flow[:, :, 1:] - flow[:, :, :-1]).abs().mean()
         n, _, ih, iw = c_paired.shape
         if self.interflowloss:
-            key = ("s1grid", n, ih, iw, str(c_paired.device))
-            if key not in _GRID_CACHE:
-                _GRID_CACHE[key] = make_grid(n, ih, iw).to(c_paired.device)
-            grid = _GRID_CACHE[key]
+            # F.interpolate(size, bilinear) + normalise + base grid + grid_sample(border) of cloth and mask: hrv_flow_warp_nchw and its
+            # fixed-order backward (torch's grid_sample / interpolate backward accumulate with atomics)
             for i in range(len(flow_list) - 1):
-                fl = flow_list[i]
-                fh, fw = fl.shape[1], fl.shape[2]
-                fl = F.interpolate(fl.permute(0, 3, 1, 2), size=(ih, iw), mode="bilinear").permute(0, 2, 3, 1)
-                fn = torch.cat([fl[..., 0:1] / ((fw - 1.0) / 2.0), fl[..., 1:2] / ((fh - 1.0) / 2.0)], 3)
-                wc = F.grid_sample(c_paired, fn + grid, padding_mode="border", align_corners=False)
-                wcm = F.grid_sample(cm_paired, fn + grid, padding_mode="border", align_corners=False)
+                fh, fw = flow_list[i].shape[1], flow_list[i].shape[2]
+                wc, wcm = autograd_tocg.FlowWarpNchwFn.apply(flow_list[i], c_paired, cm_paired, (ih, iw), ((fw - 1.0) / 2.0, (fh - 1.0) / 2.0))
                 wcm = self._remove_overlap(F.softmax(seg, dim=1), wcm)
                 loss_l1 = loss_l1 + F.l1_loss(wcm, pcm) / (2 ** (4 - i))
                 loss_vgg = loss_vgg + autograd_g.vgg_loss(self.vgg, self.vgg_weights, wc, im_c) / (2 ** (4 - i))
-        ce = F.cross_entropy(seg, batch["parse_onehot"][:, 0].long(), ignore_index=250)  # utils.cross_entropy2d
+        ce = cross_entropy_ignore(seg, batch["parse_onehot"][:, 0].long(), ignore_index=250)  # utils.cross_entropy2d
         soft = torch.softmax(seg, 1)
         d_in = torch.cat((input1.detach(), input2.detach(), soft), 1)
         loss_g_gan = self._lsgan(autograd_tocg.tocg_discriminator_forward_train(self.D, d_in), True)
@@ -357,6 +350,17 @@ class Stage1Trainer(_GraphMixin):
             self.reducers["D"].reduce()
         self.opt_d.step()
         return {"loss_g": loss_g.detach(), "loss_d": loss_d.detach(), "l1": loss_l1.detach(), "vgg": loss_vgg.detach(), "ce": ce.detach()}
+
+
+def cross_entropy_ignore(logits, target, ignore_index=250):
+    """F.cross_entropy(logits (N,C,H,W), target (N,H,W), ignore_index) (mean over the non-ignored pixels) from elementwise ops and
+    fixed-tree sums: log_softmax, a one-hot comparison and a valid-pixel mask.  Unlike the NLL loss kernel it has a deterministic CUDA
+    forward and backward, so it runs under torch.use_deterministic_algorithms(True)."""
+    logp = F.log_softmax(logits, dim=1)
+    classes = torch.arange(logits.shape[1], device=logits.device).view(1, -1, 1, 1)
+    picked = (logp * (target[:, None] == classes)).sum(1)
+    valid = target != ignore_index
+    return -(picked * valid).sum() / valid.sum()
 
 
 def synthetic_batch_stage1(n, h, w, device, seed=0):

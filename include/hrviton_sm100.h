@@ -113,8 +113,10 @@ int hrv_conv2d_fwd(const hrv_conv_params* p, hrv_stream stream);
 /* Per-(n,c) InstanceNorm statistics of  v = src(c) + noise[n,y,x]*noise_scale[c]  over the h*w pixels of
  * the (virtual) tensor  cat(up2^x0_shift(x0), x1)  — nn.InstanceNorm2d(affine=False) statistics
  * (network_generator.py:86,110; biased variance, eps inside the sqrt) without materialising the sum,
- * the up-sampling or the concatenation.  h,w = statistics extent.  workspace: 2*N*C doubles, zeroed by
- * the call.  Writes mean[N][C], rstd[N][C].  fp32 storage: x0/x1 may be fp32 (both). */
+ * the up-sampling or the concatenation.  h,w = statistics extent.  workspace: hrv_instnorm_stats_workspace_bytes(...) bytes,
+ * 8-byte aligned: every block writes its sums into its own slab, added in a fixed order (reproducible run to run); the first 2*N*C
+ * doubles hold the raw sums {sum v, sum v^2}[N][C] afterwards.  Writes mean[N][C], rstd[N][C].  fp32 storage: x0/x1 may be fp32 (both). */
+size_t hrv_instnorm_stats_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1, int32_t h, int32_t w);
 int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w,
                        const float* noise, const float* noise_scale, float eps,
                        float* mean, float* rstd, void* workspace, size_t workspace_bytes, hrv_stream stream);
@@ -122,7 +124,9 @@ int hrv_instnorm_stats(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor*
 /* The same statistics for up to TWO norms that share the input but draw their own noise (norm_s and norm_0 of a SPADEResBlock,
  * network_generator.py:160-170), from ONE pass over the SOURCE tensors: x0 is read at its own (half) resolution, the noise enters
  * through the sums {sum nz, sum nz^2, sum x*nz} (see csrc/aux_kernels.cu).  noise1 / mean1 / rstd1 may be NULL (one norm).
- * workspace: (4*N*C + 4*N) doubles.  fp32 storage: x0/x1 may be fp32 (both). */
+ * workspace: hrv_instnorm_stats2_workspace_bytes(...) bytes (per-block slabs, added in a fixed order).  fp32 storage: x0/x1 may be
+ * fp32 (both). */
+size_t hrv_instnorm_stats2_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1);
 int hrv_instnorm_stats2(const hrv_tensor* x0, int32_t x0_shift, const hrv_tensor* x1, int32_t h, int32_t w, const float* noise0,
                         const float* noise_scale0, const float* noise1, const float* noise_scale1, float eps, float* mean0,
                         float* rstd0, float* mean1, float* rstd1, void* workspace, size_t workspace_bytes, hrv_stream stream);
@@ -140,21 +144,27 @@ int hrv_norm_apply_affine(const hrv_tensor* x, const float* mean, const float* r
 /* Backward of  h = act(xn*(1+gamma)+beta),  xn = InstanceNorm(cat(up2^x0_shift(x0), x1) + noise*noise_scale)
  * (network_generator.py:101-122,170-171), pass 1 of 2: per element dv = dh*act'(h), dgamma = dv*xn, dbeta = dv,
  * dxn = dv*(1+gamma); writes dgb (bf16 (n,h,w,2C), columns 2c = dgamma_c, 2c+1 = dbeta_c = dY of the gamma|beta GEMM; optional)
- * and dxn (bf16 (n,h,w,C)); accumulates sums[N][C][4] (fp64, zeroed by the call) = {sum dxn, sum dxn*xn, sum dgamma, sum dbeta}.
+ * and dxn (bf16 (n,h,w,C)); writes sums[N][C][4] (fp64) = {sum dxn, sum dxn*xn, sum dgamma, sum dbeta}: per-block slabs in
+ * `workspace` (hrv_norm_bwd_reduce_workspace_bytes(...) bytes, 8-byte aligned), added in a fixed order (reproducible run to run).
  * gamma == NULL means plain Instance/BatchNorm + activation: dxn = dv * chan_scale[c] (chan_scale = the BatchNorm affine weight,
  * NULL = 1). h is ignored when act == NONE. */
+size_t hrv_norm_bwd_reduce_workspace_bytes(const hrv_tensor* x0, const hrv_tensor* x1, int32_t H, int32_t W);
 int hrv_norm_bwd_reduce(const hrv_tensor* dh, const hrv_tensor* h, const hrv_tensor* gamma, const hrv_tensor* x0,
                         int32_t x0_shift, const hrv_tensor* x1, int32_t H, int32_t W, const float* noise,
                         const float* noise_scale, const float* mean, const float* rstd, const float* chan_scale, int32_t act,
-                        const hrv_tensor* dgb, const hrv_tensor* dxn, double* sums, hrv_stream stream);
+                        const hrv_tensor* dgb, const hrv_tensor* dxn, double* sums, void* workspace, size_t workspace_bytes,
+                        hrv_stream stream);
 
 /* Pass 2: InstanceNorm backward dxs = rstd*(dxn - m1 - xn*m2) (m1 = sum dxn / HW, m2 = sum dxn*xn / HW, [N][C] fp32) for the
  * channel slice [c_off, c_off+src.c) of the virtual input; src = x0 (shift = x0_shift: the 2x2 children of every source pixel are
- * summed = backward of the nearest up-sampling) or x1 (shift 0). Writes dx (bf16, src extent) and accumulates
- * dns[c] += sum dxs*noise (fp64 [C], caller-zeroed; may be NULL). */
+ * summed = backward of the nearest up-sampling) or x1 (shift 0). Writes dx (bf16, src extent) and
+ * dns[c] = sum dxs*noise for c in [c_off, c_off+src.c) (fp64; may be NULL), from per-block slabs in `workspace`
+ * (hrv_norm_bwd_apply_workspace_bytes(src) bytes, needed only with dns) added in a fixed order. */
+size_t hrv_norm_bwd_apply_workspace_bytes(const hrv_tensor* src);
 int hrv_norm_bwd_apply(const hrv_tensor* dxn, const hrv_tensor* src, int32_t shift, int32_t c_off, int32_t C, int32_t H,
                        int32_t W, const float* noise, const float* noise_scale, const float* mean, const float* rstd,
-                       const float* m1, const float* m2, const hrv_tensor* dx, double* dns, hrv_stream stream);
+                       const float* m1, const float* m2, const hrv_tensor* dx, double* dns, void* workspace, size_t workspace_bytes,
+                       hrv_stream stream);
 
 /* Convolution weight gradient on wgmma: dw[co][ci][ky][kx] = sum_{n,y,x} dy[n,y,x,co] * x[n,y+ky-pad,x+kx-pad,ci]
  * (stride 1; x: (n,h,w,cin), dy: (n,h+2pad-kh+1, w+2pad-kw+1, cout), both bf16 NHWC; kw <= 4). dw is fp32 in the reference's
@@ -166,8 +176,14 @@ size_t hrv_conv2d_wgrad_workspace_bytes(const hrv_tensor* x, const hrv_tensor* d
 int hrv_conv2d_wgrad(const hrv_tensor* x, const hrv_tensor* dy, int32_t kh, int32_t kw, int32_t pad, float* dw, void* workspace,
                      size_t workspace_bytes, hrv_stream stream);
 
-/* dv = dy * act'(y) on NHWC bf16 (dv optional) and bias_sum[c] = sum over all pixels of dv (fp64 [roundup8(C)], zeroed by the
- * call; optional): the activation backward + bias gradient of a conv epilogue act(conv + b) in one pass. */
+/* dv = dy * act'(y) on NHWC bf16 (dv optional) and bias_sum[c] = sum over all pixels of dv (fp64 [roundup8(C)]; optional):
+ * the activation backward + bias gradient of a conv epilogue act(conv + b) in one pass.  The blocks' sums land in per-block slabs of
+ * `workspace` (hrv_act_bwd_bias_ordered_workspace_bytes(dy) bytes, needed only with bias_sum), added in a fixed order: reproducible. */
+size_t hrv_act_bwd_bias_ordered_workspace_bytes(const hrv_tensor* dy);
+int hrv_act_bwd_bias_ordered(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, const hrv_tensor* dv, double* bias_sum,
+                             void* workspace, size_t workspace_bytes, hrv_stream stream);
+/* Legacy, non-reproducible form of hrv_act_bwd_bias_ordered that the package no longer calls: the block sums meet in bias_sum
+ * (zeroed by the call) through fp64 atomics, so the last bits depend on block timing. */
 int hrv_act_bwd_bias(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, const hrv_tensor* dv, double* bias_sum,
                      hrv_stream stream);
 
@@ -207,12 +223,22 @@ int hrv_flow_warp(const float* flow_lo, const float* lin_x, const float* lin_y, 
  * the gradient w.r.t. `b` is dout itself). */
 int hrv_bilinear_up2_bwd(const hrv_tensor* dout, const hrv_tensor* da, hrv_stream stream);
 
-/* Backward of hrv_flow_warp (F.grid_sample backward with border padding, networks.py:135,152, fused with the flow chain):
- *   dsrc32 [n][H][W][roundup8(c)] fp32, caller-zeroed: += d_dst * lerp weight at the 4 taps (atomic scatter; may be NULL);
+/* Backward of hrv_flow_warp (F.grid_sample backward with border padding, networks.py:135,152, fused with the flow chain),
+ * reproducible bit for bit:
+ *   dsrc32 [n][src.h][src.w][roundup8(c)] fp32, WRITTEN (may be NULL): d_dst * lerp weight gathered at every source pixel from the
+ *          (destination pixel, tap) pairs that sample it, summed in ascending (destination pixel, tap) order without FMA contraction
+ *          (one thread per destination pixel writes the taps, a stable radix sort by source pixel orders them, then a gather);
  *   dflow_up [n][H][W][2] fp32, caller-initialised (zeros, or the gradient arriving directly at the up-sampled flow):
- *            += analytic d/d(flow_up) of the sampled values (zero where the coordinate was clamped; a coordinate exactly
- *               on the border, 0 or size-1, counts as clamped, as in torch's grid_sample backward);
- *   dflow_lo [n][H/2][W/2][2] fp32: written = adjoint of the x2 bilinear flow up-sampling applied to dflow_up (may be NULL). */
+ *            += analytic d/d(flow_up) of the sampled values, added per 8-channel group in ascending group order (zero where the
+ *               coordinate was clamped; a coordinate exactly on the border, 0 or size-1, counts as clamped, as in torch's
+ *               grid_sample backward);
+ *   dflow_lo [n][H/2][W/2][2] fp32: written = adjoint of the x2 bilinear flow up-sampling applied to dflow_up (may be NULL).
+ * workspace: hrv_flow_warp_bwd_ordered_workspace_bytes(src, ddst) bytes, 256-byte aligned (sort keys and values, weights, partials). */
+size_t hrv_flow_warp_bwd_ordered_workspace_bytes(const hrv_tensor* src, const hrv_tensor* ddst);
+int hrv_flow_warp_bwd_ordered(const float* flow_lo, const float* lin_x, const float* lin_y, const hrv_tensor* src, const hrv_tensor* ddst,
+                              float* dsrc32, float* dflow_up, float* dflow_lo, void* workspace, size_t workspace_bytes, hrv_stream stream);
+/* Legacy, non-reproducible form of hrv_flow_warp_bwd_ordered that the package no longer calls: dsrc32 is caller-zeroed and
+ * receives d_dst * weight through fp32 atomics (+=), dflow_up likewise, so the last bits depend on thread timing. */
 int hrv_flow_warp_bwd(const float* flow_lo, const float* lin_x, const float* lin_y, const hrv_tensor* src, const hrv_tensor* ddst,
                       float* dsrc32, float* dflow_up, float* dflow_lo, hrv_stream stream);
 
@@ -262,15 +288,29 @@ int hrv_flow_warp_nchw(const float* flow_lo, int32_t n, int32_t hl, int32_t wl, 
                        float div_y, float* grid_out, const float* mask_src, const float* overlap, float* mask_out,
                        int32_t composite, hrv_stream stream);
 
+/* Backward of hrv_flow_warp_nchw w.r.t. flow_lo only (the cloth and its mask are data; overlap / composite have no backward here:
+ * apply remove_overlap and the composite outside, as differentiable ops).  d_dst (n,c,h,w) and d_mask (n,1,h,w) are the incoming
+ * gradients of the warped cloth and mask (either may be NULL, not both).  Writes d_flow_lo (n,hl,wl,2) fp32: the analytic
+ * grid_sample(border) coordinate gradient per hi-res pixel (channels then mask, in that order; none where the coordinate was clamped
+ * or exactly on the border), times 1/div, then the adjoint of the any-factor bilinear resize (align_corners=False) as a row-then-column
+ * gather in ascending order: reproducible bit for bit.  workspace: hrv_flow_warp_nchw_bwd_workspace_bytes(n, h, w, wl) bytes, 8-byte aligned. */
+size_t hrv_flow_warp_nchw_bwd_workspace_bytes(int32_t n, int32_t h, int32_t w, int32_t wl);
+int hrv_flow_warp_nchw_bwd(const float* flow_lo, int32_t n, int32_t hl, int32_t wl, const float* lin_x, const float* lin_y,
+                           const float* src, int32_t c, int32_t hs, int32_t ws, const float* d_dst, int32_t h, int32_t w,
+                           float div_x, float div_y, const float* mask_src, const float* d_mask, float* d_flow_lo,
+                           void* workspace, size_t workspace_bytes, hrv_stream stream);
+
 /* im2col for tiny-Cin convolutions: dst[n,y,x, (ky*kw+kx)*src.c + ci] = src[n, y+ky-pad, x+kx-pad, ci], zero outside the image
  * and in channels >= kh*kw*src.c.  Lets SPADE's 3x3 mlp_shared convolution over the 7-channel label map
  * (network_generator.py:182-184) run as a single K=64 GEMM block (hrv_conv2d_fwd with kh=kw=1) and its weight gradient as a 1x1.
  * fp32 storage: src and dst fp32. */
 int hrv_im2col(const hrv_tensor* src, const hrv_tensor* dst, int32_t kh, int32_t kw, int32_t pad, hrv_stream stream);
 
-/* L1 feature loss (VGGLoss, networks.py:244-251): *sum = sum |a - b| over the views (fp64); da = sign(a - b) * (*gscale)
+/* L1 feature loss (VGGLoss, networks.py:244-251): *sum = sum |a - b| over the views (fp64; every block writes its partial into
+ * `workspace`, hrv_l1_sum_workspace_bytes(a) bytes, added in a fixed order: reproducible); da = sign(a - b) * (*gscale)
  * (times (a > 0) when relu_gate != 0: the ReLU backward of the producer of a, fused). */
-int hrv_l1_sum(const hrv_tensor* a, const hrv_tensor* b, double* sum, hrv_stream stream);
+size_t hrv_l1_sum_workspace_bytes(const hrv_tensor* a);
+int hrv_l1_sum(const hrv_tensor* a, const hrv_tensor* b, double* sum, void* workspace, size_t workspace_bytes, hrv_stream stream);
 int hrv_l1_bwd(const hrv_tensor* a, const hrv_tensor* b, const float* gscale, const hrv_tensor* da, int32_t relu_gate, hrv_stream stream);
 
 /* fp32 parameter (cout,cin,kh,kw) -> bf16 GEMM operand [kh*kw][n_pad][cin_k] of hrv_conv2d_fwd, zero padded, in one pass.
