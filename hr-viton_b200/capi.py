@@ -18,7 +18,7 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_instnorm_stats_workspace_bytes", "hrv_instnorm_stats2_workspace_bytes", "hrv_norm_bwd_reduce_workspace_bytes",
            "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
-           "hrv_last_error",
+           "hrv_grad_unscale_check", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 
 
@@ -112,6 +112,7 @@ def lib(dtype=None):
     L.hrv_l1_sum_workspace_bytes.argtypes = [TP]
     L.hrv_flow_warp_nchw_bwd.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, vp, sz, vp]
     L.hrv_flow_warp_nchw_bwd_workspace_bytes.argtypes = [i32, i32, i32, i32]
+    L.hrv_grad_unscale_check.argtypes = [vp, i32, vp, vp, vp]
     for name in FLAVOURED:
         twin = getattr(L, name + "_f16")
         twin.argtypes = getattr(L, name).argtypes

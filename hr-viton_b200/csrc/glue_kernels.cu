@@ -566,6 +566,74 @@ __global__ void l1_bwd_kernel(GView a, GView b, GView da, int G, long long total
   st16(reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(da.ptr)) + pix * da.pitch + g * 8, pk8(o));
 }
 
+// ---------------------------------------------------------------------------------------------- loss-scaling gradient pass
+// g *= *inv_scale in place over a device table of fp32 segments; found_inf = 1 if any input element is inf or NaN.  Each segment is
+// cut into chunks of kUnChunk float4 starting at its first 16-byte boundary; chunk k of the concatenated chunk sequence belongs to
+// block k % gridDim.x, so large and small segments spread over all blocks without a prefix-sum table.  Every block walks the whole
+// table, staged through shared memory kUnThreads descriptors at a time.  The block that owns a segment's chunk 0 also handles the
+// (at most 3 + 3) elements before the first and after the last 16-byte boundary.
+constexpr int kUnThreads = 256, kUnVec = 4;
+constexpr long long kUnChunk = (long long)kUnThreads * kUnVec;  // float4 per chunk: 16 KiB
+__device__ __forceinline__ bool nonfinite(float v) { return (__float_as_uint(v) & 0x7f800000u) == 0x7f800000u; }
+__device__ __forceinline__ void unscale1(float& v, float s, bool& bad) {
+  bad |= nonfinite(v);
+  v = __fmul_rn(v, s);
+}
+// the table's pointers come through shared memory: the explicit .global accesses spare the generic-address check
+__device__ __forceinline__ void unscale_at(float* p, float s, bool& bad) {
+  float v = __ldcg(p);
+  unscale1(v, s, bad);
+  __stcg(p, v);
+}
+
+__global__ void __launch_bounds__(kUnThreads) grad_unscale_check_kernel(const hrv_grad_segment* __restrict__ segs, int nseg,
+                                                                        const float* __restrict__ inv_scale, float* __restrict__ found_inf) {
+  __shared__ hrv_grad_segment tab[kUnThreads];
+  const float s = __ldg(inv_scale);
+  const unsigned G = gridDim.x;
+  bool bad = false;
+  unsigned long long base = 0;  // chunks of all earlier segments
+  for (int s0 = 0; s0 < nseg; s0 += kUnThreads) {
+    const int cnt = min(kUnThreads, nseg - s0);
+    __syncthreads();
+    if ((int)threadIdx.x < cnt) tab[threadIdx.x] = segs[s0 + threadIdx.x];
+    __syncthreads();
+    for (int i = 0; i < cnt; ++i) {
+      float* p = tab[i].ptr;
+      const long long n = tab[i].n;
+      const long long head = min(n, (long long)((((uintptr_t)0 - (uintptr_t)p) & 15) >> 2));
+      const long long nv = (n - head) >> 2, tail = n - head - 4 * nv;
+      const long long nc = nv ? (nv + kUnChunk - 1) / kUnChunk : (n ? 1 : 0);
+      const unsigned r = (unsigned)(base % G);
+      long long c = blockIdx.x >= r ? blockIdx.x - r : blockIdx.x + G - r;  // first chunk of this segment owned by this block
+      base += nc;
+      if (c == 0) {
+        if ((long long)threadIdx.x < head) unscale_at(p + threadIdx.x, s, bad);
+        if ((long long)threadIdx.x < tail) unscale_at(p + head + 4 * nv + threadIdx.x, s, bad);
+      }
+      float4* q = reinterpret_cast<float4*>(p + head);
+      for (; c < nc; c += G) {
+        const long long b = c * kUnChunk, lim = min(kUnChunk, nv - b);
+        float4 v[kUnVec];
+#pragma unroll
+        for (int u = 0; u < kUnVec; ++u) {
+          const long long j = threadIdx.x + u * kUnThreads;
+          if (j < lim) v[u] = __ldcg(q + b + j);
+        }
+#pragma unroll
+        for (int u = 0; u < kUnVec; ++u) {
+          const long long j = threadIdx.x + u * kUnThreads;
+          if (j < lim) {
+            unscale1(v[u].x, s, bad); unscale1(v[u].y, s, bad); unscale1(v[u].z, s, bad); unscale1(v[u].w, s, bad);
+            __stcg(q + b + j, v[u]);
+          }
+        }
+      }
+    }
+  }
+  if (__syncthreads_or(bad) && threadIdx.x == 0) *found_inf = 1.f;
+}
+
 }  // namespace
 }  // namespace hrv
 
@@ -770,4 +838,13 @@ extern "C" int hrv_l1_bwd(const hrv_tensor* a, const hrv_tensor* b, const float*
   const long long total = (long long)a->n * a->h * a->w * G;
   if (total) l1_bwd_kernel<<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(gv(a), gv(b), gv(da), G, total, gscale, relu_gate);
   return launched("l1_bwd");
+}
+
+extern "C" int hrv_grad_unscale_check(const hrv_grad_segment* segments, int32_t num_segments, const float* inv_scale, float* found_inf,
+                                      hrv_stream stream) {
+  if (!segments || num_segments < 0 || !inv_scale || !found_inf) return set_error(HRV_EINVAL, "grad_unscale_check: bad arguments");
+  if (num_segments == 0) return HRV_OK;
+  // 8 blocks of 256 threads per SM (the thread limit), 4 x 16 bytes in flight per thread
+  grad_unscale_check_kernel<<<(unsigned)sm_count() * 8, kUnThreads, 0, (cudaStream_t)stream>>>(segments, num_segments, inv_scale, found_inf);
+  return launched("grad_unscale_check");
 }

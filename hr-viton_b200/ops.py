@@ -450,6 +450,25 @@ def l1_bwd(a, b, gscale, relu_gate=False, out=None):
     return da
 
 
+def grad_unscale_check(grads, inv_scale, found_inf, table=None):
+    """In place over the fp32 cuda tensors `grads`: g *= inv_scale, found_inf = 1 where any g was inf / NaN (hrv_grad_unscale_check;
+    inv_scale and found_inf are 1-element fp32 cuda tensors, found_inf is only ever set, never cleared).  The kernel reads a device
+    table {data_ptr, numel} of the tensors: pass the `table` returned by the previous call to reuse it while no tensor has moved.  It is
+    rebuilt (a host-to-device copy) otherwise, which a CUDA-graph capture cannot record.  Returns the table."""
+    key = tuple((g.data_ptr(), g.numel()) for g in grads)
+    if table is None or table[0] != key:
+        for g in grads:
+            assert g.is_cuda and g.dtype == torch.float32 and g.is_contiguous(), "grad_unscale_check needs contiguous fp32 cuda tensors"
+        if torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("grad_unscale_check: the gradient tensors moved during CUDA-graph capture; keep them allocated across steps "
+                               "(zero_grad(set_to_none=False)) and run one step before capturing")
+        table = (key, torch.tensor(key, dtype=torch.int64).reshape(len(key), 2).to(inv_scale.device))
+    with _Timed("glue", 0.0, label="grad_unscale_check"):
+        capi.check(capi.lib().hrv_grad_unscale_check(table[1].data_ptr(), len(key), inv_scale.data_ptr(), found_inf.data_ptr(), _stream()),
+                   "grad_unscale_check")
+    return table
+
+
 def parse_blur_argmax(seg, size, group_of=None, groups=0, want_idx=True, overlap_classes=None):
     """seg (n,c,h,w) fp32 cuda -> (idx (n,1,H,W) int64 | None, onehot (n,groups,H,W) fp32 | None[, overlap (n,1,H,W)]);
     hrv_parse_blur_argmax.  overlap_classes: class ids whose softmax (over the blurred scores) is summed into `overlap`."""

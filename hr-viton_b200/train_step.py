@@ -7,6 +7,7 @@ Hot path = the three networks (kernels of this repo).  The per-step tensor glue 
 import torch
 import torch.nn.functional as F
 
+from . import loss_scale as loss_scale_mod
 from . import ops
 
 _GRID_CACHE = {}
@@ -196,11 +197,36 @@ class _GraphMixin:
         torch.cuda.synchronize()
 
 
-class Stage2Trainer(_GraphMixin):
-    """Holds the optimisers / criteria of train_generator.py:145-159 and runs one step."""
+class _LossScaling:
+    """loss_scale="dynamic": one loss_scale.DynamicLossScaler per loss ("G", "D"), as apex O1 with num_losses=2.  The scaled step keeps
+    every gradient tensor allocated across steps (zero_grad(set_to_none=False)), so the device table of the unscale kernel is built once
+    and a captured graph can run it; with loss_scale=None (the default) the step is exactly the unscaled one."""
+
+    def _init_loss_scale(self, loss_scale, optimizers):
+        device = optimizers["G"].param_groups[0]["params"][0].device
+        self.scalers = loss_scale_mod.make_scalers(loss_scale, list(optimizers), device)
+        for name, sc in self.scalers.items():
+            optimizers[name].found_inf = sc.found_inf  # torch's fused Adam skips the update (and undoes its step count) where it is 1
+
+    def _backward(self, loss, name):
+        sc = self.scalers.get(name)
+        (loss if sc is None else sc.scale_loss(loss)).backward()
+
+    def _opt_step(self, opt, name):
+        sc = self.scalers.get(name)
+        if sc is not None:
+            sc.unscale_and_check(opt, self.reducers.get(name))
+        opt.step()
+        if sc is not None:
+            sc.update()
+
+
+class Stage2Trainer(_GraphMixin, _LossScaling):
+    """Holds the optimisers / criteria of train_generator.py:145-159 and runs one step.  loss_scale: None or "dynamic" (fp16 storage:
+    apex O1's dynamic loss scaling, see loss_scale.py and _LossScaling)."""
 
     def __init__(self, tocg, generator, discriminator, vgg, lambda_feat=10.0, lambda_vgg=10.0, g_lr=1e-4, d_lr=4e-4,
-                 reducers=None, occlusion=True):
+                 reducers=None, occlusion=True, loss_scale=None):
         from .spade import GANLoss
         self.tocg, self.G, self.D, self.vgg = tocg, generator, discriminator, vgg
         self.crit_gan = GANLoss("hinge")
@@ -211,6 +237,7 @@ class Stage2Trainer(_GraphMixin):
         self.opt_d = torch.optim.Adam(discriminator.parameters(), lr=d_lr, betas=(0.0, 0.9), fused=True, capturable=True)
         self.reducers = reducers or {}  # {"G": GradBucketReducer, "D": ...} for data-parallel runs
         self._explicit_reduce = _attach_reducers(self.reducers)
+        self._init_loss_scale(loss_scale, {"G": self.opt_g, "D": self.opt_d})
 
     @staticmethod
     def _split(pred):
@@ -236,11 +263,11 @@ class Stage2Trainer(_GraphMixin):
                 loss_feat = loss_feat + autograd_g.FeatMatchFn.apply(pred[i][j]) * self.lambda_feat / num_d
         loss_vgg = autograd_g.vgg_loss(self.vgg, self.vgg_weights, out, im) * self.lambda_vgg
         loss_gen = (loss_gan + loss_feat + loss_vgg).mean()
-        self.opt_g.zero_grad(set_to_none=True)
-        loss_gen.backward()  # data-parallel: bucket all-reduces are launched from gradient hooks DURING this call (ddp.py)
+        self.opt_g.zero_grad(set_to_none=not self.scalers)
+        self._backward(loss_gen, "G")  # data-parallel: bucket all-reduces are launched from gradient hooks DURING this call (ddp.py)
         if "G" in self.reducers and self._explicit_reduce:
             self.reducers["G"].reduce()
-        self.opt_g.step()
+        self._opt_step(self.opt_g, "G")
         # ---------------- discriminator update (train_generator.py:327-360)
         with torch.no_grad():
             out2 = self.G(g_in, parse)
@@ -248,11 +275,11 @@ class Stage2Trainer(_GraphMixin):
         pred = autograd_g.discriminator_forward_train(self.D, d_in, need_wgrad=True, as_float=False)
         pred_fake, pred_real = self._split(pred)
         loss_dis = (self.crit_gan(pred_fake, False, for_discriminator=True) + self.crit_gan(pred_real, True, for_discriminator=True)).mean()
-        self.opt_d.zero_grad(set_to_none=True)
-        loss_dis.backward()
+        self.opt_d.zero_grad(set_to_none=not self.scalers)
+        self._backward(loss_dis, "D")
         if "D" in self.reducers and self._explicit_reduce:
             self.reducers["D"].reduce()
-        self.opt_d.step()
+        self._opt_step(self.opt_d, "D")
         return {"loss_gen": loss_gen.detach(), "loss_dis": loss_dis.detach(), "gan": loss_gan.detach(),
                 "feat": loss_feat.detach() if torch.is_tensor(loss_feat) else loss_feat, "vgg": loss_vgg.detach()}
 
@@ -276,12 +303,13 @@ def synthetic_batch(n, h, w, device, seed=0):
 
 # ------------------------------------------------------------------------------------------------ stage 1 (train_condition.py)
 
-class Stage1Trainer(_GraphMixin):
+class Stage1Trainer(_GraphMixin, _LossScaling):
     """One train_condition.py step (train_condition.py:133-286) with the README's flags (--Ddownx2 --Ddropout --lasttvonly
-    --interflowloss --occlusion): tocg forward+backward on this repo's kernels (train-mode BatchNorm), L1 + VGG + TV + CE + LSGAN."""
+    --interflowloss --occlusion): tocg forward+backward on this repo's kernels (train-mode BatchNorm), L1 + VGG + TV + CE + LSGAN.
+    loss_scale: None or "dynamic" (as Stage2Trainer)."""
 
     def __init__(self, tocg, D, vgg, lr=2e-4, lasttvonly=True, interflowloss=True, occlusion=True, tvlambda=2.0, ce_lambda=10.0,
-                 gan_lambda=1.0, reducers=None):
+                 gan_lambda=1.0, reducers=None, loss_scale=None):
         self.tocg, self.D, self.vgg = tocg, D, vgg
         self.lasttvonly, self.interflowloss, self.occlusion = lasttvonly, interflowloss, occlusion
         self.tvlambda, self.ce_lambda, self.gan_lambda = tvlambda, ce_lambda, gan_lambda
@@ -290,6 +318,7 @@ class Stage1Trainer(_GraphMixin):
         self.opt_d = torch.optim.Adam(D.parameters(), lr=lr, betas=(0.5, 0.999), fused=True, capturable=True)
         self.reducers = reducers or {}
         self._explicit_reduce = _attach_reducers(self.reducers)
+        self._init_loss_scale(loss_scale, {"G": self.opt_g, "D": self.opt_d})
 
     @staticmethod
     def _remove_overlap(seg_out, warped_cm):  # train_condition.py:26-31
@@ -336,19 +365,19 @@ class Stage1Trainer(_GraphMixin):
         pred_real = autograd_tocg.tocg_discriminator_forward_train(self.D, torch.cat((input1.detach(), input2.detach(), batch["parse"]), 1))
         loss_d = self._lsgan(pred_fake, False) + self._lsgan(pred_real, True)
         loss_g = (10 * loss_l1 + loss_vgg + self.tvlambda * loss_tv) + (ce * self.ce_lambda + loss_g_gan * self.gan_lambda)
-        self.opt_g.zero_grad(set_to_none=True)
-        self.opt_d.zero_grad(set_to_none=True)
-        loss_g.backward()
+        self.opt_g.zero_grad(set_to_none=not self.scalers)
+        self.opt_d.zero_grad(set_to_none=not self.scalers)
+        self._backward(loss_g, "G")
         d_stale = [p.grad for p in self.D.parameters()]  # the G loss also back-propagates into D: the reference zeroes it (optimizer_D.zero_grad)
         if "G" in self.reducers and self._explicit_reduce:
             self.reducers["G"].reduce()
-        self.opt_g.step()
+        self._opt_step(self.opt_g, "G")
         del d_stale
-        self.opt_d.zero_grad(set_to_none=True)
-        loss_d.backward()
+        self.opt_d.zero_grad(set_to_none=not self.scalers)
+        self._backward(loss_d, "D")
         if "D" in self.reducers and self._explicit_reduce:
             self.reducers["D"].reduce()
-        self.opt_d.step()
+        self._opt_step(self.opt_d, "D")
         return {"loss_g": loss_g.detach(), "loss_d": loss_d.detach(), "l1": loss_l1.detach(), "vgg": loss_vgg.detach(), "ce": ce.detach()}
 
 

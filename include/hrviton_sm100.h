@@ -313,6 +313,20 @@ size_t hrv_l1_sum_workspace_bytes(const hrv_tensor* a);
 int hrv_l1_sum(const hrv_tensor* a, const hrv_tensor* b, double* sum, void* workspace, size_t workspace_bytes, hrv_stream stream);
 int hrv_l1_bwd(const hrv_tensor* a, const hrv_tensor* b, const float* gscale, const hrv_tensor* da, int32_t relu_gate, hrv_stream stream);
 
+/* Dynamic loss scaling (the reference's apex-O1 --fp16 runs, train_generator.py:161-169,317-321,355-359): one in-place pass over
+ * fp32 gradient tensors after the backward of a loss multiplied by a scale S.  For every element g of every segment:
+ *   g = g * (*inv_scale)                         (inv_scale: device scalar, read at run time so a graph replay sees the current 1/S)
+ *   *found_inf = 1.0f   if g was inf or NaN      (otherwise *found_inf is left as is: the caller zeroes it before the call)
+ * segments: DEVICE array of num_segments {ptr, n} entries (n fp32 elements at ptr, 4-byte aligned; n may be 0).  Aligned 16-byte
+ * accesses, scalar head and tail.  No workspace; no atomics: every writer of found_inf stores the same value, so the result does not
+ * depend on timing.  With S a power of two the product is exact unless it falls below fp32's normal range. */
+typedef struct hrv_grad_segment {
+  float* ptr;
+  int64_t n;
+} hrv_grad_segment;
+int hrv_grad_unscale_check(const hrv_grad_segment* segments, int32_t num_segments, const float* inv_scale, float* found_inf,
+                           hrv_stream stream);
+
 /* fp32 parameter (cout,cin,kh,kw) -> bf16 GEMM operand [kh*kw][n_pad][cin_k] of hrv_conv2d_fwd, zero padded, in one pass.
  * w1 (optional): second parameter of identical shape whose rows are interleaved with w0's (row 2c = w0[c], 2c+1 = w1[c]: the
  * SPADE gamma|beta GEMM).  transpose_flip != 0 packs the operand of the data-gradient convolution instead (rows = input channels,
