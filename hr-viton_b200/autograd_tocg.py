@@ -7,32 +7,41 @@ dropout of the stage-1 discriminator remain torch ops in this training path."""
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import ddp, ops
 from .autograd_g import AvgPool3S2Fn, FromNCHW, InstNormActFn, conv, space_to_depth_t, _s2d_weight_t
 from .ops import ACT_LRELU, ACT_NONE, ACT_RELU, Act
 
 
 class BatchNormActFn(torch.autograd.Function):
     """y = act(BatchNorm2d_train(x) (+ res)) on a pixel-major bf16 buffer (networks.py:188-198): batch statistics from one pass of the
-    statistics kernel, running statistics updated as torch's BatchNorm2d does (momentum, unbiased variance)."""
+    statistics kernel, running statistics updated as torch's BatchNorm2d does (momentum, unbiased variance).
+    group (SynchronizedBatchNorm2d with several ranks): the statistics, and the two means of the backward, cover the samples of every
+    rank of that process group — one fp64 all-reduce of a [2C+1] buffer per direction (ops.batchnorm_stats_sync, ops.norm_bwd)."""
 
     @staticmethod
-    def forward(ctx, x_buf, weight, bias, res_buf, bn, act):
+    def forward(ctx, x_buf, weight, bias, res_buf, bn, act, group=None):
         c = weight.shape[0]
         c8 = ops.round_up(c, 8)  # kernels work on groups of 8 channels; pad channels hold zeros and get weight = bias = 0
         a = Act(x_buf, c=c8)
         n = a.n
-        mean, var = ops.batchnorm_stats(a, bn.eps)
-        if bn.track_running_stats and bn.training:
-            with torch.no_grad():
-                cnt = float(n * a.h * a.w)
-                m = bn.momentum if bn.momentum is not None else 0.1
-                bn.running_mean.mul_(1 - m).add_(mean[:c] * m)
-                bn.running_var.mul_(1 - m).add_(var[:c] * (cnt / max(cnt - 1.0, 1.0)) * m)
+        update = bn.track_running_stats and bn.training
+        m = bn.momentum if bn.momentum is not None else 0.1
+        if group is not None:
+            mean_nc, rstd_nc = ops.batchnorm_stats_sync(a, bn.eps, lambda wire: ddp.syncbn_all_reduce(wire, group),
+                                                        bn.running_mean if update else None, bn.running_var if update else None, m)
+            if update:
                 bn.num_batches_tracked += 1
-        rstd = torch.rsqrt(var + bn.eps)
-        mean_nc = mean[None].expand(n, c8).contiguous()
-        rstd_nc = rstd[None].expand(n, c8).contiguous()
+        else:
+            mean, var = ops.batchnorm_stats(a, bn.eps)
+            if update:
+                with torch.no_grad():
+                    cnt = float(n * a.h * a.w)
+                    bn.running_mean.mul_(1 - m).add_(mean[:c] * m)
+                    bn.running_var.mul_(1 - m).add_(var[:c] * (cnt / max(cnt - 1.0, 1.0)) * m)
+                    bn.num_batches_tracked += 1
+            rstd = torch.rsqrt(var + bn.eps)
+            mean_nc = mean[None].expand(n, c8).contiguous()
+            rstd_nc = rstd[None].expand(n, c8).contiguous()
         w32 = torch.zeros(c8, dtype=torch.float32, device=x_buf.device)
         b32 = torch.zeros(c8, dtype=torch.float32, device=x_buf.device)
         w32[:c] = weight.detach().float()
@@ -40,6 +49,7 @@ class BatchNormActFn(torch.autograd.Function):
         y = ops.norm_apply_affine(a, mean_nc, rstd_nc, w32, b32, Act(res_buf, c=c8) if res_buf is not None else None, act)
         ctx.save_for_backward(x_buf, w32, mean_nc, rstd_nc, y.buf)
         ctx.meta = (act, res_buf is not None, c, c8)
+        ctx.group = group
         return y.buf
 
     @staticmethod
@@ -47,15 +57,17 @@ class BatchNormActFn(torch.autograd.Function):
         x_buf, w32, mean_nc, rstd_nc, y = ctx.saved_tensors
         act, has_res, c, c8 = ctx.meta
         dya = Act(dy.contiguous(), c=c8)
+        group = ctx.group
         _, dx, _, _, dgamma, dbeta = ops.norm_bwd(dya, Act(y, c=c8), None, Act(x_buf, c=c8), 0, None, None, None, mean_nc, rstd_nc, act,
-                                                  want_dgb=False, chan_scale=w32, batch_stats=True)
+                                                  want_dgb=False, chan_scale=w32, batch_stats=True,
+                                                  all_reduce=None if group is None else (lambda wire: ddp.syncbn_all_reduce(wire, group)))
         dres = None
         if has_res and ctx.needs_input_grad[3]:
             dres = ops.act_bwd_bias(dya, Act(y, c=c8), act, want_bias=False)[0].buf
         dxb = dx.buf
         if dxb.shape[3] != x_buf.shape[3]:
             dxb = F.pad(dxb, (0, x_buf.shape[3] - dxb.shape[3]))
-        return dxb, dgamma[:c].contiguous(), dbeta[:c].contiguous(), dres, None, None
+        return dxb, dgamma[:c].contiguous(), dbeta[:c].contiguous(), dres, None, None, None
 
 
 class Up2Fn(torch.autograd.Function):
@@ -134,8 +146,10 @@ def _resblock(rb, x_buf):
     else:
         r = _up2(conv(x_buf, rb.scale[1].weight, rb.scale[1].bias, pad=0))  # 1x1 commuted below the up-sampling (kernel fwd + bwd)
     bn0, bn1 = rb.block[1], rb.block[4]
-    h = BatchNormActFn.apply(conv(r, rb.block[0].weight, rb.block[0].bias), bn0.weight, bn0.bias, None, bn0, ACT_RELU)
-    return BatchNormActFn.apply(conv(h, rb.block[3].weight, rb.block[3].bias), bn1.weight, bn1.bias, r, bn1, ACT_RELU)
+    g0 = ddp.syncbn_group() if isinstance(bn0, ddp.SynchronizedBatchNorm2d) else None
+    g1 = ddp.syncbn_group() if isinstance(bn1, ddp.SynchronizedBatchNorm2d) else None
+    h = BatchNormActFn.apply(conv(r, rb.block[0].weight, rb.block[0].bias), bn0.weight, bn0.bias, None, bn0, ACT_RELU, g0)
+    return BatchNormActFn.apply(conv(h, rb.block[3].weight, rb.block[3].bias), bn1.weight, bn1.bias, r, bn1, ACT_RELU, g1)
 
 
 _GRIDS = {}

@@ -18,7 +18,7 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_instnorm_stats_workspace_bytes", "hrv_instnorm_stats2_workspace_bytes", "hrv_norm_bwd_reduce_workspace_bytes",
            "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
-           "hrv_grad_unscale_check", "hrv_last_error",
+           "hrv_grad_unscale_check", "hrv_syncbn_combine", "hrv_syncbn_fwd_finalize", "hrv_syncbn_bwd_finalize", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 
 
@@ -113,6 +113,10 @@ def lib(dtype=None):
     L.hrv_flow_warp_nchw_bwd.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, vp, sz, vp]
     L.hrv_flow_warp_nchw_bwd_workspace_bytes.argtypes = [i32, i32, i32, i32]
     L.hrv_grad_unscale_check.argtypes = [vp, i32, vp, vp, vp]
+    f64 = ctypes.c_double
+    L.hrv_syncbn_combine.argtypes = [vp, i32, i32, i32, f64, vp, vp]
+    L.hrv_syncbn_fwd_finalize.argtypes = [vp, i32, i32, i32, f32, f64, vp, vp, vp, vp, vp]
+    L.hrv_syncbn_bwd_finalize.argtypes = [vp, i32, i32, vp, vp, vp]
     for name in FLAVOURED:
         twin = getattr(L, name + "_f16")
         twin.argtypes = getattr(L, name).argtypes

@@ -42,7 +42,8 @@ def broadcast_module_state(module, src=0, group=None):
 
 def average_module_buffers(module, group=None):
     """Averages floating-point buffers (BatchNorm running_mean/var) over ranks and re-broadcasts the rest from rank 0 —
-    call before saving a checkpoint so that the saved statistics describe the global batch, not rank 0's shard."""
+    call before saving a checkpoint so that the saved statistics describe the global batch, not rank 0's shard.  Not needed for a
+    model whose BatchNorm layers are all SynchronizedBatchNorm2d: every rank updates them from the same global statistics."""
     w = _world(group)
     if w == 1:
         return
@@ -231,6 +232,8 @@ class DataParallelWithCallback(nn.Module):
             broadcast_module_state(module)
             if params:
                 self._reducer = GradBucketReducer(params).attach()
+            if any(isinstance(m, SynchronizedBatchNorm2d) for m in module.modules()):
+                syncbn_group()  # made here, at the same point on every rank (new_group is collective)
 
     def forward(self, *args, **kwargs):
         return self.module(*args, **kwargs)
@@ -240,3 +243,88 @@ class DataParallelWithCallback(nn.Module):
         if self._reducer is None or self._reducer._hooks:
             return 0
         return self._reducer.reduce()
+
+
+# ------------------------------------------------------------------------------------------------ synchronised BatchNorm
+
+_SYNCBN_GROUP = [None, None]  # (default process group it was made from, the SyncBN group)
+
+
+def syncbn_group():
+    """The process group of SynchronizedBatchNorm2d's collectives, or None with one process (the layers then run the per-rank
+    path, which is the same computation).  Same ranks as the default group but its own communicator: the gradient buckets are
+    all-reduced asynchronously from hooks while backward() runs, and the statistics exchange must not queue behind them or depend
+    on how the two interleave.  Made on first use; new_group is collective, so every rank reaches that point together."""
+    if _world() == 1:
+        return None
+    default = dist.distributed_c10d._get_default_group()
+    if _SYNCBN_GROUP[0] is not default:
+        _SYNCBN_GROUP[1] = dist.new_group(ranks=list(range(dist.get_world_size())), backend=dist.get_backend())
+        _SYNCBN_GROUP[0] = default
+    return _SYNCBN_GROUP[1]
+
+
+def syncbn_all_reduce(buf, group):
+    """In-place sum of a SyncBN wire buffer (fp64, on the GPU) over `group`, ordered on the current stream.  NCCL reduces it on the
+    device (and can be captured in a CUDA graph); gloo reduces in host memory, so the buffer is staged there."""
+    if dist.get_backend(group) == "gloo":
+        host = buf.cpu()
+        dist.all_reduce(host, op=dist.ReduceOp.SUM, group=group)
+        buf.copy_(host)
+    else:
+        dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
+
+
+class SynchronizedBatchNorm2d(nn.BatchNorm2d):
+    """sync_batchnorm.SynchronizedBatchNorm2d: BatchNorm2d whose train-mode statistics cover the batch of every data-parallel rank.
+    Same constructor defaults and state_dict as nn.BatchNorm2d, so checkpoints load either way.  Inside ConditionGenerator /
+    ResBlock training each layer exchanges one fp64 buffer of per-channel sums per direction (hrviton_b200.autograd_tocg); with one
+    process it runs exactly the nn.BatchNorm2d path.  Eval mode uses the running statistics (folded into the convolution).  The
+    affine gradients stay per rank: the gradient average over ranks then equals torch.nn.SyncBatchNorm's."""
+
+    def __init__(self, num_features, eps=1e-5, momentum=0.1, affine=True):
+        super().__init__(num_features, eps=eps, momentum=momentum, affine=affine)
+
+    def forward(self, input):
+        if self.training and _world() > 1:
+            raise NotImplementedError("a standalone SynchronizedBatchNorm2d has no synchronised kernel path: its statistics are exchanged "
+                                      "inside ConditionGenerator / ResBlock training")
+        return super().forward(input)
+
+
+class SynchronizedBatchNorm1d(nn.BatchNorm1d):
+    """Import parity with the reference's sync_batchnorm: no model here has 1-D BatchNorm, so using it raises."""
+
+    def forward(self, input):
+        raise NotImplementedError("SynchronizedBatchNorm1d is not implemented (only SynchronizedBatchNorm2d is)")
+
+
+class SynchronizedBatchNorm3d(nn.BatchNorm3d):
+    """Import parity with the reference's sync_batchnorm: no model here has 3-D BatchNorm, so using it raises."""
+
+    def forward(self, input):
+        raise NotImplementedError("SynchronizedBatchNorm3d is not implemented (only SynchronizedBatchNorm2d is)")
+
+
+def convert_model(module):
+    """sync_batchnorm.convert_model for 2-D BatchNorm: returns `module` with every nn.BatchNorm2d replaced by a SynchronizedBatchNorm2d
+    that keeps its running statistics (the same buffers), affine parameters (copies) and train/eval mode.  A module wrapped in
+    nn.DataParallel or DataParallelWithCallback comes back wrapped in a new DataParallelWithCallback (the old wrapper's gradient hooks
+    are removed: they belong to parameters that have been replaced)."""
+    if isinstance(module, (nn.DataParallel, DataParallelWithCallback)):
+        if isinstance(module, DataParallelWithCallback) and module._reducer is not None:
+            module._reducer.detach()
+        return DataParallelWithCallback(convert_model(module.module), device_ids=module.device_ids)
+    mod = module
+    if isinstance(module, nn.BatchNorm2d) and not isinstance(module, SynchronizedBatchNorm2d):
+        mod = SynchronizedBatchNorm2d(module.num_features, module.eps, module.momentum, module.affine)
+        mod.running_mean = module.running_mean
+        mod.running_var = module.running_var
+        mod.num_batches_tracked = module.num_batches_tracked
+        if module.affine:
+            mod.weight = nn.Parameter(module.weight.detach().clone(), requires_grad=module.weight.requires_grad)
+            mod.bias = nn.Parameter(module.bias.detach().clone(), requires_grad=module.bias.requires_grad)
+        mod.train(module.training)
+    for name, child in module.named_children():
+        mod.add_module(name, convert_model(child))
+    return mod

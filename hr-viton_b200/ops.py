@@ -609,8 +609,11 @@ def flow_warp(flow_lo, src, dst, want_flow_up=True, want_idx=False):
     return flow_up, idx
 
 
-def norm_bwd(dh, h, gamma, x0, x0_shift, x1, noise, noise_scale, mean, rstd, act, want_dgb, chan_scale=None, batch_stats=False):
+def norm_bwd(dh, h, gamma, x0, x0_shift, x1, noise, noise_scale, mean, rstd, act, want_dgb, chan_scale=None, batch_stats=False,
+             all_reduce=None):
     """Fused backward of the SPADE modulation + InstanceNorm (gamma given) or of InstanceNorm + activation (gamma None).
+    all_reduce (with batch_stats): synchronised BatchNorm — the two means run over the pixels of every rank: the local sums go through
+    one wire buffer that all_reduce sums over the ranks in place.  sum_dgamma / sum_dbeta stay local.
     Returns (dgb Act | None, dx0 Act, dx1 Act | None, d_noise_scale fp32 [C] | None, sum_dgamma fp32 [C], sum_dbeta fp32 [C])."""
     n, H, W = dh.n, dh.h, dh.w
     c0 = x0.c
@@ -636,7 +639,14 @@ def norm_bwd(dh, h, gamma, x0, x0_shift, x1, noise, noise_scale, mean, rstd, act
                                          ctypes.byref(tx1), H, W, _p(noise), _p(noise_scale), mean.data_ptr(), rstd.data_ptr(),
                                          _p(chan_scale), act, ctypes.byref(tdgb), ctypes.byref(tdxn), sums.data_ptr(), ws.data_ptr(), nws,
                                          _stream()), "norm_bwd_reduce")
-    if batch_stats:  # BatchNorm: the two means run over (N,H,W)
+    if batch_stats and all_reduce is not None:
+        wire = syncbn_combine(sums, 4, n * H * W)
+        all_reduce(wire)
+        m1 = torch.empty((n, C), dtype=torch.float32, device=dev)
+        m2 = torch.empty_like(m1)
+        with _Timed("syncbn", C * 16.0, label="bwd_finalize c%d" % C):
+            capi.check(capi.lib().hrv_syncbn_bwd_finalize(wire.data_ptr(), n, C, m1.data_ptr(), m2.data_ptr(), _stream()), "syncbn_bwd_finalize")
+    elif batch_stats:  # BatchNorm: the two means run over (N,H,W)
         tot = sums.sum(0, keepdim=True) / float(n * H * W)
         m1 = tot[:, :, 0].expand(n, C).float().contiguous()
         m2 = tot[:, :, 1].expand(n, C).float().contiguous()
@@ -711,6 +721,43 @@ def batchnorm_stats(x, eps=1e-5):
     mean = sums[:, 0] / cnt
     var = (sums[:, 1] / cnt - mean * mean).clamp_min(0.0)
     return mean.float(), var.float()
+
+
+def syncbn_combine(sums, stride, count):
+    """The fp64 wire buffer [2C+1] of one synchronised BatchNorm layer: per-channel sums of columns 0 and 1 of `sums` ([N][C][stride]
+    fp64, contiguous) over the local images, in image order, followed by the element count `count` (hrv_syncbn_combine)."""
+    assert sums.dtype == torch.float64 and sums.is_contiguous() and sums.shape[2] == stride
+    n, c = sums.shape[0], sums.shape[1]
+    wire = torch.empty(2 * c + 1, dtype=torch.float64, device=sums.device)
+    with _Timed("syncbn", n * c * 16.0, label="combine c%d n%d" % (c, n)):
+        capi.check(capi.lib().hrv_syncbn_combine(sums.data_ptr(), n, c, stride, float(count), wire.data_ptr(), _stream()), "syncbn_combine")
+    return wire
+
+
+def batchnorm_stats_sync(x, eps, all_reduce, running_mean=None, running_var=None, momentum=0.1):
+    """Train-mode BatchNorm2d statistics over the (N,H,W) of every rank: the statistics kernel on the local shard, its per-image sums
+    combined into one wire buffer, all_reduce(wire) (in place, sum over the ranks), then hrv_syncbn_fwd_finalize.  Updates
+    running_mean / running_var (fp32 [c_run], c_run <= x.c; optional) in place.  Returns (mean [N][C], rstd [N][C]) fp32, the tables
+    of norm_apply_affine."""
+    n, c = x.n, x.c
+    mean_nc = torch.empty((n, c), dtype=torch.float32, device=x.buf.device)
+    rstd_nc = torch.empty_like(mean_nc)
+    t0 = x.ct()
+    L = _L(x)
+    ws = _workspace(int(L.hrv_instnorm_stats_workspace_bytes(ctypes.byref(t0), ctypes.byref(_NULL), x.h, x.w)), x.buf.device)
+    with _Timed("instnorm_stats", n * x.h * x.w * 2.0 * c, launches=2, label="syncbn c%d n%d %dx%d" % (c, n, x.h, x.w)):
+        capi.check(L.hrv_instnorm_stats(ctypes.byref(t0), 0, ctypes.byref(_NULL), x.h, x.w, None, None, eps, mean_nc.data_ptr(),
+                                        rstd_nc.data_ptr(), ws.data_ptr(), ws.numel(), _stream()), "batchnorm_stats_sync")
+    wire = syncbn_combine(ws[: n * c * 16].view(torch.float64).view(n, c, 2), 2, n * x.h * x.w)
+    all_reduce(wire)
+    c_run = 0
+    if running_mean is not None:
+        assert running_mean.dtype == torch.float32 and running_var.dtype == torch.float32 and running_mean.is_contiguous()
+        c_run = running_mean.numel()
+    with _Timed("syncbn", c * 16.0, label="fwd_finalize c%d" % c):
+        capi.check(capi.lib().hrv_syncbn_fwd_finalize(wire.data_ptr(), n, c, c_run, eps, float(momentum), mean_nc.data_ptr(), rstd_nc.data_ptr(),
+                                                      _p(running_mean), _p(running_var), _stream()), "syncbn_fwd_finalize")
+    return mean_nc, rstd_nc
 
 
 def norm_apply_affine(x, mean_nc, rstd_nc, gamma, beta, res, act, out=None):

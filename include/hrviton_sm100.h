@@ -327,6 +327,27 @@ typedef struct hrv_grad_segment {
 int hrv_grad_unscale_check(const hrv_grad_segment* segments, int32_t num_segments, const float* inv_scale, float* found_inf,
                            hrv_stream stream);
 
+/* Synchronised train-mode BatchNorm2d across data-parallel ranks (the reference's sync_batchnorm.SynchronizedBatchNorm2d): each
+ * rank reduces its shard with the kernels above, the caller all-reduces (sum) one fp64 wire buffer per layer and direction, and a
+ * finalize kernel turns the global sums into the per-image tables the apply kernels read.  No atomics: reproducible run to run.
+ *
+ * Combine: wire[2c + k] = sum over images i = 0..n-1, added in index order, of sums[(i*c_count + c)*stride + k] (k = 0, 1), and
+ * wire[2*c_count] = count (the elements behind the sums: n*h*w).  sums = the {sum x, sum x^2}[n][C] hrv_instnorm_stats leaves at the
+ * start of its workspace (stride 2), or the {sum dxn, sum dxn*xn, ...}[n][C][4] of hrv_norm_bwd_reduce (stride 4).  The wire holds
+ * 2*c_count + 1 doubles; since the count is summed with the sums, ranks with unequal shards are still normalised by the global count. */
+int hrv_syncbn_combine(const double* sums, int32_t n, int32_t c_count, int32_t stride, double count, double* wire, hrv_stream stream);
+
+/* Forward finalize of the all-reduced wire (2*c + 1 doubles): mean = S1/count and biased var = S2/count - mean^2 (>= 0) in fp64,
+ * rounded to fp32; rstd = rsqrtf(var + eps) in fp32 (the arithmetic of the per-rank BatchNorm path).  Writes mean[n][c], rstd[n][c] (fp32, the same row for every image: the layout of
+ * hrv_norm_apply_affine).  running_mean / running_var (fp32 [c_run], both or neither) are updated in place for channels < c_run
+ * as torch's BatchNorm2d does: r = r*(1-momentum) + x*momentum, the variance with the unbiased factor count/(count-1). */
+int hrv_syncbn_fwd_finalize(const double* wire, int32_t n, int32_t c, int32_t c_run, float eps, double momentum, float* mean,
+                            float* rstd, float* running_mean, float* running_var, hrv_stream stream);
+
+/* Backward finalize of the all-reduced wire of the backward sums: m1[n][c] = S1/count, m2[n][c] = S2/count (fp32), the inputs of
+ * hrv_norm_bwd_apply for BatchNorm statistics over every rank's pixels. */
+int hrv_syncbn_bwd_finalize(const double* wire, int32_t n, int32_t c, float* m1, float* m2, hrv_stream stream);
+
 /* fp32 parameter (cout,cin,kh,kw) -> bf16 GEMM operand [kh*kw][n_pad][cin_k] of hrv_conv2d_fwd, zero padded, in one pass.
  * w1 (optional): second parameter of identical shape whose rows are interleaved with w0's (row 2c = w0[c], 2c+1 = w1[c]: the
  * SPADE gamma|beta GEMM).  transpose_flip != 0 packs the operand of the data-gradient convolution instead (rows = input channels,
