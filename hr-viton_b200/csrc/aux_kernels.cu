@@ -316,9 +316,10 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, int C, int SH
   const int x = (int)(pix % dst.w);
   const int y = (int)((pix / dst.w) % dst.h);
   const int n = (int)(pix / ((long long)dst.w * dst.h));
-  // src = floor(dst * in / out): exact in integers
-  const int sy = (int)(((long long)y * SH) / dst.h);
-  const int sx = (int)(((long long)x * SW) / dst.w);
+  // F.interpolate(mode='nearest'): src = min(floor(dst * (in / out)), in - 1) with the scale and the product rounded to fp32, as torch
+  // computes it.  The exact integer floor(dst * in / out) picks the next pixel where the fp32 product falls just below an integer.
+  const int sy = min((int)floorf(__fmul_rn((float)y, __fdiv_rn((float)SH, (float)dst.h))), SH - 1);
+  const int sx = min((int)floorf(__fmul_rn((float)x, __fdiv_rn((float)SW, (float)dst.w))), SW - 1);
   float f[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {

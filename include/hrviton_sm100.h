@@ -187,8 +187,9 @@ int hrv_act_bwd_bias_ordered(const hrv_tensor* dy, const hrv_tensor* y, int32_t 
 int hrv_act_bwd_bias(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, const hrv_tensor* dv, double* bias_sum,
                      hrv_stream stream);
 
-/* fp32 NCHW -> bf16 NHWC with nearest resampling to (dst.h, dst.w): src index = floor(dst*in/out)
- * (F.interpolate(mode='nearest'), network_generator.py:164,222) and zero fill of dst channels >= C.
+/* fp32 NCHW -> bf16 NHWC with nearest resampling to (dst.h, dst.w): src index = min(floorf(dst * (in/out)), in-1), the scale
+ * in/out and the product rounded to fp32 as F.interpolate(mode='nearest') computes them (network_generator.py:164,222; not the
+ * exact floor(dst*in/out), which differs where the fp32 product falls just below an integer), and zero fill of dst channels >= C.
  * src: [n][c][src_h][src_w] fp32 contiguous.  fp32 storage: dst may be fp32 NHWC. */
 int hrv_nchw_to_nhwc(const float* src, int32_t c, int32_t src_h, int32_t src_w, const hrv_tensor* dst, hrv_stream stream);
 

@@ -57,10 +57,16 @@ def np_bilinear_up2(x):
 
 
 def np_nearest_resize(x, oh, ow):
-    """F.interpolate(mode='nearest'): src = floor(dst * in / out) (network_generator.py:164,222)."""
+    """F.interpolate(mode='nearest'): src = min(floor(dst * (in / out)), in - 1) with the scale and the product rounded to fp32, as
+    torch computes them (network_generator.py:164,222).  The exact floor(dst * in / out) differs where the fp32 product falls just
+    below an integer (200 -> 24: dst 15 reads row 124, not 125)."""
     h, w = x.shape[-2:]
-    yi = np.minimum(np.floor(np.arange(oh) * (h / oh)).astype(np.int64), h - 1)
-    xi = np.minimum(np.floor(np.arange(ow) * (w / ow)).astype(np.int64), w - 1)
+
+    def idx(n_in, n_out):
+        scale = np.float32(n_in) / np.float32(n_out)
+        return np.minimum(np.floor(np.arange(n_out, dtype=np.float32) * scale).astype(np.int64), n_in - 1)
+
+    yi, xi = idx(h, oh), idx(w, ow)
     return x[..., yi[:, None], xi[None, :]]
 
 

@@ -89,6 +89,10 @@ def test_np_nearest_and_pool():
     for oh, ow in [(8, 6), (32, 24), (2, 1), (4, 3)]:
         ref = F.interpolate(x, size=(oh, ow), mode="nearest")
         assert maxdiff(orc.np_nearest_resize(x.numpy(), oh, ow), ref) == 0.0
+    # non-dyadic ratios, where torch's fp32 index floor(dst * (in / out)) differs from the exact floor(dst * in / out)
+    for (ih, iw), (oh, ow) in [((200, 336), (24, 80)), ((336, 200), (80, 24)), ((37, 199), (259, 7))]:
+        z = torch.arange(ih * iw, dtype=torch.float32).reshape(1, 1, ih, iw)
+        assert maxdiff(orc.np_nearest_resize(z.numpy(), oh, ow), F.interpolate(z, size=(oh, ow), mode="nearest")) == 0.0
     for hh, ww in [(16, 12), (17, 13), (9, 7)]:
         y = synth.uniform((1, 2, hh, ww), 3, "p%d" % hh)
         ref = F.avg_pool2d(y, 3, stride=2, padding=1, count_include_pad=False)
