@@ -10,6 +10,8 @@ import torch
 import torch.nn.functional as F
 
 from . import ops
+from .graphs import CapturedCall
+from .spade import _param_key
 from .train_step import GROUP_OF_13, OCCLUSION_CLASSES
 
 
@@ -38,6 +40,123 @@ def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_c
             warped_cloth, _ = ops.flow_warp_nchw(flow_list[-1], clothes.float(), (ih, iw), div)
         output = generator(torch.cat((agnostic, densepose, warped_cloth), 1), parse)
     return output, warped_cloth, parse
+
+
+class _GraphRunner:
+    """One captured CUDA graph per (input shapes, storage precision) over static copies of the inputs.  Before every replay the
+    state key of the modules (ops.STORAGE and spade._param_key of each: ops.PARAM_GEN and (data_ptr, _version) of every parameter
+    and buffer, the key of the derived-weight caches) is compared with the one the graph was captured under; a graph captured
+    before a load_state_dict, an optimiser step, a parameter or running-statistics edit or a set_precision is released and
+    captured again.  Subclasses define _body(static) -> outputs."""
+
+    def __init__(self, modules):
+        self._modules = modules
+        self._graphs = {}  # (shapes, storage) -> _Entry
+
+    class _Entry:
+        def __init__(self, static, state):
+            self.static, self.state = static, state
+            self.captured = None
+            self.keep = []
+
+    def _state_key(self):
+        return (ops.STORAGE[0],) + tuple(_param_key(m) for m in self._modules)
+
+    def _check_ready(self, inputs, channels):
+        if ops.PROFILE is not None:
+            raise RuntimeError("%s: ops.PROFILE is on — profiling records CUDA events around every call, which cannot run inside a "
+                               "CUDA-graph capture; set ops.PROFILE = None" % type(self).__name__)
+        for m in self._modules:
+            if any(s.training for s in m.modules()):
+                raise RuntimeError("%s: %s is in train mode; the captured forward is the eval-mode one: call .eval()"
+                                   % (type(self).__name__, type(m).__name__))
+        for name, c in channels.items():
+            t = inputs[name]
+            if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.float32 and t.dim() == 4 and t.shape[1] == c):
+                raise ValueError("%s: input %r must be a CUDA float32 (N,%d,H,W) tensor, got %s" % (
+                    type(self).__name__, name, c, "%s %s %s" % (t.device, t.dtype, tuple(t.shape)) if torch.is_tensor(t) else type(t)))
+
+    def _run(self, inputs):
+        key = tuple(tuple(t.shape) for t in inputs.values()) + (ops.STORAGE[0],)
+        state = self._state_key()
+        e = self._graphs.get(key)
+        if e is not None and e.state != state:
+            self._graphs.pop(key).captured.release()
+            e = None
+        if e is None:
+            e = self._Entry({k: v.detach().clone() for k, v in inputs.items()}, state)
+            e.captured = CapturedCall(lambda: self._body(e.static), warm=1, keep_rng=True)
+            # the graph reads the packed weights / folded BatchNorm tables of the modules' caches: keeping them alive means an
+            # eager call that rebuilds a cache never frees memory a captured graph still reads
+            e.keep = [getattr(s, a) for m in self._modules for s in m.modules() for a in ("_cache", "_pyr") if getattr(s, a, None) is not None]
+            self._graphs[key] = e
+        else:
+            for k, v in inputs.items():
+                e.static[k].copy_(v)
+        return e.captured.replay()
+
+    def release(self):
+        """Destroy every captured graph (and the outputs they returned)."""
+        for e in self._graphs.values():
+            e.captured.release()
+        self._graphs.clear()
+
+
+class TryOnGraph(_GraphRunner):
+    """tryon_forward(tocg, generator, inputs, occlusion=..., clothmask_composition=...) replayed from a CUDA graph: no Python-driven
+    launches, C-ABI calls, TMA descriptor encodes or cache-key checks per network on the critical path — what matters when requests
+    arrive one or a few images at a time.
+
+    runner(inputs) takes the dict tryon_forward takes (cloth / cloth_mask as tensors or {setting: tensor} dicts, picked by
+    `datasetting`); every input is a CUDA float32 NCHW tensor at the fine resolution.  The first call with a new (batch, H, W,
+    storage precision) captures that shape (one eager warm-up call on a side stream, then the capture); every call copies the
+    inputs into the graph's static buffers and replays.  Returns (output, warped_cloth, parse), equal to what tryon_forward
+    returns for the same inputs, weights and noise.  The returned tensors belong to the runner: they stay valid until its next
+    call, which overwrites them — clone() what must outlive it.
+
+    Both modules must be in eval mode.  SPADE noise is drawn inside the graph from torch's CUDA generator (graph-safe Philox): every
+    replay draws fresh noise and advances the generator exactly as one eager call does.  A generator's noise_source is called during
+    the capture and what it returns there is what every replay reads; it must produce device tensors without host synchronisation."""
+
+    def __init__(self, tocg, generator, occlusion=True, clothmask_composition="warp_grad"):
+        super().__init__([tocg, generator])
+        self.tocg, self.generator = tocg, generator
+        self.occlusion, self.clothmask_composition = occlusion, clothmask_composition
+        self._channels = {"cloth": 3, "cloth_mask": 1, "agnostic": 3, "densepose": 3, "parse_agnostic": tocg.io[1] - 3}
+
+    def _body(self, static):
+        return tryon_forward(self.tocg, self.generator, static, occlusion=self.occlusion, clothmask_composition=self.clothmask_composition)
+
+    def __call__(self, inputs, datasetting="paired"):
+        pick = lambda v: v[datasetting] if isinstance(v, dict) else v
+        inputs = {k: pick(inputs[k]) for k in self._channels}
+        self._check_ready(inputs, self._channels)
+        if len({(t.shape[0],) + tuple(t.shape[2:]) for t in inputs.values()}) != 1:
+            raise ValueError("TryOnGraph: every input must have the same batch, height and width; got %s"
+                             % {k: tuple(t.shape) for k, t in inputs.items()})
+        return self._run(inputs)
+
+
+class GeneratorGraph(_GraphRunner):
+    """generator(x, seg) under torch.no_grad() replayed from a CUDA graph, with the contract of TryOnGraph: one graph per (x shape,
+    seg shape, storage precision), eval mode, CUDA float32 inputs, recapture when the weights or the precision changed, fresh SPADE
+    noise per replay from torch's CUDA generator.  Returns the (N,3,H,W) image, owned by the runner and valid until its next call."""
+
+    def __init__(self, generator):
+        super().__init__([generator])
+        self.generator = generator
+        self._channels = {"x": generator.conv_0.in_channels, "seg": generator.head_0.norm_0.conv_shared[0].in_channels}
+
+    def _body(self, static):
+        with torch.no_grad():
+            return self.generator(static["x"], static["seg"])
+
+    def __call__(self, x, seg):
+        inputs = {"x": x, "seg": seg}
+        self._check_ready(inputs, self._channels)
+        if x.shape[0] != seg.shape[0]:
+            raise ValueError("GeneratorGraph: x and seg must have the same batch size; got %d and %d" % (x.shape[0], seg.shape[0]))
+        return self._run(inputs)
 
 
 def psnr(a, b, peak=2.0):

@@ -156,23 +156,17 @@ class _GraphMixin:
     """Capture one whole step (all optimiser updates) into a CUDA graph over static copies of the batch: removes the thousands of
     Python-driven launches per step from the critical path.  capture(batch, *step_args) once, then replay(new_batch)."""
 
+    _captured = None
+
     def capture(self, batch, *step_args, warm=2):
+        from .graphs import CapturedCall
         self._static = {k: v.clone() for k, v in batch.items()}
-        cur = torch.cuda.current_stream()
-        side = torch.cuda.Stream()
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):
-            for _ in range(warm):
-                self.step(self._static, *step_args)
-        cur.wait_stream(side)
-        torch.cuda.synchronize()
-        self._graph = torch.cuda.CUDAGraph()
         import torch.distributed as dist
         multi = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
         # with NCCL inside the graph the process group's watchdog thread keeps polling CUDA events: thread-local capture mode keeps
         # those calls from invalidating the capture
-        with torch.cuda.graph(self._graph, capture_error_mode="thread_local" if multi else "global"):
-            self._graph_out = self.step(self._static, *step_args)
+        self._captured = CapturedCall(lambda: self.step(self._static, *step_args), warm=warm,
+                                      capture_error_mode="thread_local" if multi else "global")
         return self
 
     def replay(self, batch=None, feeder=None):
@@ -181,20 +175,15 @@ class _GraphMixin:
         elif batch is not None:
             for k, v in batch.items():
                 self._static[k].copy_(v, non_blocking=True)
-        self._graph.replay()
-        from . import ops
+        out = self._captured.replay()
         ops.PARAM_GEN[0] += 1  # the replayed optimiser step changed parameters without touching tensor._version: derived caches are stale
-        return self._graph_out
+        return out
 
     def release_graph(self):
-        """Destroy the captured graph (its nodes hold references on the NCCL communicator: ncclCommDestroy at process-group
-        tear-down waits for them — the round-2 two-GPU runs printed their result and then hung in destroy_process_group)."""
-        torch.cuda.synchronize()
-        self._graph = None
-        self._graph_out = None
-        import gc
-        gc.collect()
-        torch.cuda.synchronize()
+        """Destroy the captured graph (graphs.CapturedCall.release)."""
+        if self._captured is not None:
+            self._captured.release()
+            self._captured = None
 
 
 class _LossScaling:
