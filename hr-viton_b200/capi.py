@@ -18,7 +18,7 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_instnorm_stats_workspace_bytes", "hrv_instnorm_stats2_workspace_bytes", "hrv_norm_bwd_reduce_workspace_bytes",
            "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
-           "hrv_grad_unscale_check", "hrv_syncbn_combine", "hrv_syncbn_fwd_finalize", "hrv_syncbn_bwd_finalize", "hrv_last_error",
+           "hrv_grad_unscale_check", "hrv_syncbn_combine", "hrv_syncbn_fwd_finalize", "hrv_syncbn_bwd_finalize", "hrv_seg_softmax_cat", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 
 
@@ -82,6 +82,7 @@ def lib(dtype=None):
     L.hrv_conv2d_wgrad_workspace_bytes.argtypes = [TP, TP, i32, i32]
     L.hrv_nchw_to_nhwc.argtypes = [vp, i32, i32, i32, TP, vp]
     L.hrv_nhwc_to_nchw.argtypes = [TP, vp, vp]
+    L.hrv_seg_softmax_cat.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, TP, vp, vp]
     L.hrv_space_to_depth.argtypes = [TP, TP, vp]
     L.hrv_avgpool3s2.argtypes = [TP, TP, vp]
     L.hrv_bilinear_up2_add.argtypes = [TP, TP, TP, vp]

@@ -329,6 +329,63 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, int C, int SH
   st8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + g * 8, f);
 }
 
+// The condition discriminator's input [input1 | input2 | third] built in one pass from three fp32 NCHW tensors (test_condition.py:
+// 106-120, get_norm_const.py:99-115).  thread = one pixel: it needs all K scores of the pixel for the soft-max, reads every plane
+// coalesced, and writes the pixel's G 8-channel groups.  `third` is seg with channel cm_channel multiplied by cm (mode 1) or by
+// (cm > 0.5) (mode 2), then its channel soft-max (softmax = 1: maximum subtracted, expf, true division) or itself (softmax = 0).
+// The scores are re-read from L1 for the maximum, the sum and the write rather than held in K registers.
+struct SegCatSrc {
+  const float* in1;
+  const float* in2;
+  const float* seg;
+  const float* cm;
+  int c1, c2, K, cm_channel, mode, softmax;
+};
+__device__ __forceinline__ float seg_cat_score(const SegCatSrc& S, const float* seg_px, long long hw, int k, float m) {
+  const float s = __ldg(seg_px + (long long)k * hw);
+  return k == S.cm_channel ? __fmul_rn(s, m) : s;
+}
+template <typename T>
+__global__ void seg_softmax_cat_kernel(SegCatSrc S, View dst, float* __restrict__ seg_out, int G, long long npix) {
+  const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= npix) return;
+  const long long hw = (long long)dst.h * dst.w;
+  const long long n = pix / hw, rem = pix - n * hw;
+  const float* seg_px = S.seg + n * S.K * hw + rem;
+  float m = 1.f;
+  if (S.mode != 0) {
+    m = __ldg(S.cm + pix);
+    if (S.mode == 2) m = m > 0.5f ? 1.f : 0.f;
+  }
+  float mx = -INFINITY, sum = 0.f;
+  if (S.softmax) {
+    for (int k = 0; k < S.K; ++k) mx = fmaxf(mx, seg_cat_score(S, seg_px, hw, k, m));
+    for (int k = 0; k < S.K; ++k) sum += expf(seg_cat_score(S, seg_px, hw, k, m) - mx);
+  }
+  if (seg_out)
+    for (int k = 0; k < S.K; ++k) seg_out[n * S.K * hw + (long long)k * hw + rem] = seg_cat_score(S, seg_px, hw, k, m);
+  const int c12 = S.c1 + S.c2;
+  T* out = reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch;
+  for (int g = 0; g < G; ++g) {
+    float f[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const int c = g * 8 + i;
+      if (c < S.c1) {
+        f[i] = __ldg(S.in1 + (n * S.c1 + c) * hw + rem);
+      } else if (c < c12) {
+        f[i] = __ldg(S.in2 + (n * S.c2 + (c - S.c1)) * hw + rem);
+      } else if (c < c12 + S.K) {
+        const float s = seg_cat_score(S, seg_px, hw, c - c12, m);
+        f[i] = S.softmax ? __fdiv_rn(expf(s - mx), sum) : s;
+      } else {
+        f[i] = 0.f;
+      }
+    }
+    st8(out + g * 8, f);
+  }
+}
+
 // thread = (pixel); loops channels; writes are coalesced per plane.
 __global__ void nhwc_to_nchw_kernel(View src, float* __restrict__ dst, long long npix) {
   const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -730,6 +787,25 @@ extern "C" int hrv_nchw_to_nhwc(const float* src, int32_t c, int32_t src_h, int3
   const long long total = (long long)dst->n * dst->h * dst->w * G;
   HRV_LAUNCH_STORAGE(dt, nchw_to_nhwc_kernel, blocks_for(total, 256), 256, 0, (cudaStream_t)stream, src, c, src_h, src_w, mk(dst), G, total);
   return launch_ok("nchw_to_nhwc");
+}
+
+extern "C" int hrv_seg_softmax_cat(const float* input1, int32_t c1, const float* input2, int32_t c2, const float* seg, int32_t k,
+                                   const float* cm, int32_t cm_channel, int32_t mode, int32_t softmax, const hrv_tensor* dst,
+                                   float* seg_out, hrv_stream stream) {
+  const int dt = storage_of(dst);
+  int rc = check_vec(dst, "seg_softmax_cat dst", dt);
+  if (rc) return rc;
+  if (!input1 || !input2 || !seg || c1 < 1 || c2 < 1 || k < 1) return set_error(HRV_EINVAL, "seg_softmax_cat: null input or empty operand");
+  if (dst->c != c1 + c2 + k) return set_error(HRV_EINVAL, "seg_softmax_cat: dst has %d channels, the operands %d + %d + %d", dst->c, c1, c2, k);
+  if (mode < 0 || mode > 2) return set_error(HRV_EINVAL, "seg_softmax_cat: mode must be 0 (none), 1 (multiply by cm) or 2 (by cm > 0.5)");
+  if (mode != 0 && (!cm || cm_channel < 0 || cm_channel >= k))
+    return set_error(HRV_EINVAL, "seg_softmax_cat: mode %d needs cm and 0 <= cm_channel < %d", mode, k);
+  const int G = (dst->c + 7) / 8;
+  if (G * 8 > dst->pitch) return set_error(HRV_EINVAL, "seg_softmax_cat: dst pitch too small for padded channels");
+  SegCatSrc S{input1, input2, seg, cm, c1, c2, k, mode != 0 ? cm_channel : -1, mode, softmax ? 1 : 0};
+  const long long npix = (long long)dst->n * dst->h * dst->w;
+  HRV_LAUNCH_STORAGE(dt, seg_softmax_cat_kernel, blocks_for(npix, 128), 128, 0, (cudaStream_t)stream, S, mk(dst), seg_out, G, npix);
+  return launch_ok("seg_softmax_cat");
 }
 
 extern "C" int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream) {

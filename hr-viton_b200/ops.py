@@ -144,6 +144,39 @@ def from_nchw(x, c_pad=None, size=None, out=None):
     return out
 
 
+SEG_CAT_MODES = {"no_composition": 0, "warp_grad": 1, "detach": 2}
+
+
+def seg_softmax_cat(input1, input2, seg, cm=None, cm_channel=3, composition="warp_grad", softmax=True, want_seg=False, out=None):
+    """The condition discriminator's input [input1 | input2 | third] as one NHWC Act in the storage type (hrv_seg_softmax_cat):
+    third = seg with channel `cm_channel` multiplied by cm ('warp_grad') or by (cm > 0.5) ('detach'), then its channel soft-max
+    (softmax=True) or itself.  All inputs fp32 NCHW (cuda) at one (N,H,W); cm (N,1,H,W), None = no composition.
+    want_seg=True also returns the composed seg as fp32 NCHW; out: the destination Act (c1+c2+K channels), as for from_nchw."""
+    if composition not in SEG_CAT_MODES:
+        raise ValueError("composition must be one of %s, got %r" % ("/".join(SEG_CAT_MODES), composition))
+    mode = 0 if cm is None else SEG_CAT_MODES[composition]
+    ts = [input1, input2, seg] + ([cm] if mode else [])
+    for t in ts:
+        if not t.is_cuda:
+            raise RuntimeError("seg_softmax_cat runs on the GPU only (no CPU fallback): got a %s tensor" % t.device)
+        if t.dtype != torch.float32 or t.dim() != 4 or (t.shape[0],) + tuple(t.shape[2:]) != (seg.shape[0],) + tuple(seg.shape[2:]):
+            raise ValueError("seg_softmax_cat: every input must be float32 (N,C,H,W) at one (N,H,W); got %s" % [tuple(t.shape) for t in ts])
+    if mode and cm.shape[1] != 1:
+        raise ValueError("seg_softmax_cat: cm must be (N,1,H,W), got %s" % (tuple(cm.shape),))
+    input1, input2, seg = input1.contiguous(), input2.contiguous(), seg.contiguous()
+    cm = cm.contiguous() if mode else None
+    n, k, h, w = seg.shape
+    if out is None:
+        out = Act.empty(n, h, w, input1.shape[1] + input2.shape[1] + k)
+    seg_out = torch.empty_like(seg) if want_seg else None
+    t = out.ct()
+    with _Timed("glue", 0.0, label="seg_softmax_cat"):
+        capi.check(_L(out).hrv_seg_softmax_cat(input1.data_ptr(), input1.shape[1], input2.data_ptr(), input2.shape[1], seg.data_ptr(), k,
+                                               _p(cm), cm_channel, mode, int(bool(softmax)), ctypes.byref(t), _p(seg_out), _stream()),
+                   "seg_softmax_cat")
+    return (out, seg_out) if want_seg else out
+
+
 # ----------------------------------------------------------------------------------------------- weights
 
 def pick_bk(cin):

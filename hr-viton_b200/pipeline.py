@@ -15,9 +15,89 @@ from .spade import _param_key
 from .train_step import GROUP_OF_13, OCCLUSION_CLASSES
 
 
-def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_composition="warp_grad", datasetting="paired"):
+def d_logit(preds):
+    """The reference's D_logit (get_norm_const.py:60-64) on a MultiscaleDiscriminator result: the sum over scales of the last
+    output's mean over (1,2,3), each divided by 2.  The 2 is hard-coded there: the result is the mean over scales only for
+    num_D=2 (the reference's configuration); the reference's arithmetic is kept for every num_D.  (N,) fp32, no synchronisation."""
+    score = 0
+    for p in preds:
+        score = score + p[-1].mean((1, 2, 3)) / 2
+    return score
+
+
+def _check_norm_const(norm_const):
+    if norm_const is None or not norm_const > 0:
+        raise ValueError("norm_const must be the positive normalising constant M of discriminator rejection "
+                         "(pipeline.norm_constant / the reference's get_norm_const.py), got %r" % (norm_const,))
+
+
+def condition_logit(D, input1, input2, third, cm=None, composition="warp_grad", softmax=True, return_maps=False):
+    """l = d_logit(D([input1 | input2 | third'])) for a try-on condition, (N,) fp32 on the device (get_norm_const.py:99-120).
+    third' is `third` with its cloth channel (3) multiplied by cm (composition 'warp_grad') or by (cm > 0.5) ('detach'), then
+    soft-maxed over channels (softmax=True: the generated segmentation scores) or taken as is (softmax=False: the one-hot `parse`
+    label of the real branch).  One kernel builds the discriminator's NHWC input; D runs its eval forward on it.
+    return_maps=True also returns the per-scale logit maps the means are taken of."""
+    for t in (input1, input2, third) + (() if cm is None else (cm,)):
+        if not t.is_cuda:
+            raise RuntimeError("condition_logit: hrviton_b200 runs on sm_90a only — got a CPU tensor (there is no CPU fallback)")
+    with torch.no_grad():
+        a = ops.seg_softmax_cat(input1.float(), input2.float(), third.float(), cm=None if cm is None else cm.float(),
+                                composition=composition, softmax=softmax)
+        preds = D.forward_act(a)
+        l = d_logit(preds)
+    return (l, [p[-1] for p in preds]) if return_maps else l
+
+
+def _condition(tocg, inputs, opt, datasetting):
+    """input1, input2 and the tocg outputs for a cp_dataset batch at the tocg resolution (test_condition.py:81-103)."""
+    pick = lambda v: v[datasetting] if isinstance(v, dict) else v
+    cm = (pick(inputs["cloth_mask"]) > 0.5).float()                                            # test_condition.py:84 (numpy round trip there)
+    input1 = torch.cat([pick(inputs["cloth"]), cm], 1)
+    input2 = torch.cat([inputs["parse_agnostic"], inputs["densepose"]], 1)
+    return input1, input2, (tocg(input1, input2) if opt is None else tocg(opt, input1, input2))
+
+
+def rejection_scores(tocg, D, inputs, norm_const, opt=None, clothmask_composition="warp_grad", datasetting="paired"):
+    """Discriminator rejection (test_condition.py:99-127): inputs is the cp_dataset batch dict at the tocg resolution (cloth /
+    cloth_mask as tensors or {setting: tensor} dicts, parse_agnostic, densepose; CUDA fp32 NCHW).  Returns (score (N,), l (N,),
+    (flow_list, fake_segmap, warped_cloth, warped_clothmask)) with score = l / (1 - l) / norm_const, on the device."""
+    _check_norm_const(norm_const)
+    with torch.no_grad():
+        input1, input2, outs = _condition(tocg, inputs, opt, datasetting)
+        cm = None if clothmask_composition == "no_composition" else outs[3]
+        l = condition_logit(D, input1, input2, outs[1], cm=cm, composition=clothmask_composition)
+        score = l / (1 - l) / norm_const
+    return score, l, outs
+
+
+def norm_constant(tocg, D, batches, opt=None, clothmask_composition="warp_grad", datasetting="paired"):
+    """The normalising constant M of discriminator rejection (get_norm_const.get_const, :65-132): the maximum of l / (1 - l) over
+    the real (third = batch["parse"], the one-hot label, no soft-max) and the generated condition of every sample of `batches`
+    (an iterable of cp_dataset batch dicts with "parse").  The maximum is kept on the device; the one synchronisation is the
+    read of the result."""
+    m = None
+    with torch.no_grad():
+        for inputs in batches:
+            input1, input2, outs = _condition(tocg, inputs, opt, datasetting)
+            cm = None if clothmask_composition == "no_composition" else outs[3]
+            l = torch.cat([condition_logit(D, input1, input2, inputs["parse"], softmax=False),
+                           condition_logit(D, input1, input2, outs[1], cm=cm, composition=clothmask_composition)])
+            v = (l / (1 - l)).max()
+            m = v if m is None else torch.maximum(m, v)
+    if m is None:
+        raise ValueError("norm_constant: no batches")
+    return float(m)
+
+
+def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_composition="warp_grad", datasetting="paired",
+                  discriminator=None, norm_const=None):
     """inputs: the dict a cp_dataset_test.CPDataLoader batch provides (cloth / cloth_mask may be {setting: tensor} dicts or tensors);
-    CUDA fp32 NCHW tensors at the fine resolution.  Returns (output image (N,3,H,W), warped_cloth, parse (N,7,H,W))."""
+    CUDA fp32 NCHW tensors at the fine resolution.  Returns (output image (N,3,H,W), warped_cloth, parse (N,7,H,W)).
+    With discriminator= (the stage-1 condition discriminator) and norm_const= the 256x192 condition is also scored as
+    rejection_scores does, and a fourth value, score (N,), is returned; the generator still runs for every sample — the caller
+    filters on score."""
+    if discriminator is not None:
+        _check_norm_const(norm_const)
     pick = lambda v: v[datasetting] if isinstance(v, dict) else v
     clothes, pre_cm = pick(inputs["cloth"]), pick(inputs["cloth_mask"])
     agnostic, densepose, parse_agnostic = inputs["agnostic"], inputs["densepose"], inputs["parse_agnostic"]
@@ -26,7 +106,16 @@ def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_c
         input1 = torch.cat([F.interpolate(clothes, size=(256, 192), mode="bilinear"), F.interpolate(pre_cm, size=(256, 192), mode="nearest")], 1)
         input2 = torch.cat([F.interpolate(parse_agnostic, size=(256, 192), mode="nearest"), F.interpolate(densepose, size=(256, 192), mode="bilinear")], 1)
         flow_list, fake_segmap, _, warped_cm = tocg(input1, input2) if opt is None else tocg(opt, input1, input2)
-        if clothmask_composition != "no_composition":
+        if discriminator is not None:
+            # the kernel that builds the discriminator's input also writes the composed scores the parse map is made of
+            composed = clothmask_composition != "no_composition"
+            a = ops.seg_softmax_cat(input1, input2, fake_segmap.float(), cm=warped_cm if composed else None,
+                                    composition=clothmask_composition, want_seg=composed)
+            if composed:
+                a, fake_segmap = a
+            l = d_logit(discriminator.forward_act(a))
+            score = l / (1 - l) / norm_const
+        elif clothmask_composition != "no_composition":
             cm = (warped_cm > 0.5).float() if clothmask_composition == "detach" else warped_cm   # test_generator.py:163-176
             fake_segmap = torch.cat([fake_segmap[:, :3], fake_segmap[:, 3:4] * cm, fake_segmap[:, 4:]], 1)
         n, _, ih, iw = clothes.shape
@@ -39,7 +128,7 @@ def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_c
             _, parse = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False)
             warped_cloth, _ = ops.flow_warp_nchw(flow_list[-1], clothes.float(), (ih, iw), div)
         output = generator(torch.cat((agnostic, densepose, warped_cloth), 1), parse)
-    return output, warped_cloth, parse
+    return (output, warped_cloth, parse) if discriminator is None else (output, warped_cloth, parse, score)
 
 
 class _GraphRunner:
@@ -95,6 +184,16 @@ class _GraphRunner:
                 e.static[k].copy_(v)
         return e.captured.replay()
 
+    def _run_batch(self, inputs, datasetting):
+        """_run on the self._channels entries of a cp_dataset batch dict ({setting: tensor} entries picked by `datasetting`)."""
+        pick = lambda v: v[datasetting] if isinstance(v, dict) else v
+        inputs = {k: pick(inputs[k]) for k in self._channels}
+        self._check_ready(inputs, self._channels)
+        if len({(t.shape[0],) + tuple(t.shape[2:]) for t in inputs.values()}) != 1:
+            raise ValueError("%s: every input must have the same batch, height and width; got %s"
+                             % (type(self).__name__, {k: tuple(t.shape) for k, t in inputs.items()}))
+        return self._run(inputs)
+
     def release(self):
         """Destroy every captured graph (and the outputs they returned)."""
         for e in self._graphs.values():
@@ -116,25 +215,46 @@ class TryOnGraph(_GraphRunner):
 
     Both modules must be in eval mode.  SPADE noise is drawn inside the graph from torch's CUDA generator (graph-safe Philox): every
     replay draws fresh noise and advances the generator exactly as one eager call does.  A generator's noise_source is called during
-    the capture and what it returns there is what every replay reads; it must produce device tensors without host synchronisation."""
+    the capture and what it returns there is what every replay reads; it must produce device tensors without host synchronisation.
 
-    def __init__(self, tocg, generator, occlusion=True, clothmask_composition="warp_grad"):
-        super().__init__([tocg, generator])
-        self.tocg, self.generator = tocg, generator
+    discriminator= (the stage-1 condition discriminator, eval mode) with norm_const= scores the 256x192 condition inside the same
+    graph and returns (output, warped_cloth, parse, score), score as ConditionGraph's.  A graph cannot skip the generator for a
+    rejected sample: every sample is generated and the caller filters on score."""
+
+    def __init__(self, tocg, generator, occlusion=True, clothmask_composition="warp_grad", discriminator=None, norm_const=None):
+        super().__init__([tocg, generator] + ([] if discriminator is None else [discriminator]))
+        if discriminator is not None:
+            _check_norm_const(norm_const)
+        self.tocg, self.generator, self.discriminator, self.norm_const = tocg, generator, discriminator, norm_const
         self.occlusion, self.clothmask_composition = occlusion, clothmask_composition
         self._channels = {"cloth": 3, "cloth_mask": 1, "agnostic": 3, "densepose": 3, "parse_agnostic": tocg.io[1] - 3}
 
     def _body(self, static):
-        return tryon_forward(self.tocg, self.generator, static, occlusion=self.occlusion, clothmask_composition=self.clothmask_composition)
+        return tryon_forward(self.tocg, self.generator, static, occlusion=self.occlusion, clothmask_composition=self.clothmask_composition,
+                             discriminator=self.discriminator, norm_const=self.norm_const)
 
     def __call__(self, inputs, datasetting="paired"):
-        pick = lambda v: v[datasetting] if isinstance(v, dict) else v
-        inputs = {k: pick(inputs[k]) for k in self._channels}
-        self._check_ready(inputs, self._channels)
-        if len({(t.shape[0],) + tuple(t.shape[2:]) for t in inputs.values()}) != 1:
-            raise ValueError("TryOnGraph: every input must have the same batch, height and width; got %s"
-                             % {k: tuple(t.shape) for k, t in inputs.items()})
-        return self._run(inputs)
+        return self._run_batch(inputs, datasetting)
+
+
+class ConditionGraph(_GraphRunner):
+    """rejection_scores(tocg, D, inputs, norm_const, clothmask_composition=...) replayed from a CUDA graph, with the contract of
+    TryOnGraph: one graph per (input shapes, storage precision), both modules in eval mode, CUDA float32 inputs at the tocg
+    resolution (cloth, cloth_mask, parse_agnostic, densepose; cloth / cloth_mask as tensors or {setting: tensor} dicts), recapture
+    when the weights of either module or the precision changed.  Returns (score, l, (flow_list, fake_segmap, warped_cloth,
+    warped_clothmask)), bit-identical to the eager call and owned by the runner until its next call."""
+
+    def __init__(self, tocg, D, norm_const, clothmask_composition="warp_grad"):
+        super().__init__([tocg, D])
+        _check_norm_const(norm_const)
+        self.tocg, self.D, self.norm_const, self.clothmask_composition = tocg, D, norm_const, clothmask_composition
+        self._channels = {"cloth": 3, "cloth_mask": 1, "parse_agnostic": tocg.io[1] - 3, "densepose": 3}
+
+    def _body(self, static):
+        return rejection_scores(self.tocg, self.D, static, self.norm_const, clothmask_composition=self.clothmask_composition)
+
+    def __call__(self, inputs, datasetting="paired"):
+        return self._run_batch(inputs, datasetting)
 
 
 class GeneratorGraph(_GraphRunner):

@@ -378,7 +378,12 @@ class MultiscaleDiscriminator(nn.Module):
             from . import autograd_tocg
             return autograd_tocg.tocg_discriminator_forward_train(self, input)
         with torch.no_grad():
-            a = ops.from_nchw(input.float())
+            return self.forward_act(ops.from_nchw(input.float()))
+
+    def forward_act(self, a):
+        """The no-grad forward on an NHWC Act that already holds the input channels (ops.from_nchw, ops.seg_softmax_cat): same
+        result as forward(nchw), list[num_D] of lists of fp32 NCHW tensors."""
+        with torch.no_grad():
             if self.Ddownx2:
                 a = ops.avgpool3s2(a)
             result = []

@@ -193,6 +193,18 @@ int hrv_act_bwd_bias(const hrv_tensor* dy, const hrv_tensor* y, int32_t act, con
  * src: [n][c][src_h][src_w] fp32 contiguous.  fp32 storage: dst may be fp32 NHWC. */
 int hrv_nchw_to_nhwc(const float* src, int32_t c, int32_t src_h, int32_t src_w, const hrv_tensor* dst, hrv_stream stream);
 
+/* The condition discriminator's input for discriminator rejection (test_condition.py:106-120, get_norm_const.py:99-115) in one pass:
+ *   dst[n,y,x,:] = [ input1 (c1) | input2 (c2) | third (k) ], zero fill of the pad channels of the last 8-channel group,
+ *   third = softmax ? softmax_over_channels(composed) : composed,
+ *   composed = seg with channel cm_channel multiplied by cm (mode 1, 'warp_grad') or by (cm > 0.5) (mode 2, 'detach'); mode 0: seg.
+ * input1, input2, seg: fp32 [n][c][h][w] contiguous at dst's (n,h,w); cm: fp32 [n][1][h][w] (NULL with mode 0).  softmax = 0 copies
+ * the third operand (the one-hot label of the real branch, get_norm_const.py:114).  The soft-max is fp32 with the maximum
+ * subtracted, expf and a correctly rounded division; every output is rounded once to dst's type.  dst: bf16 NHWC view with
+ * c = c1+c2+k, pitch % 8 == 0; fp32 storage: dst may be fp32 NHWC.  seg_out (optional): `composed` as fp32 [n][k][h][w]. */
+int hrv_seg_softmax_cat(const float* input1, int32_t c1, const float* input2, int32_t c2, const float* seg, int32_t k,
+                        const float* cm, int32_t cm_channel, int32_t mode, int32_t softmax, const hrv_tensor* dst,
+                        float* seg_out, hrv_stream stream);
+
 /* bf16|f32 NHWC view -> fp32 NCHW contiguous [n][c][h][w]. */
 int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream);
 
