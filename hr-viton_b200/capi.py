@@ -20,6 +20,9 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
            "hrv_grad_unscale_check", "hrv_syncbn_combine", "hrv_syncbn_fwd_finalize", "hrv_syncbn_bwd_finalize", "hrv_seg_softmax_cat", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
+# include/hrviton_sm100_metrics.h: fp32 / fp64 only, one flavour (no _f16 twin)
+METRICS_EXPORTS = ["hrv_lpips_input", "hrv_maxpool3s2", "hrv_lpips_dist", "hrv_ssim", "hrv_ssim_workspace_bytes"]
+SSIM_U8, SSIM_F32 = 0, 1
 
 
 class Tensor(ctypes.Structure):
@@ -121,7 +124,12 @@ def lib(dtype=None):
     for name in FLAVOURED:
         twin = getattr(L, name + "_f16")
         twin.argtypes = getattr(L, name).argtypes
-    for name in EXPORTS + EXPORTS_F16:
+    L.hrv_lpips_input.argtypes = [vp, i32, i32, i32, vp, vp, TP, vp]
+    L.hrv_maxpool3s2.argtypes = [TP, TP, vp]
+    L.hrv_lpips_dist.argtypes = [TP, vp, vp, vp]
+    L.hrv_ssim_workspace_bytes.argtypes = [i32, i32, i32]
+    L.hrv_ssim.argtypes = [vp, vp, i32, i32, i32, i32, f64, vp, vp, sz, vp]
+    for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS:
         fn = getattr(L, name)
         if "_workspace_bytes" in name:
             fn.restype = ctypes.c_size_t

@@ -231,10 +231,11 @@ class PackedConv:
     flops_per_pixel: float = 0.0  # algorithmic 2*Cin*Cout*kh*kw of the ORIGINAL convolution (unpadded, pre-s2d)
 
 
-def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixel=None, dgrad=False):
+def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixel=None, dgrad=False, storage=None):
     """w: (Cout,Cin,kh,kw) fp32 cuda (already divided by sigma / transformed). Returns PackedConv (one kernel: hrv_pack_conv_weight).
     interleave: a second weight of identical shape whose rows are interleaved (gamma_c, beta_c pairs).
-    dgrad=True packs the operand of the data-gradient convolution (flip + transpose) without materialising it."""
+    dgrad=True packs the operand of the data-gradient convolution (flip + transpose) without materialising it.
+    storage: the activation storage the convolution will run on (default: the current one, set_precision)."""
     w = w.detach()
     if w.dtype != torch.float32 or not w.is_contiguous():
         w = w.float().contiguous()
@@ -247,7 +248,8 @@ def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixe
     inter = 2 if interleave is not None else 1
     rows, cols = (cin, cout * inter) if dgrad else (cout * inter, cin)  # GEMM N rows, K columns
     k_eff = cols if cin_total is None else cin_total
-    f32 = STORAGE[0] == torch.float32
+    st = STORAGE[0] if storage is None else storage
+    f32 = st == torch.float32
     if f32:
         bk = 32  # the 3xTF32 kernel's K block: 32 fp32 channels = one 128-byte swizzle row
     else:
@@ -263,7 +265,7 @@ def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixe
             capi.check(capi.lib().hrv_pack_conv_weight_tf32x2(w.data_ptr(), _p(interleave), cout, cin, kh, kw, 1 if dgrad else 0, None,
                                                               wp.data_ptr(), n_pad, cin_k, _stream()), "pack_conv_weight_tf32x2")
     else:
-        wp = torch.empty((kh * kw, n_pad, cin_k), dtype=STORAGE[0], device=w.device)
+        wp = torch.empty((kh * kw, n_pad, cin_k), dtype=st, device=w.device)
         with _Timed("glue", 0.0, label="pack_conv_weight"):
             capi.check(_L(wp).hrv_pack_conv_weight(w.data_ptr(), _p(interleave), cout, cin, kh, kw, 1 if dgrad else 0, None, wp.data_ptr(),
                                                        n_pad, cin_k, _stream()), "pack_conv_weight")
@@ -830,3 +832,62 @@ def flow_warp_bwd(flow_lo, src, ddst, dflow_up_in, want_dsrc=True):
                                                _stream()), "flow_warp_bwd_ordered")
     dsrc = Act(dsrc32.to(src.buf.dtype)) if want_dsrc else None
     return dsrc, dflo
+
+
+# ----------------------------------------------------------------------------------------------- evaluation metrics (fp32 / fp64)
+
+LPIPS_K = 363  # conv1's im2col depth (11*11 taps x 3 channels)
+
+
+def lpips_input(x, shift, scale):
+    """LPIPS ScalingLayer + the operand of AlexNet's conv1 (11x11, stride 4, pad 2) as a 1x1 GEMM: x fp32 NCHW (n,3,h,w) cuda ->
+    fp32 NHWC Act (n, (h-7)//4+1, (w-7)//4+1, 363) (hrv_lpips_input).  shift, scale: fp32 [3] cuda."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and x.shape[1] == 3
+    x = x.contiguous()
+    n, _, h, w = x.shape
+    out = Act.empty(n, (h - 7) // 4 + 1, (w - 7) // 4 + 1, LPIPS_K, dtype=torch.float32)
+    t = out.ct()
+    with _Timed("glue", 0.0, label="lpips_input"):
+        capi.check(capi.lib().hrv_lpips_input(x.data_ptr(), n, h, w, shift.data_ptr(), scale.data_ptr(), ctypes.byref(t), _stream()), "lpips_input")
+    return out
+
+
+def maxpool3s2(x):
+    """nn.MaxPool2d(3, 2) on an fp32 NHWC Act (hrv_maxpool3s2): bit-exact."""
+    y = Act.empty(x.n, (x.h - 3) // 2 + 1, (x.w - 3) // 2 + 1, x.c, dtype=torch.float32)
+    tx, ty = x.ct(), y.ct()
+    with _Timed("glue", 0.0, label="maxpool3s2"):
+        capi.check(capi.lib().hrv_maxpool3s2(ctypes.byref(tx), ctypes.byref(ty), _stream()), "maxpool3s2")
+    return y
+
+
+def lpips_dist(feat, lin_w):
+    """One LPIPS layer (hrv_lpips_dist): feat an fp32 Act of 2N images (image i against image i + N), lin_w fp32 [C] cuda.  Returns
+    the per-pair spatial mean of sum_c w_c (f0_c - f1_c)^2 over unit-normalised features, fp32 [N]."""
+    out = torch.empty(feat.n // 2, dtype=torch.float32, device=feat.buf.device)
+    t = feat.ct()
+    with _Timed("glue", 0.0, label="lpips_dist"):
+        capi.check(capi.lib().hrv_lpips_dist(ctypes.byref(t), lin_w.data_ptr(), out.data_ptr(), _stream()), "lpips_dist")
+    return out
+
+
+def ssim(im1, im2, data_range=255.0):
+    """Mean Gaussian SSIM per image (hrv_ssim; skimage's structural_similarity with gaussian_weights=True, use_sample_covariance=False)
+    of two (N,H,W) cuda tensors, uint8 or fp32.  Returns fp64 [N]."""
+    if im1.shape != im2.shape or im1.dtype != im2.dtype or im1.dim() != 3:
+        raise ValueError("ssim: im1 and im2 must be (N,H,W) of one shape and dtype; got %s %s and %s %s"
+                         % (tuple(im1.shape), im1.dtype, tuple(im2.shape), im2.dtype))
+    if im1.dtype not in (torch.uint8, torch.float32):
+        raise TypeError("ssim: images must be uint8 or float32, got %s" % im1.dtype)
+    n, h, w = im1.shape
+    if h < 11 or w < 11:
+        raise ValueError("win_size exceeds image extent: the 11x11 Gaussian window needs images of at least 11x11, got %dx%d" % (h, w))
+    im1, im2 = im1.contiguous(), im2.contiguous()
+    out = torch.empty(n, dtype=torch.float64, device=im1.device)
+    L = capi.lib()
+    nws = int(L.hrv_ssim_workspace_bytes(n, h, w))
+    ws = torch.empty(nws, dtype=torch.uint8, device=im1.device)
+    dt = capi.SSIM_U8 if im1.dtype == torch.uint8 else capi.SSIM_F32
+    with _Timed("glue", 0.0, launches=2, label="ssim"):
+        capi.check(L.hrv_ssim(im1.data_ptr(), im2.data_ptr(), dt, n, h, w, float(data_range), out.data_ptr(), ws.data_ptr(), nws, _stream()), "ssim")
+    return out

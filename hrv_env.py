@@ -1,8 +1,8 @@
 """Environment for running the reference scripts unchanged against this repository's drop-in modules (see shims/README.md).
 
     import hrv_env; hrv_env.install()          # repo root first on sys.path, shims/ last, numpy aliases restored
-    hrv_env.load_reference_script("train_generator")   # imports oracle/_ref/train_generator.py with
-                                                        # `networks`, `network_generator`, `sync_batchnorm` bound to the drop-ins
+    hrv_env.load_reference_script("train_generator")   # imports oracle/_ref/train_generator.py with `networks`,
+                                                        # `network_generator`, `sync_batchnorm`, `eval_models` bound to the drop-ins
 """
 import importlib.util
 import os
@@ -34,6 +34,10 @@ def install():
     sys.path.insert(0, ROOT)
     if SHIMS not in sys.path:
         sys.path.append(SHIMS)  # last: a real torchgeometry / tensorboardX / apex wins
+    hub = os.path.expanduser("~/.cache/torch/hub/checkpoints")
+    # eval_models.PerceptualLoss's AlexNet backbone (tv.alexnet(pretrained=True) in the reference): random initialisation where no
+    # ImageNet file is cached, since offline machines cannot download it
+    os.environ.setdefault("HRV_ALEX_RANDOM_INIT", "1" if not os.path.exists(os.path.join(hub, "alexnet-owt-7be5be79.pth")) else "0")
     os.environ.setdefault("HRV_VGG_RANDOM_INIT", "1" if not os.path.exists(os.path.expanduser("~/.cache/torch/hub/checkpoints/vgg19-dcbb9e9d.pth")) else "0")
 
 
@@ -45,7 +49,7 @@ def reference_dir():
 
 def load_reference_script(name, alias=None):
     """Imports <reference>/<name>.py as a module.  Its own sibling imports that this repo replaces (networks, network_generator,
-    sync_batchnorm) resolve to the drop-ins at the repo root; the rest (utils, cp_dataset, eval_models) to the reference's files."""
+    sync_batchnorm, eval_models) resolve to the drop-ins at the repo root; the rest (utils, cp_dataset) to the reference's files."""
     install()
     d = reference_dir()
     if d is None:
@@ -53,6 +57,7 @@ def load_reference_script(name, alias=None):
     import network_generator  # noqa: F401  (bind the drop-ins before the reference directory becomes importable)
     import networks  # noqa: F401
     import sync_batchnorm  # noqa: F401
+    import eval_models  # noqa: F401
     if d not in sys.path:
         sys.path.insert(1, d)  # after the repo root
     spec = importlib.util.spec_from_file_location(alias or ("ref_" + name), os.path.join(d, name + ".py"))

@@ -382,4 +382,8 @@ int hrv_device_sm_count(void);
 #ifdef __cplusplus
 }
 #endif
+
+/* The evaluation metrics (LPIPS, SSIM): fp32 / fp64 only, one flavour, declared in their own header. */
+#include "hrviton_sm100_metrics.h"
+
 #endif /* HRVITON_SM100_H_ */
