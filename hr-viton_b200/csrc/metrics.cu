@@ -1,6 +1,7 @@
 // metrics.cu — the evaluation metrics of the reference's workflow (include/hrviton_sm100_metrics.h): the LPIPS AlexNet front end
-// and per-layer distance (eval_models/networks_basic.py, eval_models/__init__.py) and skimage's Gaussian SSIM as evaluate.py:67 calls
-// it.  fp32 and fp64 only, so this translation unit is compiled once (no 16-bit flavour).  No floating-point atomics: per-block
+// and per-layer distance (eval_models/networks_basic.py, eval_models/__init__.py), skimage's Gaussian SSIM as evaluate.py:67 calls
+// it, and the Inception-v3 pieces behind the Inception Score, FID and KID (input resize, global pool, fp64 Gram products, KID subset
+// sums).  fp32 and fp64 only, so this translation unit is compiled once (no 16-bit flavour).  No floating-point atomics: per-block
 // partials land in slabs that a second kernel adds in a fixed order.
 #include "hrv_host.h"
 
@@ -217,6 +218,186 @@ int ssim_tiles(int h, int w, int* tiles_x) {
   return tx * ty;
 }
 
+// ------------------------------------------------------------------------------------------------ Inception input resize
+// F.interpolate(x, (oh, ow), mode='bilinear', align_corners=False, antialias=False) on fp32 NCHW, written as fp32 NHWC.  The source
+// index, the weights and the blend are torch's own expressions in the same order (aten upsample_bilinear2d, accscalar_t = float), so
+// the result is bit-identical.  unit != 0 maps every source value v to 2v - 1 first (2v is exact: one rounding, as in torch).  One
+// thread per output element of the first 8-channel groups; channels [c, c8) are written as zeros.
+__device__ __forceinline__ float bilinear_src(float scale, int d) {
+  const float s = scale * (d + static_cast<float>(0.5)) - static_cast<float>(0.5);
+  return s < 0.f ? 0.f : s;
+}
+
+__global__ void resize_bilinear_kernel(const float* __restrict__ x, int c, int h, int w, float rh, float rw, int unit, float* __restrict__ dst,
+                                       int oh, int ow, int pitch, int c8, long long total) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int ch = (int)(idx % c8);
+  const long long pix = idx / c8;
+  float val = 0.f;
+  if (ch < c) {
+    const int ox = (int)(pix % ow), oy = (int)((pix / ow) % oh);
+    const long long img = pix / ((long long)ow * oh);
+    const float h1r = bilinear_src(rh, oy);
+    const int h1 = h1r;
+    const int h1p = (h1 < h - 1) ? 1 : 0;
+    const float h1lambda = h1r - h1;
+    const float h0lambda = static_cast<float>(1) - h1lambda;
+    const float w1r = bilinear_src(rw, ox);
+    const int w1 = w1r;
+    const int w1p = (w1 < w - 1) ? 1 : 0;
+    const float w1lambda = w1r - w1;
+    const float w0lambda = static_cast<float>(1) - w1lambda;
+    const float* p = x + (img * c + ch) * h * w;
+    float v00 = __ldg(p + (long long)h1 * w + w1), v01 = __ldg(p + (long long)h1 * w + w1 + w1p);
+    float v10 = __ldg(p + (long long)(h1 + h1p) * w + w1), v11 = __ldg(p + (long long)(h1 + h1p) * w + w1 + w1p);
+    if (unit) {
+      v00 = 2.f * v00 - 1.f; v01 = 2.f * v01 - 1.f; v10 = 2.f * v10 - 1.f; v11 = 2.f * v11 - 1.f;
+    }
+    val = h0lambda * (w0lambda * v00 + w1lambda * v01) + h1lambda * (w0lambda * v10 + w1lambda * v11);
+  }
+  dst[pix * pitch + ch] = val;
+}
+
+// ------------------------------------------------------------------------------------------------ global average pool
+// y[n, ch] = (sum over the h*w pixels in raster order, in fp64) / (h*w), rounded once to fp32.  One thread per (n, ch): a warp reads
+// 32 consecutive channels of one pixel.
+__global__ void global_avgpool_kernel(const float* __restrict__ x, int hw, int pitch, int c, float* __restrict__ y, int ypitch,
+                                      long long total) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int ch = (int)(idx % c);
+  const long long n = idx / c;
+  const float* p = x + n * hw * pitch + ch;
+  double s = 0.0;
+  for (int i = 0; i < hw; ++i) s += (double)__ldg(p + (long long)i * pitch);
+  y[n * ypitch + ch] = (float)(s / (double)hw);
+}
+
+// ------------------------------------------------------------------------------------------------ fp64 Gram product
+// C[i][j] (+)= sum_k A(i,k) * B(j,k) in fp64, A(i,k) = a[i*sam + k*sak], B(j,k) = b[j*sbn + k*sbk] (fp32 or fp64 elements).  A block
+// owns a 64x64 tile of C and one K range (split z of the grid); every thread owns a 4x4 sub-tile (rows ty + 16r, columns tx + 16q) and
+// adds its products in increasing k, one fma each (an fp32 x fp32 product is exact in fp64).  With one split the block writes C
+// (c + acc when accumulating); with several, split z writes slab z and gram_finish_kernel adds the slabs in split order.
+constexpr int kGramT = 64, kGramK = 16, kGramThreads = 256, kGramKPer = 512;
+
+template <typename T>
+__device__ __forceinline__ void gram_load(double (*s)[kGramT + 1], const T* __restrict__ g, long long si, long long sk, int i0, int ni, int k0,
+                                          int k1, bool kfast) {
+#pragma unroll
+  for (int r = 0; r < kGramT * kGramK / kGramThreads; ++r) {
+    const int e = threadIdx.x + r * kGramThreads;
+    const int ii = kfast ? e / kGramK : e % kGramT, kk = kfast ? e % kGramK : e / kGramT;  // consecutive threads: consecutive addresses
+    const int gi = i0 + ii, gk = k0 + kk;
+    s[kk][ii] = (gi < ni && gk < k1) ? (double)__ldg(g + gi * si + gk * sk) : 0.0;
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kGramThreads) gram_kernel(const T* __restrict__ a, long long sam, long long sak, const T* __restrict__ b,
+                                                            long long sbn, long long sbk, int m, int n, int k, int kper, double* __restrict__ c,
+                                                            long long ldc, int accumulate, double* __restrict__ slab) {
+  __shared__ double As[kGramK][kGramT + 1], Bs[kGramK][kGramT + 1];
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+  const int j0 = blockIdx.x * kGramT, i0 = blockIdx.y * kGramT;
+  const int kb = blockIdx.z * kper, ke = min(k, kb + kper);
+  const bool a_kfast = sak == 1 && sam != 1, b_kfast = sbk == 1 && sbn != 1;
+  double acc[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) acc[r][q] = 0.0;
+  for (int k0 = kb; k0 < ke; k0 += kGramK) {
+    gram_load(As, a, sam, sak, i0, m, k0, ke, a_kfast);
+    gram_load(Bs, b, sbn, sbk, j0, n, k0, ke, b_kfast);
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < kGramK; ++kk) {
+      double ar[4], br[4];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) ar[r] = As[kk][ty + 16 * r];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) br[q] = Bs[kk][tx + 16 * q];
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[r][q] = fma(ar[r], br[q], acc[r][q]);
+    }
+    __syncthreads();
+  }
+  double* s = slab ? slab + (long long)blockIdx.z * m * n : nullptr;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int i = i0 + ty + 16 * r, j = j0 + tx + 16 * q;
+      if (i >= m || j >= n) continue;
+      if (s) s[(long long)i * n + j] = acc[r][q];
+      else c[i * ldc + j] = accumulate ? c[i * ldc + j] + acc[r][q] : acc[r][q];
+    }
+}
+
+__global__ void gram_finish_kernel(const double* __restrict__ slab, int splits, int m, int n, double* __restrict__ c, long long ldc, int accumulate) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long mn = (long long)m * n;
+  if (idx >= mn) return;
+  double s = slab[idx];
+  for (int z = 1; z < splits; ++z) s += slab[z * mn + idx];
+  double* p = c + (idx / n) * ldc + idx % n;
+  *p = accumulate ? *p + s : s;
+}
+
+// Split-K only where the tiles alone leave most of the GPU idle and K is long; a function of the shape alone, so the summation order
+// (and the result) does not depend on the device.
+int gram_splits(int m, int n, int k, int* kper) {
+  const long long tiles = (long long)((m + kGramT - 1) / kGramT) * ((n + kGramT - 1) / kGramT);
+  int splits = 1;
+  if (tiles < 128 && k >= 2 * kGramKPer) {
+    splits = (int)((256 + tiles - 1) / tiles);
+    splits = min(splits, min(64, k / kGramKPer));
+  }
+  const int per = ((k + splits - 1) / splits + kGramK - 1) / kGramK * kGramK;
+  if (kper) *kper = per;
+  return (k + per - 1) / per;
+}
+
+// ------------------------------------------------------------------------------------------------ KID subset sums
+// Block (s, t) forms one sum of subset s over the cubic polynomial kernel k(g) = (g*gamma + 1)^3 of precomputed Gram entries:
+// t = 0: sum_{i != j} k(Gxx[ix_i][ix_j]),  t = 1: sum_{i != j} k(Gyy[iy_i][iy_j]),  t = 2: sum_{i, j} k(Gxy[ix_i][iy_j]).
+// Warp w walks the rows w, w + 16, ..., lanes the columns; fixed shuffle tree, then the warps in order.
+constexpr int kKidThreads = 512;
+__global__ void __launch_bounds__(kKidThreads) kid_sums_kernel(const double* __restrict__ gxx, const double* __restrict__ gyy,
+                                                               const double* __restrict__ gxy, int na, int nb, const int* __restrict__ ix,
+                                                               const int* __restrict__ iy, int m, double gamma, double* __restrict__ out) {
+  __shared__ double red[kKidThreads / 32];
+  const int s = blockIdx.x, t = blockIdx.y;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const double* g = t == 0 ? gxx : (t == 1 ? gyy : gxy);
+  const long long ld = t == 0 ? na : nb;
+  const int* ri = (t == 1 ? iy : ix) + (long long)s * m;
+  const int* ci = (t == 0 ? ix : iy) + (long long)s * m;
+  double acc = 0.0;
+  for (int i = warp; i < m; i += kKidThreads / 32) {
+    const double* row = g + (long long)__ldg(ri + i) * ld;
+    double r = 0.0;
+    for (int j = lane; j < m; j += 32) {
+      if (t < 2 && j == i) continue;
+      const double v = fma(__ldg(row + __ldg(ci + j)), gamma, 1.0);
+      r += v * v * v;
+    }
+    acc += r;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double tot = 0.0;
+    for (int w = 0; w < kKidThreads / 32; ++w) tot += red[w];
+    out[(long long)s * 3 + t] = tot;
+  }
+}
+
 }  // namespace hrv_metrics
 
 using namespace hrv_metrics;
@@ -280,4 +461,66 @@ extern "C" int hrv_ssim(const void* im1, const void* im2, int32_t dtype, int32_t
   if ((rc = launched("ssim"))) return rc;
   ssim_finish_kernel<<<(unsigned)n, 256, 0, st>>>(slab, tiles, 1.0 / ((double)(h - 2 * kSsimR) * (double)(w - 2 * kSsimR)), out);
   return launched("ssim finish");
+}
+
+extern "C" int hrv_resize_bilinear_nhwc(const float* x, int32_t n, int32_t c, int32_t h, int32_t w, int32_t unit_range, const hrv_tensor* dst,
+                                        hrv_stream stream) {
+  if (!x || !dst || !dst->ptr || n < 1 || c < 1 || h < 1 || w < 1)
+    return set_error(HRV_EINVAL, "resize_bilinear_nhwc: bad arguments");
+  const int c8 = (c + 7) / 8 * 8;
+  if (dst->dtype != HRV_F32 || dst->n != n || dst->c != c || dst->h < 1 || dst->w < 1 || dst->pitch < c8)
+    return set_error(HRV_EINVAL, "resize_bilinear_nhwc: dst must be fp32 NHWC (n=%d, oh, ow, c=%d) with pitch >= %d", n, c, c8);
+  const long long total = (long long)n * dst->h * dst->w * c8;
+  // torch's scale for an explicit output size: (float)in / out
+  const float rh = (float)h / dst->h, rw = (float)w / dst->w;
+  resize_bilinear_kernel<<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(x, c, h, w, rh, rw, unit_range ? 1 : 0, (float*)dst->ptr,
+                                                                                  dst->h, dst->w, dst->pitch, c8, total);
+  return launched("resize_bilinear_nhwc");
+}
+
+extern "C" int hrv_global_avgpool(const hrv_tensor* x, const hrv_tensor* y, hrv_stream stream) {
+  if (!x || !y || !x->ptr || !y->ptr || x->dtype != HRV_F32 || y->dtype != HRV_F32 || x->h < 1 || x->w < 1 || x->c < 1 || x->pitch < x->c)
+    return set_error(HRV_EINVAL, "global_avgpool: x and y must be fp32 NHWC");
+  if (y->n != x->n || y->c != x->c || y->h != 1 || y->w != 1 || y->pitch < y->c)
+    return set_error(HRV_EINVAL, "global_avgpool: y must be (n, 1, 1, c)");
+  const long long total = (long long)x->n * x->c;
+  global_avgpool_kernel<<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>((const float*)x->ptr, x->h * x->w, x->pitch, x->c,
+                                                                               (float*)y->ptr, y->pitch, total);
+  return launched("global_avgpool");
+}
+
+extern "C" size_t hrv_gram_f64_workspace_bytes(int32_t m, int32_t n, int32_t k) {
+  if (m < 1 || n < 1 || k < 1) return 0;
+  const int splits = gram_splits(m, n, k, nullptr);
+  return splits > 1 ? (size_t)splits * m * n * sizeof(double) : 0;
+}
+
+extern "C" int hrv_gram_f64(const void* a, int64_t sam, int64_t sak, const void* b, int64_t sbn, int64_t sbk, int32_t dtype, int32_t m, int32_t n,
+                            int32_t k, double* c, int64_t ldc, int32_t accumulate, void* workspace, size_t workspace_bytes, hrv_stream stream) {
+  if (!a || !b || !c || m < 1 || n < 1 || k < 1 || ldc < n || (dtype != HRV_GRAM_F32 && dtype != HRV_GRAM_F64))
+    return set_error(HRV_EINVAL, "gram_f64: bad arguments");
+  int kper;
+  const int splits = gram_splits(m, n, k, &kper);
+  const size_t need = hrv_gram_f64_workspace_bytes(m, n, k);
+  if (need && (!workspace || workspace_bytes < need))
+    return set_error(HRV_EINVAL, "gram_f64: workspace too small (%zu < %zu)", workspace_bytes, need);
+  cudaStream_t st = (cudaStream_t)stream;
+  double* slab = splits > 1 ? (double*)workspace : nullptr;
+  const dim3 grid((unsigned)((n + kGramT - 1) / kGramT), (unsigned)((m + kGramT - 1) / kGramT), (unsigned)splits);
+  if (dtype == HRV_GRAM_F32)
+    gram_kernel<float><<<grid, kGramThreads, 0, st>>>((const float*)a, sam, sak, (const float*)b, sbn, sbk, m, n, k, kper, c, ldc, accumulate, slab);
+  else
+    gram_kernel<double><<<grid, kGramThreads, 0, st>>>((const double*)a, sam, sak, (const double*)b, sbn, sbk, m, n, k, kper, c, ldc, accumulate, slab);
+  int rc = launched("gram_f64");
+  if (rc || splits == 1) return rc;
+  gram_finish_kernel<<<nblocks((long long)m * n, 256), 256, 0, st>>>(slab, splits, m, n, c, ldc, accumulate);
+  return launched("gram_f64 finish");
+}
+
+extern "C" int hrv_kid_sums(const double* gxx, const double* gyy, const double* gxy, int32_t na, int32_t nb, const int32_t* ix, const int32_t* iy,
+                            int32_t subsets, int32_t m, double gamma, double* out, hrv_stream stream) {
+  if (!gxx || !gyy || !gxy || !ix || !iy || !out || subsets < 1 || m < 2 || m > na || m > nb)
+    return set_error(HRV_EINVAL, "kid_sums: bad arguments (2 <= subset size <= the number of features of each set)");
+  kid_sums_kernel<<<dim3((unsigned)subsets, 3), kKidThreads, 0, (cudaStream_t)stream>>>(gxx, gyy, gxy, na, nb, ix, iy, m, gamma, out);
+  return launched("kid_sums");
 }

@@ -274,13 +274,13 @@ def pack_weight(w, off, cin_total=None, interleave=None, bn=None, flops_per_pixe
 
 
 def s2d_weight(w, pad):
-    """Rewrite a stride-2 conv weight (Cout,Cin,k,k) with padding `pad` (k=4,pad=2 or k=3,pad=1) as the
-    2x2 stride-1 weight over the space-to-depth input with channel order (py*2+px)*Cin8 + ci, off=(1,1)."""
+    """Rewrite a stride-2 conv weight (Cout,Cin,k,k) with padding `pad` as the 2x2 stride-1 weight over the space-to-depth input
+    with channel order (py*2+px)*Cin8 + ci: (k=4, pad=2) and (k=3, pad=1) run with off=(1,1); (k=3, pad=0) with off=(0,0)."""
     cout, cin, k, _ = w.shape
     cin8 = round_up(cin, 8)
     out = torch.zeros((cout, 4 * cin8, 2, 2), dtype=w.dtype, device=w.device)
-    shift = 0 if (k == 4 and pad == 2) else 1
-    assert (k, pad) in ((4, 2), (3, 1))
+    shift = 1 if (k == 3 and pad == 1) else 0
+    assert (k, pad) in ((4, 2), (3, 1), (3, 0)), (k, pad)
     for ky in range(k):
         ty, py = divmod(ky + shift, 2)
         for kx in range(k):
@@ -411,8 +411,8 @@ def instnorm_apply(x, mean, rstd, act, out=None):
     return out
 
 
-def space_to_depth(x):
-    out = Act.empty(x.n, (x.h + 1) // 2, (x.w + 1) // 2, 4 * round_up(x.c, 8))
+def space_to_depth(x, dtype=None):
+    out = Act.empty(x.n, (x.h + 1) // 2, (x.w + 1) // 2, 4 * round_up(x.c, 8), dtype=dtype)
     tx, ty = x.ct(), out.ct()
     with _Timed("glue", 0.0, label="space_to_depth"):
         capi.check(_L(x).hrv_space_to_depth(ctypes.byref(tx), ctypes.byref(ty), _stream()), "space_to_depth")
@@ -852,9 +852,9 @@ def lpips_input(x, shift, scale):
     return out
 
 
-def maxpool3s2(x):
-    """nn.MaxPool2d(3, 2) on an fp32 NHWC Act (hrv_maxpool3s2): bit-exact."""
-    y = Act.empty(x.n, (x.h - 3) // 2 + 1, (x.w - 3) // 2 + 1, x.c, dtype=torch.float32)
+def maxpool3s2(x, out=None):
+    """nn.MaxPool2d(3, 2) on an fp32 NHWC Act (hrv_maxpool3s2): bit-exact.  out: the destination Act (e.g. a channel slice)."""
+    y = Act.empty(x.n, (x.h - 3) // 2 + 1, (x.w - 3) // 2 + 1, x.c, dtype=torch.float32) if out is None else out
     tx, ty = x.ct(), y.ct()
     with _Timed("glue", 0.0, label="maxpool3s2"):
         capi.check(capi.lib().hrv_maxpool3s2(ctypes.byref(tx), ctypes.byref(ty), _stream()), "maxpool3s2")
@@ -890,4 +890,71 @@ def ssim(im1, im2, data_range=255.0):
     dt = capi.SSIM_U8 if im1.dtype == torch.uint8 else capi.SSIM_F32
     with _Timed("glue", 0.0, launches=2, label="ssim"):
         capi.check(L.hrv_ssim(im1.data_ptr(), im2.data_ptr(), dt, n, h, w, float(data_range), out.data_ptr(), ws.data_ptr(), nws, _stream()), "ssim")
+    return out
+
+
+def resize_bilinear_nhwc(x, size, unit_range=False, pitch=None):
+    """F.interpolate(x, size, mode='bilinear', align_corners=False) of fp32 NCHW x (cuda), bit-identical, as an fp32 NHWC Act
+    (hrv_resize_bilinear_nhwc); unit_range=True maps x to 2x - 1 first.  The pad channels up to the next multiple of 8 are zeros."""
+    assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 4
+    x = x.contiguous()
+    n, c, h, w = x.shape
+    out = Act.empty(n, size[0], size[1], c, dtype=torch.float32, device=x.device, pitch=pitch)
+    t = out.ct()
+    with _Timed("glue", 0.0, label="resize_bilinear_nhwc"):
+        capi.check(capi.lib().hrv_resize_bilinear_nhwc(x.data_ptr(), n, c, h, w, int(bool(unit_range)), ctypes.byref(t), _stream()),
+                   "resize_bilinear_nhwc")
+    return out
+
+
+def global_avgpool(x, out=None):
+    """The mean over the pixels of an fp32 Act (hrv_global_avgpool: fp64 sum in a fixed order, one rounding) as an (n,1,1,c) fp32 Act."""
+    y = Act.empty(x.n, 1, 1, x.c, dtype=torch.float32, device=x.buf.device) if out is None else out
+    tx, ty = x.ct(), y.ct()
+    with _Timed("glue", 0.0, label="global_avgpool"):
+        capi.check(capi.lib().hrv_global_avgpool(ctypes.byref(tx), ctypes.byref(ty), _stream()), "global_avgpool")
+    return y
+
+
+def _gram_operand(t, k_major):
+    """(strides (row, k), rows, k) of a 2-D fp32 / fp64 tensor read as a (rows, K) operand; k_major: t is (K, rows)."""
+    assert t.is_cuda and t.dim() == 2 and t.dtype in (torch.float32, torch.float64)
+    s0, s1 = t.stride()
+    return ((s1, s0), t.shape[1], t.shape[0]) if k_major else ((s0, s1), t.shape[0], t.shape[1])
+
+
+def gram_f64(a, b, out=None, k_major=False, accumulate=False):
+    """a @ b.T in fp64 (hrv_gram_f64: every sum in a fixed order) of a (M,K) and b (N,K) cuda tensors, fp32 or fp64 (one dtype);
+    k_major=True reads both as (K,M) / (K,N), i.e. computes a.T @ b.  out: fp64 (M,N) with unit column stride, overwritten or, with
+    accumulate=True, added to."""
+    assert a.dtype == b.dtype
+    (sam, sak), m, k = _gram_operand(a, k_major)
+    (sbn, sbk), n, kb = _gram_operand(b, k_major)
+    assert k == kb, (tuple(a.shape), tuple(b.shape), k_major)
+    if out is None:
+        assert not accumulate
+        out = torch.empty((m, n), dtype=torch.float64, device=a.device)
+    assert out.dtype == torch.float64 and out.shape == (m, n) and out.stride(1) == 1
+    L = capi.lib()
+    nws = int(L.hrv_gram_f64_workspace_bytes(m, n, k))
+    ws = torch.empty(max(nws, 8), dtype=torch.uint8, device=a.device)  # split-K slabs, added in a fixed order
+    dt = capi.GRAM_F32 if a.dtype == torch.float32 else capi.GRAM_F64
+    with _Timed("gram", 2.0 * m * n * k, launches=2 if nws else 1, label="gram %dx%dx%d" % (m, n, k)):
+        capi.check(L.hrv_gram_f64(a.data_ptr(), sam, sak, b.data_ptr(), sbn, sbk, dt, m, n, k, out.data_ptr(), out.stride(0), int(bool(accumulate)),
+                                  ws.data_ptr(), nws, _stream()), "gram_f64")
+    return out
+
+
+def kid_sums(gxx, gyy, gxy, ix, iy, gamma):
+    """fp64 [S,3] per-subset sums of KID's polynomial kernel (g*gamma + 1)^3 over the Gram matrices (hrv_kid_sums): off-diagonal
+    X-X, off-diagonal Y-Y and all X-Y pairs of subset s, whose feature indices are the rows ix[s], iy[s] (int32 (S, m) cuda)."""
+    na, nb = gxx.shape[0], gyy.shape[0]
+    assert gxx.shape == (na, na) and gyy.shape == (nb, nb) and gxy.shape == (na, nb)
+    assert all(t.is_contiguous() and t.dtype == torch.float64 for t in (gxx, gyy, gxy))
+    assert ix.dtype == torch.int32 and iy.dtype == torch.int32 and ix.shape == iy.shape and ix.is_contiguous() and iy.is_contiguous()
+    s, m = ix.shape
+    out = torch.empty((s, 3), dtype=torch.float64, device=gxx.device)
+    with _Timed("glue", 0.0, label="kid_sums"):
+        capi.check(capi.lib().hrv_kid_sums(gxx.data_ptr(), gyy.data_ptr(), gxy.data_ptr(), na, nb, ix.data_ptr(), iy.data_ptr(), s, m, float(gamma),
+                                           out.data_ptr(), _stream()), "kid_sums")
     return out

@@ -45,6 +45,37 @@ size_t hrv_ssim_workspace_bytes(int32_t n, int32_t h, int32_t w);
 int hrv_ssim(const void* im1, const void* im2, int32_t dtype, int32_t n, int32_t h, int32_t w, double data_range, double* out,
              void* workspace, size_t workspace_bytes, hrv_stream stream);
 
+/* ---- Inception-v3 (Inception Score, FID, KID; evaluate.py:43,75-76,96-106).  The convolutions run on hrv_conv2d_fwd in fp32 storage
+ * (3xTF32) with BatchNorm as the epilogue's scale / shift, stride-2 ones on hrv_space_to_depth, the max pools on hrv_maxpool3s2. */
+
+/* F.interpolate(x, (dst.h, dst.w), mode='bilinear', align_corners=False, antialias=False), bit-identical to torch's kernel, from fp32
+ * NCHW x [n][c][h][w] to fp32 NHWC dst (n, oh, ow, c), pitch >= round_up(c, 8); channels [c, round_up(c, 8)) are written as zeros.
+ * unit_range != 0 maps every input value v to 2v - 1 before the interpolation (images in [0, 1] to the network's [-1, 1]). */
+int hrv_resize_bilinear_nhwc(const float* x, int32_t n, int32_t c, int32_t h, int32_t w, int32_t unit_range, const hrv_tensor* dst,
+                             hrv_stream stream);
+
+/* Global average pool: y (n, 1, 1, c) fp32 = the mean of x (n, h, w, c) fp32 over its h*w pixels, summed in fp64 in raster order and
+ * rounded once. */
+int hrv_global_avgpool(const hrv_tensor* x, const hrv_tensor* y, hrv_stream stream);
+
+/* C = A B^T in fp64:  c[i*ldc + j] (+)= sum_{k'<k} A(i,k') B(j,k'),  A(i,k') = a[i*sam + k'*sak] (i < m),  B(j,k') = b[j*sbn + k'*sbk]
+ * (j < n), elements fp32 (HRV_GRAM_F32) or fp64 (HRV_GRAM_F64); accumulate != 0 adds the product to c instead of overwriting it.
+ * Every product is summed in increasing k' by one thread; a long K over few output tiles is split into ranges whose partial results
+ * land in workspace slabs that a second kernel adds in range order.  The split depends on (m, n, k) only: the result is the same on
+ * every run and every device.  Accesses are coalesced when one of each operand's strides is 1.
+ * workspace: hrv_gram_f64_workspace_bytes(m, n, k) bytes, 8-byte aligned (0: none needed). */
+enum hrv_gram_dtype { HRV_GRAM_F32 = 0, HRV_GRAM_F64 = 1 };
+size_t hrv_gram_f64_workspace_bytes(int32_t m, int32_t n, int32_t k);
+int hrv_gram_f64(const void* a, int64_t sam, int64_t sak, const void* b, int64_t sbn, int64_t sbk, int32_t dtype, int32_t m, int32_t n, int32_t k,
+                 double* c, int64_t ldc, int32_t accumulate, void* workspace, size_t workspace_bytes, hrv_stream stream);
+
+/* The three sums of KID's unbiased MMD^2 for each of `subsets` subsets, over the cubic polynomial kernel k(g) = (g*gamma + 1)^3 of the
+ * precomputed fp64 Gram matrices gxx [na][na] = X X^T, gyy [nb][nb] = Y Y^T and gxy [na][nb] = X Y^T.  ix, iy: int32 [subsets][m]
+ * feature indices (distinct within a subset).  out: fp64 [subsets][3] = { sum_{i!=j} k(gxx[ix_i][ix_j]), sum_{i!=j} k(gyy[iy_i][iy_j]),
+ * sum_{i,j} k(gxy[ix_i][iy_j]) }, each in a fixed order.  2 <= m <= min(na, nb). */
+int hrv_kid_sums(const double* gxx, const double* gyy, const double* gxy, int32_t na, int32_t nb, const int32_t* ix, const int32_t* iy,
+                 int32_t subsets, int32_t m, double gamma, double* out, hrv_stream stream);
+
 #ifdef __cplusplus
 }
 #endif
