@@ -22,9 +22,11 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_version", "hrv_device_sm_count"]
 # include/hrviton_sm100_metrics.h: fp32 / fp64 only, one flavour (no _f16 twin)
 METRICS_EXPORTS = ["hrv_lpips_input", "hrv_maxpool3s2", "hrv_lpips_dist", "hrv_ssim", "hrv_ssim_workspace_bytes", "hrv_resize_bilinear_nhwc",
-                   "hrv_global_avgpool", "hrv_gram_f64", "hrv_gram_f64_workspace_bytes", "hrv_kid_sums"]
+                   "hrv_global_avgpool", "hrv_gram_f64", "hrv_gram_f64_workspace_bytes", "hrv_kid_sums", "hrv_resize_bilinear_fid", "hrv_pool3x3s1"]
 SSIM_U8, SSIM_F32 = 0, 1
 GRAM_F32, GRAM_F64 = 0, 1
+FID_SRC_F32_NCHW, FID_SRC_U8_NHWC = 0, 1
+POOL3X3_AVG_EXCL_PAD, POOL3X3_MAX = 0, 1
 
 
 class Tensor(ctypes.Structure):
@@ -137,6 +139,8 @@ def lib(dtype=None):
     L.hrv_gram_f64_workspace_bytes.argtypes = [i32, i32, i32]
     L.hrv_gram_f64.argtypes = [vp, i64, i64, vp, i64, i64, i32, i32, i32, i32, vp, i64, i32, vp, sz, vp]
     L.hrv_kid_sums.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, f64, vp, vp]
+    L.hrv_resize_bilinear_fid.argtypes = [vp, i32, i32, i32, i32, i32, TP, vp]
+    L.hrv_pool3x3s1.argtypes = [TP, i32, TP, vp]
     for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS:
         fn = getattr(L, name)
         if "_workspace_bytes" in name:

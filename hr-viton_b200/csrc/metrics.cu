@@ -1,8 +1,10 @@
 // metrics.cu — the evaluation metrics of the reference's workflow (include/hrviton_sm100_metrics.h): the LPIPS AlexNet front end
 // and per-layer distance (eval_models/networks_basic.py, eval_models/__init__.py), skimage's Gaussian SSIM as evaluate.py:67 calls
 // it, and the Inception-v3 pieces behind the Inception Score, FID and KID (input resize, global pool, fp64 Gram products, KID subset
-// sums).  fp32 and fp64 only, so this translation unit is compiled once (no 16-bit flavour).  No floating-point atomics: per-block
+// sums, and the stride-1 pools and input of pytorch-fid's FID Inception).  fp32 and fp64 only, so this translation unit is compiled once (no 16-bit flavour).  No floating-point atomics: per-block
 // partials land in slabs that a second kernel adds in a fixed order.
+#include <type_traits>
+
 #include "hrv_host.h"
 
 namespace hrv_metrics {
@@ -219,23 +221,44 @@ int ssim_tiles(int h, int w, int* tiles_x) {
 }
 
 // ------------------------------------------------------------------------------------------------ Inception input resize
-// F.interpolate(x, (oh, ow), mode='bilinear', align_corners=False, antialias=False) on fp32 NCHW, written as fp32 NHWC.  The source
-// index, the weights and the blend are torch's own expressions in the same order (aten upsample_bilinear2d, accscalar_t = float), so
-// the result is bit-identical.  unit != 0 maps every source value v to 2v - 1 first (2v is exact: one rounding, as in torch).  One
-// thread per output element of the first 8-channel groups; channels [c, c8) are written as zeros.
+// F.interpolate(x, (oh, ow), mode='bilinear', align_corners=False, antialias=False), written as fp32 NHWC.  The source index, the
+// weights and the blend are torch's own expressions in the same order (aten upsample_bilinear2d, accscalar_t = float), so the result is
+// bit-identical.  The source reader gives the float value of one tap: fp32 NCHW as is, or uint8 NHWC as TF.to_tensor converts it
+// (u8 / 255, correctly rounded).  kNormBefore maps every tap v to 2v - 1 before the blend (torchvision Inception on [0, 1] images),
+// kNormAfter maps the blended value (pytorch-fid: F.interpolate, then 2x - 1); 2v is exact, so either is one rounding, as in torch.
+// One thread per output element of the first 8-channel groups; channels [c, c8) are written as zeros.
 __device__ __forceinline__ float bilinear_src(float scale, int d) {
-  const float s = scale * (d + static_cast<float>(0.5)) - static_cast<float>(0.5);
+  const float s = __fmaf_rn(scale, __fadd_rn((float)d, 0.5f), -0.5f);  // scale * (d + 0.5) - 0.5, contracted as in torch's kernel
   return s < 0.f ? 0.f : s;
 }
 
-__global__ void resize_bilinear_kernel(const float* __restrict__ x, int c, int h, int w, float rh, float rw, int unit, float* __restrict__ dst,
-                                       int oh, int ow, int pitch, int c8, long long total) {
+struct NchwF32 {
+  const float* p;
+  int c, h, w;
+  __device__ __forceinline__ float operator()(long long img, int ch, int y, int x) const { return __ldg(p + ((img * c + ch) * h + y) * w + x); }
+};
+
+struct NhwcU8 {
+  const unsigned char* p;
+  int c, h, w;
+  __device__ __forceinline__ float operator()(long long img, int ch, int y, int x) const {
+    return __fdiv_rn((float)__ldg(p + ((img * h + y) * w + x) * c + ch), 255.f);
+  }
+};
+
+enum { kNormNone = 0, kNormBefore = 1, kNormAfter = 2 };
+
+__device__ __forceinline__ float to_signed_unit(float v) { return __fsub_rn(__fmul_rn(2.f, v), 1.f); }
+
+template <typename Src, int kNorm>
+__global__ void resize_bilinear_kernel(Src src, float rh, float rw, float* __restrict__ dst, int oh, int ow, int pitch, int c8, long long total) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int ch = (int)(idx % c8);
   const long long pix = idx / c8;
+  const int h = src.h, w = src.w;
   float val = 0.f;
-  if (ch < c) {
+  if (ch < src.c) {
     const int ox = (int)(pix % ow), oy = (int)((pix / ow) % oh);
     const long long img = pix / ((long long)ow * oh);
     const float h1r = bilinear_src(rh, oy);
@@ -248,15 +271,58 @@ __global__ void resize_bilinear_kernel(const float* __restrict__ x, int c, int h
     const int w1p = (w1 < w - 1) ? 1 : 0;
     const float w1lambda = w1r - w1;
     const float w0lambda = static_cast<float>(1) - w1lambda;
-    const float* p = x + (img * c + ch) * h * w;
-    float v00 = __ldg(p + (long long)h1 * w + w1), v01 = __ldg(p + (long long)h1 * w + w1 + w1p);
-    float v10 = __ldg(p + (long long)(h1 + h1p) * w + w1), v11 = __ldg(p + (long long)(h1 + h1p) * w + w1 + w1p);
-    if (unit) {
-      v00 = 2.f * v00 - 1.f; v01 = 2.f * v01 - 1.f; v10 = 2.f * v10 - 1.f; v11 = 2.f * v11 - 1.f;
+    float v00 = src(img, ch, h1, w1), v01 = src(img, ch, h1, w1 + w1p);
+    float v10 = src(img, ch, h1 + h1p, w1), v11 = src(img, ch, h1 + h1p, w1 + w1p);
+    if (kNorm == kNormBefore) {
+      v00 = to_signed_unit(v00); v01 = to_signed_unit(v01); v10 = to_signed_unit(v10); v11 = to_signed_unit(v11);
     }
-    val = h0lambda * (w0lambda * v00 + w1lambda * v01) + h1lambda * (w0lambda * v10 + w1lambda * v11);
+    // h0lambda * (w0lambda * v00 + w1lambda * v01) + h1lambda * (w0lambda * v10 + w1lambda * v11), with the fma contraction torch's
+    // kernel is compiled with spelled out: left to the compiler, the contraction differs between instantiations of this template
+    const float top = __fmaf_rn(w0lambda, v00, __fmul_rn(w1lambda, v01));
+    const float bottom = __fmaf_rn(w0lambda, v10, __fmul_rn(w1lambda, v11));
+    val = __fmaf_rn(h0lambda, top, __fmul_rn(h1lambda, bottom));
+    if (kNorm == kNormAfter) val = to_signed_unit(val);
   }
   dst[pix * pitch + ch] = val;
+}
+
+// ------------------------------------------------------------------------------------------------ 3x3 stride-1 pool
+// F.avg_pool2d(x, 3, 1, 1, count_include_pad=False) (kMode 0) or F.max_pool2d(x, 3, 1, 1) (kMode 1) on fp32 NHWC, y the same extent.
+// As torch's CUDA kernels: the in-image taps in raster order, summed in fp32 from 0 and divided once by their count (correctly
+// rounded), or compared with `v > m || isnan(v)` from -inf (NaN propagates, the first of equal values stays): bit-identical.  One
+// thread per V consecutive channels of one output pixel (V = 4: 16-byte loads and stores, when pitches, channel offset and count allow).
+template <int kMode, int V>
+__global__ void pool3x3s1_kernel(const float* __restrict__ x, int h, int w, int xp, float* __restrict__ y, int yp, int cv, long long total) {
+  using Vec = typename std::conditional<V == 4, float4, float>::type;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const int cg = (int)(idx % cv);
+  const long long pix = idx / cv;
+  const int ox = (int)(pix % w), oy = (int)((pix / w) % h);
+  const long long n = pix / ((long long)w * h);
+  const int y0 = max(oy - 1, 0), y1 = min(oy + 2, h), x0 = max(ox - 1, 0), x1 = min(ox + 2, w);
+  float acc[V];
+#pragma unroll
+  for (int i = 0; i < V; ++i) acc[i] = kMode == 0 ? 0.f : -INFINITY;
+  for (int yy = y0; yy < y1; ++yy)
+    for (int xx = x0; xx < x1; ++xx) {
+      const Vec v = __ldg(reinterpret_cast<const Vec*>(x + ((n * h + yy) * w + xx) * xp) + cg);
+      const float* vf = reinterpret_cast<const float*>(&v);
+#pragma unroll
+      for (int i = 0; i < V; ++i) {
+        if (kMode == 0) acc[i] = __fadd_rn(acc[i], vf[i]);
+        else if (vf[i] > acc[i] || isnan(vf[i])) acc[i] = vf[i];
+      }
+    }
+  if (kMode == 0) {
+    const float cnt = (float)((y1 - y0) * (x1 - x0));
+#pragma unroll
+    for (int i = 0; i < V; ++i) acc[i] = __fdiv_rn(acc[i], cnt);
+  }
+  Vec out;
+#pragma unroll
+  for (int i = 0; i < V; ++i) reinterpret_cast<float*>(&out)[i] = acc[i];
+  reinterpret_cast<Vec*>(y + pix * yp)[cg] = out;
 }
 
 // ------------------------------------------------------------------------------------------------ global average pool
@@ -473,9 +539,56 @@ extern "C" int hrv_resize_bilinear_nhwc(const float* x, int32_t n, int32_t c, in
   const long long total = (long long)n * dst->h * dst->w * c8;
   // torch's scale for an explicit output size: (float)in / out
   const float rh = (float)h / dst->h, rw = (float)w / dst->w;
-  resize_bilinear_kernel<<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(x, c, h, w, rh, rw, unit_range ? 1 : 0, (float*)dst->ptr,
-                                                                                  dst->h, dst->w, dst->pitch, c8, total);
+  const NchwF32 src{x, c, h, w};
+  if (unit_range)
+    resize_bilinear_kernel<NchwF32, kNormBefore><<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(src, rh, rw, (float*)dst->ptr, dst->h,
+                                                                                                         dst->w, dst->pitch, c8, total);
+  else
+    resize_bilinear_kernel<NchwF32, kNormNone><<<nblocks(total, 256), 256, 0, (cudaStream_t)stream>>>(src, rh, rw, (float*)dst->ptr, dst->h,
+                                                                                                       dst->w, dst->pitch, c8, total);
   return launched("resize_bilinear_nhwc");
+}
+
+extern "C" int hrv_resize_bilinear_fid(const void* x, int32_t src, int32_t n, int32_t c, int32_t h, int32_t w, const hrv_tensor* dst,
+                                       hrv_stream stream) {
+  if (!x || !dst || !dst->ptr || n < 1 || c < 1 || h < 1 || w < 1 || (src != HRV_FID_SRC_F32_NCHW && src != HRV_FID_SRC_U8_NHWC))
+    return set_error(HRV_EINVAL, "resize_bilinear_fid: bad arguments");
+  const int c8 = (c + 7) / 8 * 8;
+  if (dst->dtype != HRV_F32 || dst->n != n || dst->c != c || dst->h < 1 || dst->w < 1 || dst->pitch < c8)
+    return set_error(HRV_EINVAL, "resize_bilinear_fid: dst must be fp32 NHWC (n=%d, oh, ow, c=%d) with pitch >= %d", n, c, c8);
+  const long long total = (long long)n * dst->h * dst->w * c8;
+  const float rh = (float)h / dst->h, rw = (float)w / dst->w;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (src == HRV_FID_SRC_U8_NHWC)
+    resize_bilinear_kernel<NhwcU8, kNormAfter><<<nblocks(total, 256), 256, 0, st>>>(NhwcU8{(const unsigned char*)x, c, h, w}, rh, rw,
+                                                                                    (float*)dst->ptr, dst->h, dst->w, dst->pitch, c8, total);
+  else
+    resize_bilinear_kernel<NchwF32, kNormAfter><<<nblocks(total, 256), 256, 0, st>>>(NchwF32{(const float*)x, c, h, w}, rh, rw,
+                                                                                     (float*)dst->ptr, dst->h, dst->w, dst->pitch, c8, total);
+  return launched("resize_bilinear_fid");
+}
+
+extern "C" int hrv_pool3x3s1(const hrv_tensor* x, int32_t mode, const hrv_tensor* y, hrv_stream stream) {
+  if (!x || !y || !x->ptr || !y->ptr || x->dtype != HRV_F32 || y->dtype != HRV_F32 || x->n < 1 || x->h < 1 || x->w < 1 || x->c < 1 ||
+      (mode != HRV_POOL3X3_AVG_EXCL_PAD && mode != HRV_POOL3X3_MAX))
+    return set_error(HRV_EINVAL, "pool3x3s1: x and y must be fp32 NHWC, mode 0 (average) or 1 (max)");
+  if (y->n != x->n || y->h != x->h || y->w != x->w || y->c != x->c || x->pitch < x->c || y->pitch < y->c)
+    return set_error(HRV_EINVAL, "pool3x3s1: y must have x's extent (%d,%d,%d,%d)", x->n, x->h, x->w, x->c);
+  const bool vec4 = x->c % 4 == 0 && x->pitch % 4 == 0 && y->pitch % 4 == 0 && ((uintptr_t)x->ptr & 15) == 0 && ((uintptr_t)y->ptr & 15) == 0;
+  const int cv = vec4 ? x->c / 4 : x->c;
+  const long long total = (long long)x->n * x->h * x->w * cv;
+  const unsigned nb = nblocks(total, 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  const float* xp = (const float*)x->ptr;
+  float* yp = (float*)y->ptr;
+  if (mode == HRV_POOL3X3_AVG_EXCL_PAD) {
+    if (vec4) pool3x3s1_kernel<0, 4><<<nb, 256, 0, st>>>(xp, x->h, x->w, x->pitch, yp, y->pitch, cv, total);
+    else pool3x3s1_kernel<0, 1><<<nb, 256, 0, st>>>(xp, x->h, x->w, x->pitch, yp, y->pitch, cv, total);
+  } else {
+    if (vec4) pool3x3s1_kernel<1, 4><<<nb, 256, 0, st>>>(xp, x->h, x->w, x->pitch, yp, y->pitch, cv, total);
+    else pool3x3s1_kernel<1, 1><<<nb, 256, 0, st>>>(xp, x->h, x->w, x->pitch, yp, y->pitch, cv, total);
+  }
+  return launched("pool3x3s1");
 }
 
 extern "C" int hrv_global_avgpool(const hrv_tensor* x, const hrv_tensor* y, hrv_stream stream) {

@@ -13,12 +13,17 @@ Gaussian SSIM as evaluate.py:67 calls it, and the Inception-v3 metrics: evaluate
     f = metrics.fid(a, b)
     kid_mean, kid_std = metrics.kid(pool_a, pool_b)
 
+    fid_net = metrics.InceptionV3.from_fid_weights("pt_inception-2015-12-05-6726825d.pth")  # pytorch-fid's network
+    pool, logits = fid_net(images01)       # (N,2048), (N,1008); images01 (N,3,H,W) fp32 cuda in [0, 1], or (N,H,W,3) uint8 cuda
+    mu, sigma = metrics.FeatureStats.load_npz("published_stats.npz")
+    f = metrics.fid_of_moments((a.mean(), a.cov()), (mu, sigma))
+
 LPIPS and Inception always run in fp32 storage with 3xTF32 convolutions, whatever ops.get_precision() says: they are the numbers people
 report, and they must not move with the training precision.  They are inference-only (no gradient).
 
-FID and KID here are computed from torchvision's ImageNet Inception-v3.  Published FID / KID numbers use the TensorFlow-ported "FID
-Inception" (pytorch-fid, clean-fid: other pool blocks, 1008 classes), so values from this module are comparable with each other, not
-with those."""
+FID and KID are comparable with published numbers only when they come from the network those numbers used.  from_fid_weights runs
+pytorch-fid's FID Inception (its weights, its stride-1 pools, its resize-then-2x-1 input), so its FID matches pytorch-fid's on the same
+images.  from_torchvision runs torchvision's ImageNet Inception-v3: values from it are comparable with each other only."""
 import os
 import warnings
 
@@ -244,6 +249,40 @@ _BLOCKS = {
                    ["branch3x3dbl_1", "branch3x3dbl_2", ("branch3x3dbl_3a", "branch3x3dbl_3b")], ["branch_pool"]],
 }
 _POOLED = ("InceptionA", "InceptionC", "InceptionE")  # their branch_pool is F.avg_pool2d(3, 1, 1) and a 1x1 BasicConv2d
+# pytorch-fid's FID Inception pools every branch_pool with F.avg_pool2d(3, 1, 1, count_include_pad=False), except Mixed_7c's
+# (FIDInceptionE_2), which takes F.max_pool2d(3, 1, 1)
+_FID_MAX_POOL = "Mixed_7c"
+FID_CLASSES = 1008
+
+
+def fid_inception_model(state_dict_or_path):
+    """pytorch-fid's FID Inception weights (pt_inception-2015-12-05-6726825d.pth: a plain state dict with torchvision's key names) in an
+    eval-mode torchvision Inception3(num_classes=1008, aux_logits=False) on the CPU.  Loading is strict: only the BatchNorm
+    num_batches_tracked counters may be absent; any other missing, extra or mis-shaped key raises ValueError naming it.  Nothing is
+    downloaded: a missing file raises FileNotFoundError."""
+    from torchvision.models.inception import Inception3
+    sd = state_dict_or_path
+    if isinstance(sd, (str, os.PathLike)):
+        if not os.path.isfile(sd):
+            raise FileNotFoundError("FID Inception weights not found: %r (pytorch-fid's pt_inception-2015-12-05-6726825d.pth; nothing "
+                                    "is downloaded)" % os.fspath(sd))
+        sd = torch.load(sd, map_location="cpu", weights_only=True)
+    if not isinstance(sd, dict):
+        raise ValueError("FID Inception weights: expected a state dict, got %s" % type(sd).__name__)
+    model = Inception3(num_classes=FID_CLASSES, aux_logits=False, init_weights=False)
+    own = model.state_dict()
+    missing = sorted(k for k in own if k not in sd and not k.endswith("num_batches_tracked"))
+    if missing:
+        raise ValueError("FID Inception weights: missing key %r (%d missing)" % (missing[0], len(missing)))
+    extra = sorted(k for k in sd if k not in own)
+    if extra:
+        raise ValueError("FID Inception weights: unexpected key %r (%d unexpected)" % (extra[0], len(extra)))
+    for k, v in sd.items():
+        if not torch.is_tensor(v) or tuple(v.shape) != tuple(own[k].shape):
+            raise ValueError("FID Inception weights: %r has shape %s, expected %s"
+                             % (k, tuple(v.shape) if torch.is_tensor(v) else type(v).__name__, tuple(own[k].shape)))
+    model.load_state_dict(sd, strict=False)  # every key but the num_batches_tracked counters checked above
+    return model.eval()
 
 
 def fold_basic_conv(bc, pool=False, affine=None):
@@ -315,10 +354,15 @@ class InceptionV3:
     the stride-2 ones over hrv_space_to_depth, the average-pool branches as 3x3 convolutions with weights w/9, the max pools on
     hrv_maxpool3s2, the branches of a block written into channel slices of one buffer (the torch.cat), then hrv_global_avgpool and fc as
     a 1x1 convolution.  The aux head is never run.  Build it with from_torchvision(model); weights are re-packed whenever a parameter or
-    buffer of the model changes (spade._param_key), and always kept in fp32 whatever ops.get_precision() says."""
+    buffer of the model changes (spade._param_key), and always kept in fp32 whatever ops.get_precision() says.
+    from_fid_weights(...) builds the "fid" variant, pytorch-fid's FID Inception: the same torchvision blocks, but each branch_pool is
+    hrv_pool3x3s1 (average without the padding, Mixed_7c: max) into a scratch buffer followed by its 1x1 BasicConv2d, and the input is
+    hrv_resize_bilinear_fid.  The variant lives here, not in the module types, because pytorch-fid's blocks hold torchvision's modules."""
 
-    def __init__(self, model):
+    def __init__(self, model, variant="torchvision"):
+        assert variant in ("torchvision", "fid")
         self.model = model
+        self.variant = variant
         self._key = None
         self._packs = None
 
@@ -334,13 +378,25 @@ class InceptionV3:
             raise RuntimeError("InceptionV3: the model's weights are on the CPU; move it to the GPU with .cuda() (no CPU fallback)")
         return cls(model)
 
+    @classmethod
+    def from_fid_weights(cls, state_dict_or_path, device="cuda"):
+        """pytorch-fid's FID Inception (fid_inception_v3) with the given weights (a state dict or the path of
+        pt_inception-2015-12-05-6726825d.pth; loaded strictly by fid_inception_model) on `device`.  forward(images) returns the 2048
+        pool features and the 1008 logits of images in [0, 1]: fp32 (N,3,H,W) or uint8 (N,H,W,3), resized to 299x299 as pytorch-fid
+        does (F.interpolate bilinear, then 2x - 1)."""
+        device = torch.device(device)
+        if device.type != "cuda":
+            raise RuntimeError("InceptionV3.from_fid_weights runs on the GPU only (no CPU fallback): got %s" % device)
+        return cls(fid_inception_model(state_dict_or_path).to(device), variant="fid")
+
     @property
     def device(self):
         return self.model.fc.weight.device
 
     def _pack(self):
         m = self.model
-        key = (_param_key(m), bool(m.transform_input))
+        key = (_param_key(m), bool(m.transform_input), self.variant)
+        fold_pool = self.variant != "fid"  # count_include_pad=True is a 3x3 convolution with weights w/9; pytorch-fid's pools are not
         if self._key == key:
             return self._packs
         with torch.no_grad():
@@ -360,7 +416,7 @@ class InceptionV3:
                     for stage in branch:
                         for name in (stage if isinstance(stage, tuple) else (stage,)):
                             if name != "maxpool":
-                                packs[blk + "." + name] = _Conv(getattr(mod, name), pool=(name == "branch_pool" and kind in _POOLED))
+                                packs[blk + "." + name] = _Conv(getattr(mod, name), pool=fold_pool and name == "branch_pool" and kind in _POOLED)
             fc_w = m.fc.weight.detach().float()
             packs["fc"] = (ops.pack_weight(fc_w.reshape(fc_w.shape[0], fc_w.shape[1], 1, 1).contiguous(), (0, 0), storage=_F32),
                            m.fc.bias.detach().float().contiguous())
@@ -384,6 +440,8 @@ class InceptionV3:
             y = x
             for stage in branch[:-1]:
                 y = packs[blk + "." + stage](y)
+            if self.variant == "fid" and branch[-1] == "branch_pool":
+                y = ops.pool3x3s1(y, "max" if blk == _FID_MAX_POOL else "avg")
             for name, width in zip(last, widths):
                 dst = out.slice(c0, width)
                 if name == "maxpool":
@@ -394,6 +452,8 @@ class InceptionV3:
         return out
 
     def _input(self, x, unit_range):
+        if self.variant == "fid":
+            return ops.resize_bilinear_fid(x, (INCEPTION_SIZE, INCEPTION_SIZE))
         n, _, h, w = x.shape
         if (h, w) != (INCEPTION_SIZE, INCEPTION_SIZE) or unit_range:
             return ops.resize_bilinear_nhwc(x, (INCEPTION_SIZE, INCEPTION_SIZE), unit_range=unit_range)
@@ -426,9 +486,16 @@ class InceptionV3:
         expects: [-1, 1] without transform_input (evaluate.py's T3 output), ImageNet-normalised with it.  unit_range=True takes images
         in [0, 1] whatever transform_input says: the network then sees 2x - 1, which for a transform_input model is what ImageNet
         normalisation followed by its transform gives (the transform is not applied a second time).
-        Other sizes than 299x299 are resized bilinearly (F.interpolate, align_corners=False) on the way in, bit for bit as torch does."""
+        Other sizes than 299x299 are resized bilinearly (F.interpolate, align_corners=False) on the way in, bit for bit as torch does.
+        The "fid" variant (from_fid_weights) takes images in [0, 1], fp32 (N,3,H,W) or uint8 (N,H,W,3), and always resizes them to
+        299x299 and then maps them to 2x - 1, as pytorch-fid does; unit_range does not apply to it."""
         _check_images(x, "InceptionV3")
-        if x.dim() != 4 or x.shape[1] != 3 or x.shape[0] < 1 or x.dtype != torch.float32:
+        if self.variant == "fid":
+            if unit_range:
+                raise ValueError("InceptionV3 (fid): images are always in [0, 1] (uint8 or fp32); unit_range does not apply")
+            if x.dim() != 4 or x.shape[0] < 1 or not ((x.dtype == torch.float32 and x.shape[1] == 3) or (x.dtype == torch.uint8 and x.shape[3] == 3)):
+                raise ValueError("InceptionV3 (fid): expected float32 images (N,3,H,W) or uint8 images (N,H,W,3), got %s %s" % (x.dtype, tuple(x.shape)))
+        elif x.dim() != 4 or x.shape[1] != 3 or x.shape[0] < 1 or x.dtype != torch.float32:
             raise ValueError("InceptionV3: expected float32 images (N,3,H,W), got %s %s" % (x.dtype, tuple(x.shape)))
         if x.device != self.device:
             raise RuntimeError("InceptionV3: the images (%s) must be on the device of the model's weights (%s)" % (x.device, self.device))
@@ -509,6 +576,21 @@ class FeatureStats:
         mu = self.mean()
         return (self.sum_sq - self.n * torch.outer(mu, mu)) / (self.n - 1)
 
+    def save_npz(self, path):
+        """mean() and cov() in pytorch-fid's statistics format: np.savez_compressed(path, mu=..., sigma=...), float64."""
+        np.savez_compressed(path, mu=self.mean().cpu().numpy(), sigma=self.cov().cpu().numpy())
+
+    @staticmethod
+    def load_npz(path):
+        """(mu, sigma) float64 numpy arrays from statistics in pytorch-fid's format (e.g. save_npz's, or published ones)."""
+        with np.load(path) as f:
+            if "mu" not in f or "sigma" not in f:
+                raise ValueError("%s holds %s, not pytorch-fid statistics (mu, sigma)" % (path, sorted(f.keys())))
+            mu, sigma = f["mu"].astype(np.float64), f["sigma"].astype(np.float64)
+        if mu.ndim != 1 or sigma.shape != (mu.shape[0], mu.shape[0]):
+            raise ValueError("%s: mu %s and sigma %s are not (d,) and (d, d)" % (path, mu.shape, sigma.shape))
+        return mu, sigma
+
 
 def fid_from_moments(mu_a, sig_a, mu_b, sig_b, mm):
     """||mu_a - mu_b||^2 + Tr sig_a + Tr sig_b - 2 Tr sqrt(sig_a sig_b) in fp64.  The trace term is the sum of the square roots of the
@@ -532,6 +614,24 @@ def fid(stats_a, stats_b):
         raise ValueError("fid: the two statistics must have one dimension and one device")
     with torch.cuda.device(stats_a.sum.device):
         return fid_from_moments(stats_a.mean(), stats_a.cov(), stats_b.mean(), stats_b.cov(), ops.gram_f64)
+
+
+def fid_of_moments(a, b, device="cuda"):
+    """The FID of two (mu, sigma) pairs, e.g. (stats.mean(), stats.cov()) or FeatureStats.load_npz(path) for published statistics;
+    numpy arrays or tensors, taken as fp64 on `device`.  The same arithmetic as fid(), so equal moments give the same bits."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError("fid_of_moments runs on the GPU only (no CPU fallback): got %s" % device)
+    moments = []
+    for mu, sigma in (a, b):
+        mu, sigma = (torch.as_tensor(t).to(device=device, dtype=torch.float64) for t in (mu, sigma))
+        if mu.dim() != 1 or tuple(sigma.shape) != (mu.shape[0], mu.shape[0]):
+            raise ValueError("fid_of_moments: expected mu (d,) and sigma (d, d), got %s and %s" % (tuple(mu.shape), tuple(sigma.shape)))
+        moments += [mu, sigma]
+    if moments[0].shape != moments[2].shape:
+        raise ValueError("fid_of_moments: the two statistics have dimensions %d and %d" % (moments[0].shape[0], moments[2].shape[0]))
+    with torch.cuda.device(device):
+        return fid_from_moments(*moments, ops.gram_f64)
 
 
 def kid_subsets(n_a, n_b, subsets, subset_size, seed=0):

@@ -907,6 +907,34 @@ def resize_bilinear_nhwc(x, size, unit_range=False, pitch=None):
     return out
 
 
+def resize_bilinear_fid(x, size=(299, 299), pitch=None):
+    """pytorch-fid's Inception input as an fp32 NHWC Act (n, size, 3) (hrv_resize_bilinear_fid): F.interpolate(v, size, 'bilinear',
+    align_corners=False) and then 2v - 1, bit-identical.  x: fp32 NCHW (n,c,h,w) cuda in [0, 1], or uint8 NHWC (n,h,w,c) cuda as PIL
+    decodes it (v = u8 / 255, as TF.to_tensor).  The pad channels up to the next multiple of 8 are zeros."""
+    assert x.is_cuda and x.dim() == 4 and x.dtype in (torch.float32, torch.uint8)
+    x = x.contiguous()
+    if x.dtype == torch.uint8:
+        (n, h, w, c), src = x.shape, capi.FID_SRC_U8_NHWC
+    else:
+        (n, c, h, w), src = x.shape, capi.FID_SRC_F32_NCHW
+    out = Act.empty(n, size[0], size[1], c, dtype=torch.float32, device=x.device, pitch=pitch)
+    t = out.ct()
+    with _Timed("glue", 0.0, label="resize_bilinear_fid"):
+        capi.check(capi.lib().hrv_resize_bilinear_fid(x.data_ptr(), src, n, c, h, w, ctypes.byref(t), _stream()), "resize_bilinear_fid")
+    return out
+
+
+def pool3x3s1(x, mode, out=None):
+    """A 3x3, stride-1, padding-1 pool of an fp32 NHWC Act (hrv_pool3x3s1), bit-exact: mode 'avg' is F.avg_pool2d(count_include_pad=False),
+    'max' is F.max_pool2d.  out: the destination Act of x's extent (e.g. a channel slice)."""
+    m = {"avg": capi.POOL3X3_AVG_EXCL_PAD, "max": capi.POOL3X3_MAX}[mode]
+    y = Act.empty(x.n, x.h, x.w, x.c, dtype=torch.float32, device=x.buf.device) if out is None else out
+    tx, ty = x.ct(), y.ct()
+    with _Timed("glue", 0.0, label="pool3x3s1 " + mode):
+        capi.check(capi.lib().hrv_pool3x3s1(ctypes.byref(tx), m, ctypes.byref(ty), _stream()), "pool3x3s1")
+    return y
+
+
 def global_avgpool(x, out=None):
     """The mean over the pixels of an fp32 Act (hrv_global_avgpool: fp64 sum in a fixed order, one rounding) as an (n,1,1,c) fp32 Act."""
     y = Act.empty(x.n, 1, 1, x.c, dtype=torch.float32, device=x.buf.device) if out is None else out

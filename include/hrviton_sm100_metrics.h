@@ -54,6 +54,23 @@ int hrv_ssim(const void* im1, const void* im2, int32_t dtype, int32_t n, int32_t
 int hrv_resize_bilinear_nhwc(const float* x, int32_t n, int32_t c, int32_t h, int32_t w, int32_t unit_range, const hrv_tensor* dst,
                              hrv_stream stream);
 
+/* ---- pytorch-fid's FID Inception (fid_inception_v3): torchvision's Inception3(num_classes=1008, aux_logits=False) whose pool
+ * branches are F.avg_pool2d(3, 1, 1, count_include_pad=False) (Mixed_5b-5d, 6b-6e, 7b) and F.max_pool2d(3, 1, 1) (Mixed_7c). */
+
+/* pytorch-fid's input: F.interpolate(v, (dst.h, dst.w), mode='bilinear', align_corners=False), then 2v - 1 (after the blend), written
+ * as fp32 NHWC dst (n, oh, ow, c), pitch >= round_up(c, 8), channels [c, round_up(c, 8)) zero; bit-identical to those torch calls.
+ * src HRV_FID_SRC_F32_NCHW: x is fp32 NCHW [n][c][h][w], v = x (images in [0, 1]).  src HRV_FID_SRC_U8_NHWC: x is uint8 NHWC
+ * [n][h][w][c] (interleaved, as PIL decodes RGB), v = u8 / 255 correctly rounded in fp32, as TF.to_tensor computes it. */
+enum hrv_fid_src { HRV_FID_SRC_F32_NCHW = 0, HRV_FID_SRC_U8_NHWC = 1 };
+int hrv_resize_bilinear_fid(const void* x, int32_t src, int32_t n, int32_t c, int32_t h, int32_t w, const hrv_tensor* dst, hrv_stream stream);
+
+/* A 3x3, stride-1, padding-1 pool of fp32 NHWC x into fp32 NHWC y of the same extent (y may be a channel slice of a wider buffer).
+ * mode HRV_POOL3X3_AVG_EXCL_PAD: F.avg_pool2d(count_include_pad=False), the in-image taps summed in raster order in fp32 and divided
+ * once by their count; mode HRV_POOL3X3_MAX: F.max_pool2d (NaN propagates, ties keep the first value).  Both bit-identical to torch's
+ * CUDA kernels.  16-byte accesses when c, both pitches and both pointers allow them. */
+enum hrv_pool3x3_mode { HRV_POOL3X3_AVG_EXCL_PAD = 0, HRV_POOL3X3_MAX = 1 };
+int hrv_pool3x3s1(const hrv_tensor* x, int32_t mode, const hrv_tensor* y, hrv_stream stream);
+
 /* Global average pool: y (n, 1, 1, c) fp32 = the mean of x (n, h, w, c) fp32 over its h*w pixels, summed in fp64 in raster order and
  * rounded once. */
 int hrv_global_avgpool(const hrv_tensor* x, const hrv_tensor* y, hrv_stream stream);
