@@ -49,14 +49,14 @@ int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* 
   return HRV_OK;
 }
 
-int encode_nhwc_map(CUtensorMap* map, const hrv_tensor& t, int box_c, int box_w, int box_h, int box_n) {
+int encode_nhwc_map(CUtensorMap* map, const hrv_tensor& t, int box_c, int box_w, int box_h, int box_n, CUtensorMapSwizzle swizzle) {
   const bool f32 = t.dtype == HRV_F32;
   const cuuint64_t elem = f32 ? 4 : 2;
   const cuuint64_t dims[4] = {(cuuint64_t)t.c, (cuuint64_t)t.w, (cuuint64_t)t.h, (cuuint64_t)t.n};
   const cuuint64_t strides[3] = {(cuuint64_t)t.pitch * elem, (cuuint64_t)t.w * t.pitch * elem, (cuuint64_t)t.h * t.w * t.pitch * elem};
   const cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_h, (cuuint32_t)box_n};
   const cuuint32_t es[4] = {1, 1, 1, 1};
-  return encode_tensor_map(map, 4, t.ptr, dims, strides, box, es, CU_TENSOR_MAP_SWIZZLE_128B,
+  return encode_tensor_map(map, 4, t.ptr, dims, strides, box, es, swizzle,
                            f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 }
 

@@ -20,8 +20,10 @@ int sm_count();
 int encode_tensor_map(CUtensorMap* map, int rank, void* base, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
                       const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle,
                       CUtensorMapDataType type = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
-// 4-D SWIZZLE_128B map {c, w, h, n} of the NHWC tensor `t` (bf16 / fp16 or fp32 by t.dtype) with box {box_c, box_w, box_h, box_n}.
-int encode_nhwc_map(CUtensorMap* map, const hrv_tensor& t, int box_c, int box_w, int box_h, int box_n);
+// 4-D map {c, w, h, n} of the NHWC tensor `t` (bf16 / fp16 or fp32 by t.dtype) with box {box_c, box_w, box_h, box_n}, swizzled
+// SWIZZLE_128B unless told otherwise (box_c * element size must not exceed the swizzle width).
+int encode_nhwc_map(CUtensorMap* map, const hrv_tensor& t, int box_c, int box_w, int box_h, int box_n,
+                    CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 // hrv_conv2d_fwd on fp32 storage (conv_f32.cu, compiled once): both flavours of hrv_conv2d_fwd hand an fp32 input to it.
 int conv2d_fwd_tf32x3(const hrv_conv_params* p, hrv_stream stream);
 
