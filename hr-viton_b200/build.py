@@ -2,7 +2,7 @@
 
 Every kernel translation unit is compiled twice: once as is (bf16 activation storage, entry points hrv_<op>) and once with
 -DHRV_F16 -Dhrv=hrv_f16 (IEEE fp16 storage, entry points hrv_<op>_f16; csrc/hrv_f16_rename.h).  capi.cu (error text, device
-introspection, TMA descriptor encoder) is shared, and so are conv_f32.cu and metrics.cu, which compute in fp32 / fp64 only."""
+introspection, TMA descriptor encoder) is shared, and so are conv_f32.cu and metrics.cu, which compute in fp32 / fp64 only, and data_kernels.cu, which takes uint8 and writes fp32."""
 import os
 import subprocess
 import sys
@@ -12,8 +12,8 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libhrviton_sm100.so")
 SHARED = ["capi.cu"]
-KERNEL_TUS = ["conv_igemm.cu", "aux_kernels.cu", "norm_bwd.cu", "conv_wgrad.cu", "glue_kernels.cu", "conv_f32.cu", "syncbn.cu", "metrics.cu"]
-SINGLE = ("conv_f32.cu", "metrics.cu")  # no 16-bit storage: compiled once
+KERNEL_TUS = ["conv_igemm.cu", "aux_kernels.cu", "norm_bwd.cu", "conv_wgrad.cu", "glue_kernels.cu", "conv_f32.cu", "syncbn.cu", "metrics.cu", "data_kernels.cu"]
+SINGLE = ("conv_f32.cu", "metrics.cu", "data_kernels.cu")  # no 16-bit storage: compiled once
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
@@ -26,6 +26,7 @@ def _stale():
     t = os.path.getmtime(LIB)
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if not f.endswith(".o")] + [os.path.join(PKG, "..", "include", "hrviton_sm100.h"),
                                                                                          os.path.join(PKG, "..", "include", "hrviton_sm100_metrics.h"),
+                                                                                         os.path.join(PKG, "..", "include", "hrviton_sm100_data.h"),
                                                                                          os.path.abspath(__file__)]
     return any(os.path.getmtime(d) > t for d in deps)
 

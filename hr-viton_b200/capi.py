@@ -27,11 +27,24 @@ SSIM_U8, SSIM_F32 = 0, 1
 GRAM_F32, GRAM_F64 = 0, 1
 FID_SRC_F32_NCHW, FID_SRC_U8_NHWC = 0, 1
 POOL3X3_AVG_EXCL_PAD, POOL3X3_MAX = 0, 1
+# include/hrviton_sm100_data.h: uint8 in, fp32 out, one flavour (no _f16 twin)
+DATA_EXPORTS = ["hrv_pil_resample_pass", "hrv_pil_nearest", "hrv_agnostic_composite", "hrv_viton_assemble"]
 
 
 class Tensor(ctypes.Structure):
     _fields_ = [("ptr", ctypes.c_void_p), ("n", ctypes.c_int32), ("h", ctypes.c_int32), ("w", ctypes.c_int32),
                 ("c", ctypes.c_int32), ("pitch", ctypes.c_int32), ("dtype", ctypes.c_int32)]
+
+
+class VitonPlanes(ctypes.Structure):
+    _fields_ = [("image", ctypes.c_void_p), ("cloth", ctypes.c_void_p * 2), ("cloth_mask", ctypes.c_void_p * 2), ("pose", ctypes.c_void_p),
+                ("densepose", ctypes.c_void_p), ("agnostic", ctypes.c_void_p), ("parse", ctypes.c_void_p)]
+
+
+class VitonOutputs(ctypes.Structure):
+    _fields_ = [("image", ctypes.c_void_p), ("cloth", ctypes.c_void_p * 2), ("cloth_mask", ctypes.c_void_p * 2), ("pose", ctypes.c_void_p),
+                ("densepose", ctypes.c_void_p), ("agnostic", ctypes.c_void_p), ("pcm", ctypes.c_void_p), ("parse_cloth", ctypes.c_void_p),
+                ("parse_onehot", ctypes.c_void_p)]
 
 
 class ConvParams(ctypes.Structure):
@@ -141,7 +154,11 @@ def lib(dtype=None):
     L.hrv_kid_sums.argtypes = [vp, vp, vp, i32, i32, vp, vp, i32, i32, f64, vp, vp]
     L.hrv_resize_bilinear_fid.argtypes = [vp, i32, i32, i32, i32, i32, TP, vp]
     L.hrv_pool3x3s1.argtypes = [TP, i32, TP, vp]
-    for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS:
+    L.hrv_pil_resample_pass.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, i32, i32, vp, vp]
+    L.hrv_pil_nearest.argtypes = [vp, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp]
+    L.hrv_agnostic_composite.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
+    L.hrv_viton_assemble.argtypes = [ctypes.POINTER(VitonPlanes), ctypes.POINTER(VitonOutputs), i32, i32, i32, vp]
+    for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS + DATA_EXPORTS:
         fn = getattr(L, name)
         if "_workspace_bytes" in name:
             fn.restype = ctypes.c_size_t

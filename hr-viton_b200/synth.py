@@ -119,3 +119,65 @@ def spade_noise(n, h, w, seed, idx):
     """
     draw = normalish((n, w, h, 1), seed, "noise%d" % idx)
     return draw.transpose(1, 3)[:, 0].contiguous()
+
+
+def write_vitonhd(root, n, h=1024, w=768, seed=0, datamode="train", pairs="pairs.txt"):
+    """A seeded synthetic VITON-HD tree under root/datamode in the real layout and image modes, plus root/pairs (each person paired
+    with the next sample's cloth for the unpaired setting): image / cloth / image-densepose RGB jpg, cloth-mask L jpg, image-parse-v3
+    and image-parse-agnostic-v3.2 P png (all 20 labels in blobs, arm labels 14 / 15 along the arms), openpose_img RGB png, and
+    openpose_json with a plausible body (every third sample misses an elbow or a wrist: the (0,0) keypoints get_agnostic skips).
+    Returns the sample names."""
+    import json
+    import os
+
+    from PIL import Image, ImageDraw
+    g = _rng(seed, "vitonhd")
+    base = os.path.join(root, datamode)
+    for d in ("image", "cloth", "cloth-mask", "image-parse-v3", "image-parse-agnostic-v3.2", "openpose_img", "openpose_json", "image-densepose"):
+        os.makedirs(os.path.join(base, d), exist_ok=True)
+    palette = [int(v) for v in g.integers(0, 256, 256 * 3)]
+
+    def smooth(c):
+        t = g.integers(0, 256, (max(2, h // 32), max(2, w // 32), c), dtype=np.uint8)
+        return Image.fromarray(t[..., 0] if c == 1 else t).resize((w, h), Image.BILINEAR)
+
+    def labels(arms, kp):
+        lab = np.kron(g.integers(0, 20, (max(1, h // 64) + 1, max(1, w // 64) + 1)), np.ones((64, 64), np.int64))[:h, :w].astype(np.uint8)
+        im = Image.fromarray(lab, "P")
+        im.putpalette(palette)
+        if arms:
+            d = ImageDraw.Draw(im)
+            for label, joints in ((14, (5, 6, 7)), (15, (2, 3, 4))):
+                pts = [tuple(kp[j]) for j in joints if kp[j][0] or kp[j][1]]
+                if len(pts) > 1:
+                    d.line(pts, label, width=max(2, w // 12))
+        return im
+
+    names = []
+    for i in range(n):
+        name = "%06d_00.jpg" % i
+        names.append(name)
+        s = np.array([w, h], np.float64)
+        kp = np.zeros((25, 3))
+        body = {0: (0.5, 0.12), 1: (0.5, 0.22), 2: (0.33, 0.23), 3: (0.27, 0.38), 4: (0.25, 0.52), 5: (0.67, 0.23), 6: (0.73, 0.38),
+                7: (0.75, 0.52), 8: (0.5, 0.55), 9: (0.42, 0.56), 12: (0.58, 0.56), 10: (0.42, 0.75), 13: (0.58, 0.75)}
+        for j, (fx, fy) in body.items():
+            kp[j, :2] = (np.array([fx, fy]) + g.uniform(-0.03, 0.03, 2)) * s
+            kp[j, 2] = 0.9
+        if i % 3 == 1:
+            kp[(4, 7)[i % 2], :2] = 0.0  # a missing wrist
+        elif i % 3 == 2:
+            kp[(3, 6)[i % 2], :2] = 0.0  # a missing elbow
+        p = os.path.join
+        smooth(3).save(p(base, "image", name), quality=95)
+        smooth(3).save(p(base, "cloth", name), quality=95)
+        Image.fromarray(((np.asarray(smooth(1)) > 128) * 255).astype(np.uint8), "L").save(p(base, "cloth-mask", name), quality=95)
+        labels(True, kp[:, :2]).save(p(base, "image-parse-v3", name.replace(".jpg", ".png")))
+        labels(False, kp[:, :2]).save(p(base, "image-parse-agnostic-v3.2", name.replace(".jpg", ".png")))
+        smooth(3).save(p(base, "openpose_img", name.replace(".jpg", "_rendered.png")))
+        smooth(3).save(p(base, "image-densepose", name), quality=95)
+        with open(p(base, "openpose_json", name.replace(".jpg", "_keypoints.json")), "w") as f:
+            json.dump({"version": 1.3, "people": [{"person_id": [-1], "pose_keypoints_2d": kp.ravel().tolist()}]}, f)
+    with open(os.path.join(root, pairs), "w") as f:
+        f.write("".join("%s %s\n" % (names[i], names[(i + 1) % n]) for i in range(n)))
+    return names

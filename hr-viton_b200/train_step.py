@@ -111,7 +111,6 @@ class BatchFeeder:
     ONEHOT = ("parse_agnostic", "parse")
 
     def __init__(self, batch_cpu, device):
-        self.device = device
         self.host, self.classes = {}, {}
         for k, v in batch_cpu.items():
             if k in self.ONEHOT and v.dim() == 4 and v.shape[1] > 1:
@@ -119,11 +118,16 @@ class BatchFeeder:
                 self.host[k] = v.argmax(1, keepdim=True).to(torch.uint8).contiguous().pin_memory()
             else:
                 self.host[k] = v.contiguous().pin_memory()
+        self._init_staging(device)
         self.slots = [{k: torch.empty(v.shape, dtype=v.dtype, device=device) for k, v in self.host.items()} for _ in range(2)]
+        self.bytes_per_step = int(sum(v.numel() * v.element_size() for v in self.host.values()))
+
+    def _init_staging(self, device):
+        """The copy stream and the two slots' events (shared with data.VitonHDLoader, which stages a new host batch per step)."""
+        self.device = device
         self.copy_stream = torch.cuda.Stream(device)
         self.ready = [torch.cuda.Event(), torch.cuda.Event()]
         self.free = [torch.cuda.Event(), torch.cuda.Event()]
-        self.bytes_per_step = int(sum(v.numel() * v.element_size() for v in self.host.values()))
         self.slot = 0
 
     def prefetch(self, slot=None):
@@ -137,19 +141,23 @@ class BatchFeeder:
     def consume(self, out):
         """Makes the staged batch of the current slot available in `out` (dict of fp32 device tensors), then starts the copy of the
         next batch into the other slot.  Stream-ordered: no host synchronisation."""
-        from . import ops
         slot = self.slot
         cur = torch.cuda.current_stream()
         cur.wait_event(self.ready[slot])
-        for k, v in self.slots[slot].items():
-            if k in self.classes:
-                ops.onehot_u8(v, self.classes[k], out=out[k])
-            else:
-                out[k].copy_(v, non_blocking=True)
+        self._expand(self.slots[slot], out)
         self.free[slot].record(cur)
         self.slot ^= 1
         self.prefetch(self.slot)
         return out
+
+    def _expand(self, staged, out):
+        """Turns one staged slot into the step's fp32 tensors, on the current stream."""
+        from . import ops
+        for k, v in staged.items():
+            if k in self.classes:
+                ops.onehot_u8(v, self.classes[k], out=out[k])
+            else:
+                out[k].copy_(v, non_blocking=True)
 
 
 class _GraphMixin:
