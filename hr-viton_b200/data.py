@@ -321,9 +321,10 @@ class _EpochSampler(torch.utils.data.Sampler):
         self.args = (n_items, batch_size)
         self.seed, self.shuffle, self.rank, self.world = seed, shuffle, rank, world
         self.epoch = 0
+        self.start = 0  # samples of the epoch to skip (VitonHDLoader.start_at)
 
     def __iter__(self):
-        return iter(shard_indices(*self.args, self.epoch, self.seed, self.shuffle, self.rank, self.world).tolist())
+        return iter(shard_indices(*self.args, self.epoch, self.seed, self.shuffle, self.rank, self.world)[self.start:].tolist())
 
     def __len__(self):
         return len(shard_indices(*self.args, 0, self.seed, False, self.rank, self.world))
@@ -364,23 +365,26 @@ class VitonHDLoader(BatchFeeder):
     given tensors (flat keys; cloth / cloth_mask take the paired cloth), stream-ordered, and starts the copy of the following batch,
     so a captured trainer replays with replay(feeder=loader).  Incomplete batches are dropped (drop_last, as in the reference).
 
-    With an initialised process group of world size W, rank r reads a disjoint 1/W of each epoch's permutation (shard_indices)."""
+    With an initialised process group of world size W, rank r reads a disjoint 1/W of each epoch's permutation (shard_indices);
+    shard=False reads the whole set on every rank.  position() and start_at() save and restore where the batches stand."""
 
     def __init__(self, dataroot, datamode, data_list, fine_height, fine_width, batch_size, workers=4, mode="train", keys=None, shuffle=True,
-                 seed=0):
+                 seed=0, shard=True):
         import torch.distributed as dist
         self.dataset = VitonHDDataset(dataroot, datamode, data_list, fine_height, fine_width, mode=mode, keys=keys)
         ds = self.dataset
-        self.keys, self.batch_size = ds.keys, int(batch_size)
-        rank, world = (dist.get_rank(), dist.get_world_size()) if dist.is_available() and dist.is_initialized() else (0, 1)
+        self.keys, self.batch_size, self.seed = ds.keys, int(batch_size), seed
+        rank, world = (dist.get_rank(), dist.get_world_size()) if shard and dist.is_available() and dist.is_initialized() else (0, 1)
         self.sampler = _EpochSampler(len(ds), self.batch_size, seed, shuffle, rank, world)
         if len(self.sampler) == 0:
             raise ValueError("%d samples make no full batch of %d on each of %d ranks" % (len(ds), self.batch_size, world))
         self.loader = torch.utils.data.DataLoader(ds, batch_size=self.batch_size, sampler=self.sampler, num_workers=workers, collate_fn=collate,
-                                                  pin_memory=True, drop_last=True, persistent_workers=workers > 0)
+                                                  pin_memory=True, drop_last=True, persistent_workers=workers > 0,
+                                                  generator=torch.Generator().manual_seed(int(seed)))  # leaves torch's CPU generator alone
         self._init_staging(torch.device("cuda", torch.cuda.current_device()))  # the kernels launch on the current device's stream
         self.slots, self.host, self.names, self.epochs = [None, None], [None, None], [None, None], [None, None]
-        self._iter, self._epoch = None, 0
+        self.positions = [None, None]
+        self._iter, self._epoch, self._index, self._skip = None, 0, 0, 0
         h, w, fh, fw = ds.src_h, ds.src_w, ds.fine_height, ds.fine_width
         self.resize = (h, w) != (fh, fw)  # torchvision returns an image of the requested size unchanged
         dev = self.device
@@ -405,20 +409,42 @@ class VitonHDLoader(BatchFeeder):
 
     # -------- host batches, cycling through epochs
     def _next_host(self):
+        """(epoch, batch index in the epoch, host batch) of the next batch from the workers."""
         while True:
             if self._iter is None:
-                self.sampler.epoch = self._epoch
+                self.sampler.epoch, self.sampler.start = self._epoch, self._skip * self.batch_size
+                self._index, self._skip = self._skip, 0
                 self._iter = iter(self.loader)
             try:
-                return self._epoch, next(self._iter)
+                b = next(self._iter)
+                self._index += 1
+                return self._epoch, self._index - 1, b
             except StopIteration:
                 self._iter = None
                 self._epoch += 1
 
+    def position(self):
+        """(epoch, batch index) of the batch that the next consume() / next_batch() delivers."""
+        if self.host[self.slot] is not None:
+            return self.positions[self.slot]
+        if self._iter is None:
+            return self._epoch, self._skip
+        return self._epoch, self._index
+
+    def start_at(self, epoch, index):
+        """The next batch delivered is batch `index` of epoch `epoch` (position()), as an uninterrupted run would have delivered it:
+        each epoch's order derives from (seed, epoch) alone, and the workers skip the earlier samples without reading them.  Batches
+        already staged are dropped.  An index at or past the end of the epoch starts the next one."""
+        if int(epoch) < 0 or int(index) < 0:
+            raise ValueError("start_at(%r, %r): epoch and index must be >= 0" % (epoch, index))
+        torch.cuda.current_stream().wait_stream(self.copy_stream)  # a staged copy may still be writing a slot
+        self.host, self.names, self.epochs, self.positions = [None, None], [None, None], [None, None], [None, None]
+        self._iter, self._epoch, self._skip = None, int(epoch), int(index)
+
     def prefetch(self, slot=None):
         """Takes the next host batch from the workers and starts its copy into staging slot `slot` on the copy stream."""
         slot = self.slot if slot is None else slot
-        epoch, b = self._next_host()
+        epoch, index, b = self._next_host()
         ds = self.dataset
         n = self.batch_size
         if self.slots[slot] is None:
@@ -437,7 +463,7 @@ class VitonHDLoader(BatchFeeder):
                     self.slots[slot][k][:v.shape[0]].copy_(v, non_blocking=True)
             self.ready[slot].record(self.copy_stream)
         self.bytes_per_step = int(sum(v.numel() for k, v in b.items() if torch.is_tensor(v)))
-        self.host[slot], self.names[slot], self.epochs[slot] = b, (b["im_name"], b["c_name"]), epoch
+        self.host[slot], self.names[slot], self.epochs[slot], self.positions[slot] = b, (b["im_name"], b["c_name"]), epoch, (epoch, index)
 
     def consume(self, out):
         unknown = [k for k in out if k not in TRAIN_KEYS]

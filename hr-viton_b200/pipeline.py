@@ -174,7 +174,9 @@ class _GraphRunner:
             e = None
         if e is None:
             e = self._Entry({k: v.detach().clone() for k, v in inputs.items()}, state)
-            e.captured = CapturedCall(lambda: self._body(e.static), warm=1, keep_rng=True)
+            # thread-local capture: a DataLoader's pin-memory thread in this process (data.VitonHDLoader feeding a training run that
+            # evaluates through this runner) allocates pinned memory while the graph is captured, which global mode refuses
+            e.captured = CapturedCall(lambda: self._body(e.static), warm=1, keep_rng=True, capture_error_mode="thread_local")
             # the graph reads the packed weights / folded BatchNorm tables of the modules' caches: keeping them alive means an
             # eager call that rebuilds a cache never frees memory a captured graph still reads
             e.keep = [getattr(s, a) for m in self._modules for s in m.modules() for a in ("_cache", "_pyr") if getattr(s, a, None) is not None]

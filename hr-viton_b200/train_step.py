@@ -166,16 +166,67 @@ class _GraphMixin:
 
     _captured = None
 
-    def capture(self, batch, *step_args, warm=2):
+    def capture(self, batch, *step_args, warm=2, rollback=False):
+        """rollback=True: the warm-up steps and the capture leave no trace.  Parameters, buffers (BatchNorm running statistics,
+        spectral-norm vectors), Adam state, loss scalers and torch's CPU and CUDA generators are put back as they were, by copy_ into
+        the same storage, so the graph's addresses stay valid and the first replay is the step that would have come next."""
         from .graphs import CapturedCall
         self._static = {k: v.clone() for k, v in batch.items()}
         import torch.distributed as dist
         multi = dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1
+        snap = self._snapshot() if rollback else None
+        cpu_rng = torch.get_rng_state() if rollback else None
+
+        def body():
+            if rollback:
+                # fused Adam updates parameters without bumping tensor._version, so a derived-weight cache filled during the
+                # warm-up (the generator's input pyramid, packed by its no-grad forward in the discriminator update) would look
+                # current and the graph would replay those warm-up weights.  A new generation makes the capture record the packing.
+                ops.PARAM_GEN[0] += 1
+            return self.step(self._static, *step_args)
         # with NCCL inside the graph the process group's watchdog thread keeps polling CUDA events: thread-local capture mode keeps
         # those calls from invalidating the capture
-        self._captured = CapturedCall(lambda: self.step(self._static, *step_args), warm=warm,
-                                      capture_error_mode="thread_local" if multi else "global")
+        self._captured = CapturedCall(body, warm=warm, capture_error_mode="thread_local" if multi else "global", keep_rng=rollback)
+        if rollback:
+            self._restore(snap)
+            torch.set_rng_state(cpu_rng)
         return self
+
+    def _state_tensors(self):
+        """Every tensor a training step updates, keyed by storage (modules shared between roles are listed once), and the parameters that
+        have no Adam state yet (the warm-up creates it)."""
+        out, stateless = {}, []
+        for m in self.modules():
+            for t in list(m.parameters()) + list(m.buffers()):
+                out.setdefault(t.data_ptr(), t)
+        for opt in (self.opt_g, self.opt_d):
+            for group in opt.param_groups:
+                for p in group["params"]:
+                    st = opt.state.get(p)
+                    if not st:
+                        stateless.append((opt, p))
+                    for v in (st or {}).values():
+                        if torch.is_tensor(v):
+                            out.setdefault(v.data_ptr(), v)
+        for sc in self.scalers.values():
+            for t in (sc.scale, sc.growth_tracker, sc.found_inf):
+                out.setdefault(t.data_ptr(), t)
+        return out, stateless
+
+    def _snapshot(self):
+        tensors, stateless = self._state_tensors()
+        return [(t, t.detach().clone()) for t in tensors.values()], stateless
+
+    def _restore(self, snap):
+        saved, stateless = snap
+        with torch.no_grad():
+            for t, v in saved:
+                t.copy_(v)
+            for opt, p in stateless:  # Adam's lazily created state starts at zero (step, exp_avg, exp_avg_sq)
+                for v in opt.state[p].values():
+                    if torch.is_tensor(v):
+                        v.zero_()
+        ops.PARAM_GEN[0] += 1  # parameters changed behind tensor._version: derived caches are stale
 
     def replay(self, batch=None, feeder=None):
         if feeder is not None:
@@ -192,6 +243,59 @@ class _GraphMixin:
         if self._captured is not None:
             self._captured.release()
             self._captured = None
+
+
+class _TrainState:
+    """Learning rates and the resumable optimiser / loss-scaler state shared by both trainers.
+
+    tensor_lr=True builds both fused Adams with a one-element device tensor as lr, which a captured step reads on every replay:
+    set_lr_factor(f) writes base_lr * f into it between replays, without a recapture.  With tensor_lr=False (the default) the
+    optimisers are today's, with a Python float lr."""
+
+    def _make_optimizers(self, g_params, d_params, g_lr, d_lr, betas, tensor_lr):
+        g_params, d_params = list(g_params), list(d_params)
+        self.base_lr = {"G": float(g_lr), "D": float(d_lr)}
+        self.lr_factor = 1.0
+        self.tensor_lr = bool(tensor_lr)
+
+        def lr(name, params):
+            if not tensor_lr:
+                return self.base_lr[name]
+            return torch.tensor(self.base_lr[name], dtype=torch.float32, device=params[0].device)
+        self.opt_g = torch.optim.Adam(g_params, lr=lr("G", g_params), betas=betas, fused=True, capturable=True)
+        self.opt_d = torch.optim.Adam(d_params, lr=lr("D", d_params), betas=betas, fused=True, capturable=True)
+        self._lr = {n: opt.param_groups[0]["lr"] for n, opt in (("G", self.opt_g), ("D", self.opt_d))}
+
+    def set_lr_factor(self, factor):
+        """lr = base_lr * factor for both optimisers, in place (tensor_lr=True only): a captured step uses it from its next replay."""
+        if not self.tensor_lr:
+            raise RuntimeError("set_lr_factor needs a trainer built with tensor_lr=True")
+        self.lr_factor = float(factor)
+        for name, t in self._lr.items():
+            t.fill_(self.base_lr[name] * self.lr_factor)
+
+    def state_dict(self):
+        """Both optimisers' state, the loss scalers and the LR factor (device tensors; the caller moves them where it saves them)."""
+        return {"optimizers": {"G": self.opt_g.state_dict(), "D": self.opt_d.state_dict()},
+                "scalers": {n: sc.state_dict() for n, sc in self.scalers.items()}, "lr_factor": self.lr_factor}
+
+    def load_state_dict(self, sd):
+        """Restores state_dict() before capture(): Optimizer.load_state_dict replaces the state tensors, which a captured graph
+        would keep using.  The optimisers keep their own lr (a device tensor with tensor_lr=True), set from the saved factor."""
+        if self._captured is not None:
+            raise RuntimeError("load_state_dict() after capture(): release_graph() first, or load before capturing")
+        if set(sd["scalers"]) != set(self.scalers):
+            raise ValueError("the saved loss scalers %s do not match this trainer's %s" % (sorted(sd["scalers"]), sorted(self.scalers)))
+        for name, opt in (("G", self.opt_g), ("D", self.opt_d)):
+            opt.load_state_dict(sd["optimizers"][name])
+            for group in opt.param_groups:
+                group["lr"] = self._lr[name]
+        for name, sc in self.scalers.items():
+            sc.load_state_dict(sd["scalers"][name])
+        if self.tensor_lr:
+            self.set_lr_factor(sd["lr_factor"])
+        elif sd["lr_factor"] != 1.0:
+            raise ValueError("LR factor %r saved; a trainer without tensor_lr trains at factor 1" % (sd["lr_factor"],))
 
 
 class _LossScaling:
@@ -218,23 +322,25 @@ class _LossScaling:
             sc.update()
 
 
-class Stage2Trainer(_GraphMixin, _LossScaling):
+class Stage2Trainer(_GraphMixin, _TrainState, _LossScaling):
     """Holds the optimisers / criteria of train_generator.py:145-159 and runs one step.  loss_scale: None or "dynamic" (fp16 storage:
-    apex O1's dynamic loss scaling, see loss_scale.py and _LossScaling)."""
+    apex O1's dynamic loss scaling, see loss_scale.py and _LossScaling).  tensor_lr: see _TrainState."""
 
     def __init__(self, tocg, generator, discriminator, vgg, lambda_feat=10.0, lambda_vgg=10.0, g_lr=1e-4, d_lr=4e-4,
-                 reducers=None, occlusion=True, loss_scale=None):
+                 reducers=None, occlusion=True, loss_scale=None, tensor_lr=False):
         from .spade import GANLoss
         self.tocg, self.G, self.D, self.vgg = tocg, generator, discriminator, vgg
         self.crit_gan = GANLoss("hinge")
         self.vgg_weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
         self.lambda_feat, self.lambda_vgg = lambda_feat, lambda_vgg
         self.occlusion = occlusion  # opt.occlusion: the README trains stage 2 with --occlusion
-        self.opt_g = torch.optim.Adam(generator.parameters(), lr=g_lr, betas=(0.0, 0.9), fused=True, capturable=True)
-        self.opt_d = torch.optim.Adam(discriminator.parameters(), lr=d_lr, betas=(0.0, 0.9), fused=True, capturable=True)
+        self._make_optimizers(generator.parameters(), discriminator.parameters(), g_lr, d_lr, (0.0, 0.9), tensor_lr)
         self.reducers = reducers or {}  # {"G": GradBucketReducer, "D": ...} for data-parallel runs
         self._explicit_reduce = _attach_reducers(self.reducers)
         self._init_loss_scale(loss_scale, {"G": self.opt_g, "D": self.opt_d})
+
+    def modules(self):
+        return [self.tocg, self.G, self.D, self.vgg]
 
     @staticmethod
     def _split(pred):
@@ -300,22 +406,25 @@ def synthetic_batch(n, h, w, device, seed=0):
 
 # ------------------------------------------------------------------------------------------------ stage 1 (train_condition.py)
 
-class Stage1Trainer(_GraphMixin, _LossScaling):
+class Stage1Trainer(_GraphMixin, _TrainState, _LossScaling):
     """One train_condition.py step (train_condition.py:133-286) with the README's flags (--Ddownx2 --Ddropout --lasttvonly
     --interflowloss --occlusion): tocg forward+backward on this repo's kernels (train-mode BatchNorm), L1 + VGG + TV + CE + LSGAN.
-    loss_scale: None or "dynamic" (as Stage2Trainer)."""
+    loss_scale: None or "dynamic" (as Stage2Trainer).  lr: both optimisers' (--G_lr, --D_lr), unless d_lr is given.  tensor_lr: see
+    _TrainState."""
 
     def __init__(self, tocg, D, vgg, lr=2e-4, lasttvonly=True, interflowloss=True, occlusion=True, tvlambda=2.0, ce_lambda=10.0,
-                 gan_lambda=1.0, reducers=None, loss_scale=None):
+                 gan_lambda=1.0, reducers=None, loss_scale=None, d_lr=None, tensor_lr=False):
         self.tocg, self.D, self.vgg = tocg, D, vgg
         self.lasttvonly, self.interflowloss, self.occlusion = lasttvonly, interflowloss, occlusion
         self.tvlambda, self.ce_lambda, self.gan_lambda = tvlambda, ce_lambda, gan_lambda
         self.vgg_weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
-        self.opt_g = torch.optim.Adam(tocg.parameters(), lr=lr, betas=(0.5, 0.999), fused=True, capturable=True)
-        self.opt_d = torch.optim.Adam(D.parameters(), lr=lr, betas=(0.5, 0.999), fused=True, capturable=True)
+        self._make_optimizers(tocg.parameters(), D.parameters(), lr, lr if d_lr is None else d_lr, (0.5, 0.999), tensor_lr)
         self.reducers = reducers or {}
         self._explicit_reduce = _attach_reducers(self.reducers)
         self._init_loss_scale(loss_scale, {"G": self.opt_g, "D": self.opt_d})
+
+    def modules(self):
+        return [self.tocg, self.D, self.vgg]
 
     @staticmethod
     def _remove_overlap(seg_out, warped_cm):  # train_condition.py:26-31
