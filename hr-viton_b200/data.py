@@ -1,8 +1,11 @@
 """VITON-HD input pipeline: the tensors of cp_dataset.CPDataset / cp_dataset_test.CPDatasetTest, bit-identical, from the on-disk
 VITON-HD tree (jpg / png / json), with the pixel work on the GPU.
 
-The CPU workers (VitonHDDataset, run by a torch DataLoader) only decode the files with PIL and rasterise get_agnostic's pose shapes
-as one bit plane; they ship uint8 at source resolution.  The device (include/hrviton_sm100_data.h) composites the agnostic image,
+The CPU workers (VitonHDDataset, run by a torch DataLoader) read each JPEG's header and ship the files the device decodes
+(jpeg.device_decodable: baseline, grayscale or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) as their entropy-coded bytes, which hrviton_b200.jpeg
+decodes on the device bit for bit as PIL does, straight into the batch's staged uint8 planes; every other file (the PNGs, and JPEGs
+such as progressive ones) they decode with PIL and ship as uint8 at source resolution.  They also rasterise get_agnostic's pose
+shapes as one bit plane.  The file's header selects the path; there is no option.  The device (include/hrviton_sm100_data.h) composites the agnostic image,
 resizes with Pillow's own fixed-point arithmetic (tables built here), regroups the 20 parse labels to 13 and writes the fp32 outputs
 in one assembly launch; the 13-channel maps are expanded from one byte per pixel by hrv_onehot_u8.  VitonHDLoader stages each batch
 on a copy stream with two slots (train_step.BatchFeeder), so `Stage2Trainer.replay(feeder=loader)` trains from disk.
@@ -17,7 +20,7 @@ import numpy as np
 import torch
 from PIL import Image, ImageDraw
 
-from . import capi
+from . import capi, jpeg
 from .train_step import BatchFeeder
 
 PRECISION_BITS = 22  # Pillow's fixed-point precision for 8-bit resampling
@@ -267,6 +270,22 @@ class VitonHDDataset(torch.utils.data.Dataset):
             raise ValueError("%s: %dx%d, the other planes are %dx%d" % (path, a.shape[0], a.shape[1], self.src_h, self.src_w))
         return a
 
+    def _plane(self, path, modes, to_rgb=False):
+        """A JPEG plane the device decodes as its jpeg.Compact (header and entropy-coded bytes; PIL only reads the header, so the mode
+        and size checks keep their messages), any other file as PIL's uint8 array (converted to RGB with to_rgb)."""
+        im = Image.open(path)
+        if modes and im.mode not in modes:
+            raise ValueError("%s: mode %s, the loader reproduces %s only" % (path, im.mode, "/".join(modes)))
+        if (im.height, im.width) != (self.src_h, self.src_w):
+            raise ValueError("%s: %dx%d, the other planes are %dx%d" % (path, im.height, im.width, self.src_h, self.src_w))
+        if im.format == "JPEG":
+            with open(path, "rb") as f:
+                c = jpeg.compact(f.read())
+            if c is not None and (c.height, c.width) == (self.src_h, self.src_w):
+                c.name = path
+                return c
+        return self._array(im.convert("RGB") if to_rgb else im, path, modes)
+
     def __getitem__(self, index):
         paths = self._paths(index)
         im_name, c_name = self.names(index)
@@ -276,18 +295,18 @@ class VitonHDDataset(torch.utils.data.Dataset):
             if p == "cloth":  # the reference converts the cloth to RGB; the other images go to ToTensor as decoded
                 path = paths["cloth"][cloth_i]
                 cloth_i += 1
-                rgb.append(self._array(Image.open(path).convert("RGB"), path, None))
+                rgb.append(self._plane(path, None, to_rgb=True))
             else:
-                rgb.append(self._array(Image.open(paths[p]), paths[p], ("RGB",)))
+                rgb.append(self._plane(paths[p], ("RGB",)))
         if rgb:
-            out["rgb"] = np.stack(rgb)
+            out["rgb"] = rgb
         if self.lab_planes:
             lab = np.stack([self._array(Image.open(paths[p]), paths[p], ("P", "L")) for p in self.lab_planes])
             if lab.max() > 19:
                 raise ValueError("%s: parse label %d, cp_dataset's one-hot has 20 classes" % (paths[self.lab_planes[0]], lab.max()))
             out["lab"] = lab
         if self.mask_sets:
-            out["cm"] = np.stack([self._array(Image.open(p), p, ("L",)) for p in paths["cloth_mask"]])
+            out["cm"] = [self._plane(p, ("L",)) for p in paths["cloth_mask"]]
         if self.keypoints:
             with open(paths["keypoints"]) as f:
                 pose = np.array(json.load(f)["people"][0]["pose_keypoints_2d"]).reshape((-1, 3))[:, :2]
@@ -296,8 +315,31 @@ class VitonHDDataset(torch.utils.data.Dataset):
 
 
 def collate(samples):
-    """Stacks a batch plane-major ((planes, n, h, w[, 3]) uint8), so that each plane of the batch is one contiguous device image stack."""
-    out = {k: torch.from_numpy(np.stack([s[k] for s in samples], 1)) for k in ("rgb", "lab", "cm") if k in samples[0]}
+    """Stacks a batch plane-major ((planes, n, h, w[, 3]) uint8), so that each plane of the batch is one contiguous device image stack.
+    Images the device decodes travel as their entropy-coded bytes instead: 'jpeg' lists their jpeg.Compacts and 'jpeg_to' their
+    (key, plane, sample) destinations, with the bytes packed into one buffer 'jpeg_bytes'.  Where a key mixes both, its PIL images
+    travel as one stack '<key>_pil' with their (plane, sample) in '<key>_to'."""
+    out = {k: torch.from_numpy(np.stack([s[k] for s in samples], 1)) for k in ("lab",) if k in samples[0]}
+    items, item_to = [], []
+    for k in ("rgb", "cm"):
+        if k not in samples[0]:
+            continue
+        pil, pil_to = [], []
+        for p in range(len(samples[0][k])):
+            for i, s in enumerate(samples):
+                if isinstance(s[k][p], jpeg.Compact):
+                    items.append(s[k][p])
+                    item_to.append((k, p, i))
+                else:
+                    pil.append(s[k][p])
+                    pil_to.append((p, i))
+        if len(pil) == len(samples) * len(samples[0][k]):
+            out[k] = torch.from_numpy(np.stack(pil)).unflatten(0, (-1, len(samples)))
+        elif pil:
+            out[k + "_pil"], out[k + "_to"] = torch.from_numpy(np.stack(pil)), pil_to
+    if items:
+        out["jpeg_bytes"] = jpeg.pack_entropy(items)
+        out["jpeg"], out["jpeg_to"] = items, item_to
     if "bits" in samples[0]:
         out["bits"] = torch.from_numpy(np.stack([s["bits"] for s in samples]))
     out["im_name"] = [s["im_name"] for s in samples]
@@ -403,6 +445,8 @@ class VitonHDLoader(BatchFeeder):
         if self.resize and ds.mask_sets:
             self.scratch["cm"] = torch.empty((ds.mask_sets, n, fh, fw), dtype=torch.uint8, device=dev)
         self.bytes_per_step = None
+        self.device_decoded = 0  # JPEG files decoded on the device so far (the others were decoded by PIL in the workers)
+        self._jpeg_pending = None
 
     def __len__(self):
         return len(self.sampler) // self.batch_size
@@ -447,23 +491,50 @@ class VitonHDLoader(BatchFeeder):
         epoch, index, b = self._next_host()
         ds = self.dataset
         n = self.batch_size
+        self._check_jpeg_errors()  # the previous batch's decode: the loader raises no later than the next batch
         if self.slots[slot] is None:
             h, w, dev = ds.src_h, ds.src_w, self.device
             s = {}
-            if "rgb" in b:  # one plane more for the agnostic image
-                s["rgb"] = torch.empty((b["rgb"].shape[0] + (1 if ds.keypoints else 0), n, h, w, 3), dtype=torch.uint8, device=dev)
-            for k in ("lab", "cm", "bits"):
-                if k in b:
-                    s[k] = torch.empty(b[k].shape, dtype=torch.uint8, device=dev)
+            if ds.rgb_planes or ds.keypoints:  # one plane more for the agnostic image
+                s["rgb"] = torch.empty((len(ds.rgb_planes) + (1 if ds.keypoints else 0), n, h, w, 3), dtype=torch.uint8, device=dev)
+            if ds.lab_planes:
+                s["lab"] = torch.empty((len(ds.lab_planes), n, h, w), dtype=torch.uint8, device=dev)
+            if ds.mask_sets:
+                s["cm"] = torch.empty((ds.mask_sets, n, h, w), dtype=torch.uint8, device=dev)
+            if ds.keypoints:
+                s["bits"] = torch.empty((n, h, w), dtype=torch.uint8, device=dev)
             self.slots[slot] = s
+        st = self.slots[slot]
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(self.free[slot])  # the batch that used this slot last has been assembled
             for k, v in b.items():
                 if k in ("rgb", "lab", "cm", "bits"):
-                    self.slots[slot][k][:v.shape[0]].copy_(v, non_blocking=True)
+                    st[k][:v.shape[0]].copy_(v, non_blocking=True)
+                elif k in ("rgb_pil", "cm_pil"):
+                    for (p, i), img in zip(b[k[:-4] + "_to"], v):
+                        st[k[:-4]][p, i].copy_(img, non_blocking=True)
+            if "jpeg" in b:
+                batch = jpeg.Batch(b["jpeg"], b["jpeg_bytes"])
+                batch.set_destinations([st[k][p, i] for k, p, i in b["jpeg_to"]])
+                errors = batch.launch(self.device, stream=self.copy_stream)
+                self._jpeg_pending = (torch.empty(errors.shape, dtype=torch.int32).pin_memory(), torch.cuda.Event(), b)
+                self._jpeg_pending[0].copy_(errors, non_blocking=True)
+                self._jpeg_pending[1].record(self.copy_stream)
+                self.device_decoded += len(b["jpeg"])
             self.ready[slot].record(self.copy_stream)
-        self.bytes_per_step = int(sum(v.numel() for k, v in b.items() if torch.is_tensor(v)))
+        self.bytes_per_step = int(sum(v.numel() for k, v in b.items() if torch.is_tensor(v))) + len(b.get("jpeg", ())) * jpeg.DESCRIPTOR_BYTES
         self.host[slot], self.names[slot], self.epochs[slot], self.positions[slot] = b, (b["im_name"], b["c_name"]), epoch, (epoch, index)
+
+    def _check_jpeg_errors(self):
+        """Raises OSError naming the file when the last device decode met corrupt data (waits for that decode)."""
+        if self._jpeg_pending is None:
+            return
+        codes, done, b = self._jpeg_pending
+        self._jpeg_pending = None
+        done.synchronize()
+        if codes.any():
+            names = [c.name for c in b["jpeg"]]
+            jpeg.raise_errors(codes.numpy(), names)
 
     def consume(self, out):
         unknown = [k for k in out if k not in TRAIN_KEYS]

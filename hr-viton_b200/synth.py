@@ -181,3 +181,42 @@ def write_vitonhd(root, n, h=1024, w=768, seed=0, datamode="train", pairs="pairs
     with open(os.path.join(root, pairs), "w") as f:
         f.write("".join("%s %s\n" % (names[i], names[(i + 1) % n]) for i in range(n)))
     return names
+
+
+def jpeg_corpus(seed=0):
+    """Seeded JPEG files as PIL writes them, smooth and noisy: [(name, bytes)] over sizes 1x1 to 256x192, quality 1-100, subsampling
+    4:4:4 / 4:2:2 / 4:2:0, optimized Huffman tables, restart intervals (blocks and rows) and mode L."""
+    import io
+
+    from PIL import Image, ImageFile
+    g = _rng(seed, "jpeg")
+
+    def content(w, h, c, noisy):
+        if noisy:
+            a = g.integers(0, 256, (h, w, c), dtype=np.uint8)
+        else:
+            t = g.integers(0, 256, (max(2, h // 16), max(2, w // 16), c), dtype=np.uint8)
+            a = np.asarray(Image.fromarray(t[..., 0] if c == 1 else t).resize((w, h), Image.BILINEAR)).reshape(h, w, c)
+        return Image.fromarray(a[..., 0] if c == 1 else a, "L" if c == 1 else "RGB")
+
+    def save(im, **kw):
+        buf = io.BytesIO()
+        ImageFile.MAXBLOCK = max(ImageFile.MAXBLOCK, 4 * im.width * im.height * 3)  # optimize=True encodes in one buffer
+        im.save(buf, "JPEG", **kw)
+        return buf.getvalue()
+
+    out = []
+    sizes = [(1, 1), (8, 8), (9, 17), (17, 9), (3, 5), (45, 67), (67, 45), (256, 192)]
+    for w, h in sizes:
+        for q in (1, 10, 50, 75, 95, 100):
+            for sub in (0, 1, 2):
+                noisy = (w * 7 + q + sub) % 2 == 1
+                out.append(("%dx%d_q%d_s%d" % (w, h, q, sub), save(content(w, h, 3, noisy), quality=q, subsampling=sub)))
+        for name, kw in (("opt", {"optimize": True}), ("rstb", {"restart_marker_blocks": 3}), ("rstr", {"restart_marker_rows": 1})):
+            for sub in (0, 1, 2):
+                for noisy in (False, True):
+                    out.append(("%dx%d_%s_s%d_%d" % (w, h, name, sub, noisy), save(content(w, h, 3, noisy), quality=90, subsampling=sub, **kw)))
+        for q in (10, 75, 95):
+            out.append(("%dx%d_L_q%d" % (w, h, q), save(content(w, h, 1, q == 75), quality=q)))
+        out.append(("%dx%d_L_rst" % (w, h), save(content(w, h, 1, False), quality=90, restart_marker_blocks=1)))
+    return out

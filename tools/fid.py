@@ -4,8 +4,9 @@
                             [--save-stats OUT.npz] [--device cuda:0]
 
 A and B are image folders or .npz statistics in pytorch-fid's format (mu, sigma).  A folder's images are the files with pytorch-fid's
-extensions, in sorted order, decoded by PIL (.convert('RGB')) in DataLoader workers into pinned uint8 batches; all images of one batch
-must share a size.  They go to the GPU as uint8 and are resized and normalised there (hrv_resize_bilinear_fid), as pytorch-fid's
+extensions, in sorted order, decoded to RGB as PIL's .convert('RGB') does: JPEGs the device decodes (hrviton_b200.jpeg; the
+reference's try-on outputs are PIL's default baseline JPEG) go to the GPU as their entropy-coded bytes and are decoded there, bit for
+bit as PIL decodes them, every other file is decoded by PIL in the DataLoader workers; all images of one batch must share a size.  They go to the GPU as uint8 and are resized and normalised there (hrv_resize_bilinear_fid), as pytorch-fid's
 TF.to_tensor + F.interpolate + 2x - 1 does.  --save-stats writes A's statistics (A must be a folder).  --kid (two folders only) also
 prints KID's mean and std over metrics.kid's default 100 subsets of 1000 images.  The weights are never downloaded."""
 import argparse
@@ -28,7 +29,7 @@ def image_files(folder):
 
 
 class _Images:
-    """torch Dataset of uint8 (H, W, 3) RGB arrays decoded by PIL."""
+    """torch Dataset of the images: a jpeg.Compact for a JPEG the device decodes, else the uint8 (H, W, 3) RGB array PIL decodes."""
 
     def __init__(self, files):
         self.files = files
@@ -39,17 +40,48 @@ class _Images:
     def __getitem__(self, i):
         import numpy as np
         from PIL import Image
+
+        from hrviton_b200 import jpeg
         with Image.open(self.files[i]) as im:
+            if im.format == "JPEG":
+                with open(self.files[i], "rb") as f:
+                    c = jpeg.compact(f.read(), self.files[i])
+                if c is not None:
+                    return c
             return np.asarray(im.convert("RGB"), dtype=np.uint8)
 
 
-def _collate(arrays):
+def _collate(items):
+    """One pinned uint8 (N, H, W, 3) batch when PIL decoded every image, else (PIL arrays by index, jpeg.Compacts by index, packed
+    entropy-coded bytes)."""
     import numpy as np
     import torch
-    shapes = {a.shape for a in arrays}
+
+    from hrviton_b200 import jpeg
+    shapes = {(c.height, c.width, 3) if isinstance(c, jpeg.Compact) else c.shape for c in items}
     if len(shapes) != 1:
         raise ValueError("fid: the images of one batch must share a size, got %s; resize them first or use --batch-size 1" % sorted(shapes))
-    return torch.from_numpy(np.stack(arrays))
+    dev = [(i, c) for i, c in enumerate(items) if isinstance(c, jpeg.Compact)]
+    if not dev:
+        return torch.from_numpy(np.stack(items))
+    pil = [(i, torch.from_numpy(a)) for i, a in enumerate(items) if not isinstance(a, jpeg.Compact)]
+    return {"shape": shapes.pop(), "pil": pil, "jpeg": dev, "jpeg_bytes": jpeg.pack_entropy([c for _, c in dev])}
+
+
+def _device_batch(batch, device, errors):
+    """The uint8 (N, H, W, 3) CUDA batch of a mixed host batch: the JPEGs decoded into their rows, the PIL images copied.  Appends
+    the decode's device error codes and the files' names to `errors`."""
+    import torch
+
+    from hrviton_b200 import jpeg
+    n = len(batch["pil"]) + len(batch["jpeg"])
+    out = torch.empty((n,) + tuple(batch["shape"]), dtype=torch.uint8, device=device)
+    for i, a in batch["pil"]:
+        out[i].copy_(a, non_blocking=True)
+    b = jpeg.Batch([c for _, c in batch["jpeg"]], batch["jpeg_bytes"])
+    b.set_destinations([out[i] for i, _ in batch["jpeg"]])
+    errors.append((b.launch(device), [c.name for _, c in batch["jpeg"]]))
+    return out
 
 
 def folder_features(files, net, batch_size=50, workers=0, timing=None):
@@ -58,13 +90,17 @@ def folder_features(files, net, batch_size=50, workers=0, timing=None):
     import torch
     loader = torch.utils.data.DataLoader(_Images(files), batch_size=batch_size, shuffle=False, drop_last=False, num_workers=workers,
                                          collate_fn=_collate, pin_memory=True)
-    feats, wait = [], 0.0
+    from hrviton_b200 import jpeg
+    feats, wait, errors = [], 0.0, []
     t0 = time.perf_counter()
     for batch in loader:
         wait += time.perf_counter() - t0
-        pool, _ = net(batch.to(net.device, non_blocking=True))
+        x = batch.to(net.device, non_blocking=True) if torch.is_tensor(batch) else _device_batch(batch, net.device, errors)
+        pool, _ = net(x)
         feats.append(pool)
         t0 = time.perf_counter()
+    for codes, names in errors:  # corrupt JPEG data: raise naming the file
+        jpeg.raise_errors(codes.cpu().numpy(), names)
     if timing is not None:
         timing["wait_s"] = timing.get("wait_s", 0.0) + wait
     return torch.cat(feats)
