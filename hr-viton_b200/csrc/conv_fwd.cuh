@@ -18,8 +18,8 @@
 //                       (network_generator.py:115-121,170-171).
 //               The gate residual modes and gamma_out serve the backward pass and exist on 16-bit storage only.
 //
-// Shared memory of a CTA: 1 KB of mbarriers (full at +0, empty at +128), then `scratch` bytes the kernel owns, then the stage ring
-// (at least the 128 x BNT fp32 epilogue tile).
+// Shared memory of a CTA: 1 KB of mbarriers (full at +0, empty at +128, halo at +256), then `scratch` bytes the kernel owns, then
+// the halo slots (halo main loop only) and the stage ring (together at least the 128 x BNT fp32 epilogue tile).
 #pragma once
 #include "hrv_host.h"
 #include "hrv_ptx.cuh"
@@ -30,6 +30,15 @@ constexpr int kConvConsumers = 2;                        // consumer warpgroups 
 constexpr int kConvThreads = 128 * kConvConsumers + 32;  // + one producer warp
 constexpr uint32_t kConvRowBytes = 128;                  // one K block of one pixel / weight row: one SWIZZLE_128B row
 constexpr uint32_t kConvABytes = 128 * kConvRowBytes;    // 128 pixels
+
+// Halo main loop of conv_wgmma_kernel (16-bit storage, chosen by conv_fwd from the shape): the tile is 2 rows x kHaloTW pixels of
+// one image, and the producer loads its input halo once per K chunk c, as the TMA box {64 ch, kHaloTW + KW - 1, 2 + KH - 1, 1}, into
+// its own 1024-byte aligned slot with its own full barrier (bar_halo).  The stage ring behind the slots carries only B boxes.  Every
+// tap then reads its A operand out of the slot: warpgroup w's 64 pixels are one contiguous run of halo row w + ky from pixel kx.
+constexpr int kHaloTW = 64;
+__host__ __device__ constexpr uint32_t halo_box_bytes(int kh, int kw) { return kConvRowBytes * (uint32_t)(kHaloTW + kw - 1) * (uint32_t)(1 + kh); }
+__host__ __device__ constexpr uint32_t halo_slot_bytes(int kh, int kw) { return (halo_box_bytes(kh, kw) + 1023u) & ~1023u; }
+__device__ __forceinline__ uint32_t bar_halo(uint32_t bars, int c) { return bars + 256u + 8u * c; }
 
 // T = activation storage: __nv_bfloat16 (__half in the fp16 flavour) or float.
 template <typename T>
@@ -43,6 +52,7 @@ struct alignas(64) ConvArgs {
   int tw_log, th_log;
   int tiles_x, tiles_y, tiles_n;
   int KH, KW, off_y, off_x, chunks;
+  int halo;                        // conv_wgmma_kernel's halo main loop (tmA boxes the tile's halo; stage ring = B boxes only)
   int stages, n_gemm;
   int epi, act;
   const float* scale;
@@ -91,6 +101,7 @@ __device__ __forceinline__ ConvTile conv_prologue(const ConvArgs<T>& a) {
       mbar_init(bar_full(t.bars, s), 1);
       mbar_init(bar_empty(t.bars, s), 4 * kConvConsumers);  // one arrival per consumer warp
     }
+    for (int c = 0; c < (a.halo ? a.chunks : 0); ++c) mbar_init(bar_halo(t.bars, c), 1);
     fence_mbar_init();
   }
   __syncthreads();
@@ -126,8 +137,8 @@ __device__ __forceinline__ void conv_produce(const ConvArgs<T>& a, const ConvTil
 }
 
 // ------------------------------------------------------------------------------------------------ epilogue
-// The epilogue runs after the main loop and is staged through the stage ring, which is idle by then (the producer issued exactly KT
-// loads and the consumers waited on all of them):
+// The epilogue runs after the main loop and is staged through the stage ring (halo slots first in the halo main loop), which is idle
+// by then (the producer issued exactly KT loads, plus one halo box per chunk, and the consumers waited on all of them):
 //   1. each consumer thread writes its wgmma fragment into an fp32 [128 pixels][BNT] tile at the start of the ring;
 //   2. the 256 consumer threads walk the tile in row order.  A thread owns one 8-channel group (8 LINEAR columns, or 16 interleaved
 //      SPADE gamma/beta columns) and visits every (256 / threads per pixel)-th pixel, so x, the residual, out and gamma_out move as
@@ -413,8 +424,15 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
   // N tile: 64 columns for narrow GEMMs, else 128 (a 64 x 128 fp32 accumulator is 64 registers per thread).  Independent of the
   // packing's bn: the weight map's row extent is the packed n_pad, rows past it are zero fill.
   const int bnt = p->n_gemm <= 64 ? 64 : 128;
-  const int TW = pick_pow2(out.w, 128);
-  const int TH = pick_pow2(out.h, 128 / TW);
+  a.chunks = (in.c + budget.kblock - 1) / budget.kblock;
+  // Halo main loop (16-bit storage): for every kernel with more than one tap whose output rows split into 64-pixel runs and whose halo
+  // slots leave room for at least two B stages.  A 3x3 layer stages each input pixel once per chunk instead of once per tap.
+  const uint32_t halo_slot = halo_slot_bytes(p->kh, p->kw);
+  const uint32_t b_stage = (uint32_t)(budget.planes * bnt) * kConvRowBytes;
+  a.halo = !f32 && p->kh * p->kw > 1 && out.w % kHaloTW == 0 &&
+           (uint64_t)a.chunks * halo_slot + 2u * b_stage <= budget.smem - 2048u - budget.scratch;
+  const int TW = a.halo ? kHaloTW : pick_pow2(out.w, 128);
+  const int TH = a.halo ? 2 : pick_pow2(out.h, 128 / TW);
   const int TN = 128 / (TW * TH);
   a.tw_log = log2i(TW); a.th_log = log2i(TH);
   a.tiles_x = (out.w + TW - 1) / TW;
@@ -422,7 +440,6 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
   const int tiles_img = (out.n + TN - 1) / TN;
   a.tiles_n = (p->n_gemm + bnt - 1) / bnt;
   a.KH = p->kh; a.KW = p->kw; a.off_y = p->off_y; a.off_x = p->off_x;
-  a.chunks = (in.c + budget.kblock - 1) / budget.kblock;
   a.n_gemm = p->n_gemm;
   a.epi = p->epi; a.act = p->act;
   a.scale = p->scale; a.shift = p->shift;
@@ -467,19 +484,22 @@ int conv_fwd(const hrv_conv_params* p, const ConvBudget& budget, const char* nam
   }
 
   // ---- pipeline: as many stages as fit in the budget next to the scratch, at most one per K step; the ring also holds the
-  //      epilogue tile
-  const uint32_t stage_bytes = kConvABytes + (uint32_t)(budget.planes * bnt) * kConvRowBytes;
+  //      epilogue tile.  The halo main loop's stages hold B boxes only, behind the halo slots.
+  const uint32_t halo_bytes = a.halo ? (uint32_t)a.chunks * halo_slot : 0u;
+  const uint32_t stage_bytes = a.halo ? b_stage : kConvABytes + b_stage;
   const int KT = p->kh * p->kw * a.chunks;
-  int stages = (int)((budget.smem - 2048u - budget.scratch) / stage_bytes);
+  int stages = (int)((budget.smem - 2048u - budget.scratch - halo_bytes) / stage_bytes);
   if (stages > budget.max_stages) stages = budget.max_stages;
   if (stages > KT) stages = KT < 2 ? 2 : KT;
   a.stages = stages;
-  const size_t ring_stages = (size_t)stages * stage_bytes;
+  const size_t ring_stages = halo_bytes + (size_t)stages * stage_bytes;
   const size_t ring = ring_stages > conv_tile_bytes(bnt) ? ring_stages : conv_tile_bytes(bnt);
   const size_t smem = 2048 + budget.scratch + ring;  // 1 KB alignment slack + 1 KB of barriers
 
-  // ---- tensor maps: the input, and the packed weights [planes][taps][n_pad][cin_k] as laid out for this (bk, bn)
-  int rc = encode_nhwc_map(&a.tmA, in, budget.kblock, TW, TH, TN);
+  // ---- tensor maps: the input (the tile's box, or its halo), and the packed weights [planes][taps][n_pad][cin_k] as laid out for
+  //      this (bk, bn)
+  int rc = a.halo ? encode_nhwc_map(&a.tmA, in, budget.kblock, TW + p->kw - 1, TH + p->kh - 1, 1)
+                  : encode_nhwc_map(&a.tmA, in, budget.kblock, TW, TH, TN);
   if (rc) return rc;
   const cuuint64_t elem = sizeof(T);
   const cuuint64_t cin_k = (cuuint64_t)((in.c + p->bk - 1) / p->bk) * p->bk;

@@ -177,7 +177,10 @@ __device__ __forceinline__ float rna_tf32(float x) {
 
 // Shared-memory matrix descriptor of sm_90a: start>>4 at bits 0-13, LBO>>4 at 16-29, SBO>>4 at 32-45, layout type at bits 62-63
 // (1 = SW128, 2 = SW64, 3 = SW32).  K-major swizzled: SBO = stride of 8-row core-matrix groups, LBO unused (1).  MN-major swizzled:
-// LBO = stride of 64-element MN blocks, SBO = stride of 8-row K groups.  Operands start on 1024-byte boundaries (swizzle phase 0).
+// LBO = stride of 64-element MN blocks, SBO = stride of 8-row K groups.  The base-offset field (bits 49-51) stays 0: the hardware
+// applies the swizzle to absolute shared-memory address bits, as TMA does, so a K-major SW128 operand may also start any whole number
+// of 128-byte rows past a 1024-byte boundary (the halo main loop of conv_igemm.cu).  Measured on H100: every row phase 1-7 reads
+// the TMA layout correctly with base offset 0, and wrongly with base offset = (start >> 7) & 7.
 __device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type, uint32_t lbo_bytes = 16) {
   return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
          ((uint64_t)layout_type << 62);
