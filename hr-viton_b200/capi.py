@@ -30,7 +30,8 @@ POOL3X3_AVG_EXCL_PAD, POOL3X3_MAX = 0, 1
 # include/hrviton_sm100_data.h: uint8 in, fp32 out, one flavour (no _f16 twin)
 DATA_EXPORTS = ["hrv_pil_resample_pass", "hrv_pil_nearest", "hrv_agnostic_composite", "hrv_viton_assemble"]
 # include/hrviton_sm100_jpeg.h: uint8 in and out, one flavour (no _f16 twin)
-JPEG_EXPORTS = ["hrv_jpeg_huffman", "hrv_jpeg_idct", "hrv_jpeg_color"]
+JPEG_EXPORTS = ["hrv_jpeg_huffman", "hrv_jpeg_idct", "hrv_jpeg_color", "hrv_jpeg_encode_bounds", "hrv_jpeg_encode"]
+JPEG_SRC_U8_NHWC, JPEG_SRC_F32_NCHW = 0, 1
 
 
 class Tensor(ctypes.Structure):
@@ -163,6 +164,8 @@ def lib(dtype=None):
     L.hrv_jpeg_huffman.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     L.hrv_jpeg_idct.argtypes = [vp, i32, vp, vp, i32, vp]
     L.hrv_jpeg_color.argtypes = [vp, i32, vp, i32, vp]
+    L.hrv_jpeg_encode_bounds.argtypes = [i32, i32, i32, ctypes.POINTER(sz), ctypes.POINTER(sz)]
+    L.hrv_jpeg_encode.argtypes = [vp, i32, i32, i32, i32, vp, vp, sz, vp, sz, vp, vp]
     for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS + DATA_EXPORTS + JPEG_EXPORTS:
         fn = getattr(L, name)
         if "_workspace_bytes" in name:

@@ -636,6 +636,14 @@ class VitonHDLoader(BatchFeeder):
     def next_batch(self):
         return self._take()
 
+    def close(self):
+        """Stops the worker processes (they persist across epochs otherwise); the loader is not used after this."""
+        self._iter = None
+        it = getattr(self.loader, "_iterator", None)
+        if it is not None:
+            it._shutdown_workers()
+            self.loader._iterator = None
+
     def __iter__(self):
         if self.slots[self.slot] is None or self.host[self.slot] is None:
             self.prefetch()

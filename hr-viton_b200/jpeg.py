@@ -1,5 +1,10 @@
-"""Baseline JPEG decoding on the GPU, bit-identical to PIL (libjpeg-turbo's default decode: islow IDCT, fancy upsampling, separate
-upsample-then-convert colour path).
+"""Baseline JPEG decoding and encoding on the GPU, bit-identical to PIL (libjpeg-turbo's default decode: islow IDCT, fancy upsampling,
+separate upsample-then-convert colour path; its default encode: quality 75, 4:2:0, islow FDCT, standard Huffman tables).
+
+Encoding: encode() writes the bytes of Image.fromarray(rgb).save(f, format='JPEG') for a batch of same-size images whose width and
+height are multiples of 16, through the kernels of include/hrviton_sm100_jpeg.h; encode_np() is the same encoder in numpy, the CPU
+oracle the tests hold against PIL.  Both also take the generator's fp32 (N, 3, H, W) output in [-1, 1] and convert it as the
+reference's utils.save_images does.
 
 parse() reads a file's markers on the host into a Header: size, components and sampling, quantisation tables, Huffman tables as
 BITS/HUFFVAL, the restart interval, and the byte range of the entropy-coded segment with the offsets of its RSTn markers.
@@ -18,7 +23,7 @@ import torch
 
 from . import capi
 
-SOI, EOI, SOS, DQT, DHT, DRI = 0xD8, 0xD9, 0xDA, 0xDB, 0xC4, 0xDD
+SOI, EOI, SOS, DQT, DHT, DRI, APP0 = 0xD8, 0xD9, 0xDA, 0xDB, 0xC4, 0xDD, 0xE0
 SOF_HUFFMAN_SEQUENTIAL = (0xC0, 0xC1)
 SOF_ALL = (0xC0, 0xC1, 0xC2, 0xC3, 0xC5, 0xC6, 0xC7, 0xC9, 0xCA, 0xCB, 0xCD, 0xCE, 0xCF)
 
@@ -655,3 +660,334 @@ def decode(sources, device=None, rgb=False, out=None):
     errors = b.launch(device).cpu().numpy()
     raise_errors(errors, names)
     return out[0] if single else out
+
+
+# ------------------------------------------------------------------------------------------------ encoding: tables and headers
+# What PIL writes for Image.fromarray(rgb).save(f, format='JPEG'): libjpeg's defaults (jcparam.c jpeg_set_defaults) at quality 75,
+# 4:2:0, islow FDCT, the standard Huffman tables (not optimised), no restart interval, a JFIF 1.01 APP0.
+
+SOF0 = 0xC0
+QUALITY = 75
+
+# jcparam.c std_luminance_quant_tbl / std_chrominance_quant_tbl (ITU T.81 Annex K), natural order
+STD_QUANT = np.array([[16, 11, 10, 16, 24, 40, 51, 61, 12, 12, 14, 19, 26, 58, 60, 55, 14, 13, 16, 24, 40, 57, 69, 56, 14, 17, 22, 29, 51, 87, 80, 62,
+                       18, 22, 37, 56, 68, 109, 103, 77, 24, 35, 55, 64, 81, 104, 113, 92, 49, 64, 78, 87, 103, 121, 120, 101, 72, 92, 95, 98, 112,
+                       100, 103, 99],
+                      [17, 18, 24, 47, 99, 99, 99, 99, 18, 21, 26, 66, 99, 99, 99, 99, 24, 26, 56, 99, 99, 99, 99, 99, 47, 66, 99, 99, 99, 99, 99, 99]
+                      + [99] * 32], np.int64)
+
+# jstdhuff.c: BITS and HUFFVAL of the standard tables (ITU T.81 K.3), keyed as Header.huffman: (0 = DC / 1 = AC, table id)
+STD_HUFFMAN = {
+    (0, 0): (np.array([0, 1, 5, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0, 0, 0], np.uint8), np.arange(12, dtype=np.uint8)),
+    (1, 0): (np.array([0, 2, 1, 3, 3, 2, 4, 3, 5, 5, 4, 4, 0, 0, 1, 0x7D], np.uint8), np.frombuffer(bytes.fromhex(
+        "01020300041105122131410613516107227114328191a1082342b1c11552d1f02433627282090a161718191a25262728292a3435363738393a434445464748"
+        "494a535455565758595a636465666768696a737475767778797a838485868788898a92939495969798999aa2a3a4a5a6a7a8a9aab2b3b4b5b6b7b8b9bac2c3"
+        "c4c5c6c7c8c9cad2d3d4d5d6d7d8d9dae1e2e3e4e5e6e7e8e9eaf1f2f3f4f5f6f7f8f9fa"), np.uint8)),
+    (0, 1): (np.array([0, 3, 1, 1, 1, 1, 1, 1, 1, 1, 1, 0, 0, 0, 0, 0], np.uint8), np.arange(12, dtype=np.uint8)),
+    (1, 1): (np.array([0, 2, 1, 2, 4, 4, 3, 4, 7, 5, 4, 4, 0, 1, 2, 0x77], np.uint8), np.frombuffer(bytes.fromhex(
+        "000102031104052131061241510761711322328108144291a1b1c109233352f0156272d10a162434e125f11718191a262728292a35363738393a434445464748"
+        "494a535455565758595a636465666768696a737475767778797a82838485868788898a92939495969798999aa2a3a4a5a6a7a8a9aab2b3b4b5b6b7b8b9bac2c3"
+        "c4c5c6c7c8c9cad2d3d4d5d6d7d8d9dae2e3e4e5e6e7e8e9eaf2f3f4f5f6f7f8f9fa"), np.uint8)),
+}
+
+
+def quant_tables(quality=QUALITY):
+    """jcparam.c jpeg_set_quality: jpeg_quality_scaling, then jpeg_add_quant_table with force_baseline (entries clamped to 1..255).
+    int64 (2, 64), natural order: luminance, chrominance."""
+    scale = 5000 // quality if quality < 50 else 200 - 2 * quality
+    return np.clip((STD_QUANT * scale + 50) // 100, 1, 255)
+
+
+def huffman_codes(bits, vals):
+    """jchuff.c jpeg_make_c_derived_tbl: (code, length) of every symbol, int64 [256] each (length 0: the symbol has no code)."""
+    code_of, size_of = np.zeros(256, np.int64), np.zeros(256, np.int64)
+    code, p = 0, 0
+    for l in range(1, 17):
+        for _ in range(int(bits[l - 1])):
+            code_of[vals[p]], size_of[vals[p]] = code, l
+            code += 1
+            p += 1
+        code <<= 1
+    return code_of, size_of
+
+
+def reciprocals(q):
+    """jcdctmgr.c compute_reciprocal over each divisor qtbl << 3 (the islow FDCT's output is scaled by 8), with libjpeg-turbo's
+    16-bit DCTELEM: (reciprocal, correction, shift) int64 [64] each, natural order.  quantize() then computes
+    ((|x| + correction) * reciprocal) >> shift and restores the sign: division with rounding to nearest, half away from zero, as long
+    as the reciprocal is exact enough, which this restates rather than assumes."""
+    d = np.asarray(q, np.int64) << 3
+    recip, corr, shift = np.zeros(64, np.int64), np.zeros(64, np.int64), np.zeros(64, np.int64)
+    for i, div in enumerate(d.tolist()):
+        b = div.bit_length() - 1
+        r = 16 + b
+        fq, fr = (1 << r) // div, (1 << r) % div
+        c = div // 2
+        if fr == 0:  # a power of two: fq would be one bit too wide for 16 bits
+            fq >>= 1
+            r -= 1
+        elif fr <= div // 2:
+            c += 1
+        else:
+            fq += 1
+        recip[i], corr[i], shift[i] = fq, c, r
+    return recip, corr, shift
+
+
+def _marker(m, payload):
+    return bytes([0xFF, m, (len(payload) + 2) >> 8, (len(payload) + 2) & 0xFF]) + payload
+
+
+def encode_header(height, width):
+    """The bytes before the entropy-coded data: SOI, APP0 (JFIF 1.01, density 1x1, no units), DQT 0, DQT 1, SOF0 (3 components, Y 2x2,
+    Cb / Cr 1x1), DHT DC0 / AC0 / DC1 / AC1, SOS — the order Pillow (libjpeg-turbo) writes them in."""
+    q = quant_tables()
+    out = bytes([0xFF, SOI]) + _marker(APP0, b"JFIF\0" + bytes([1, 1, 0, 0, 1, 0, 1, 0, 0]))
+    for t in (0, 1):
+        out += _marker(DQT, bytes([t]) + q[t][ZIGZAG[:64]].astype(np.uint8).tobytes())
+    out += _marker(SOF0, bytes([8, height >> 8, height & 0xFF, width >> 8, width & 0xFF, 3, 1, 0x22, 0, 2, 0x11, 1, 3, 0x11, 1]))
+    for tc, th in ((0, 0), (1, 0), (0, 1), (1, 1)):
+        bits, vals = STD_HUFFMAN[(tc, th)]
+        out += _marker(DHT, bytes([(tc << 4) | th]) + bits.tobytes() + vals.tobytes())
+    return out + _marker(SOS, bytes([3, 1, 0x00, 2, 0x11, 3, 0x11, 0, 63, 0]))
+
+
+def check_encodable(images):
+    """(n, h, w) of an encode() / encode_np() batch: uint8 (N, H, W, 3) or fp32 (N, 3, H, W), H and W multiples of 16.  ValueError
+    otherwise."""
+    shape, dtype = tuple(images.shape), str(images.dtype).replace("torch.", "")
+    if dtype == "uint8" and len(shape) == 4 and shape[3] == 3:
+        n, h, w = shape[:3]
+    elif dtype == "float32" and len(shape) == 4 and shape[1] == 3:
+        n, _, h, w = shape
+    else:
+        raise ValueError("jpeg.encode: need uint8 (N, H, W, 3) RGB or float32 (N, 3, H, W) in [-1, 1], got %s %s" % (dtype, shape))
+    if n < 1 or h < 16 or w < 16 or h % 16 or w % 16 or h > 65535 or w > 65535:
+        raise ValueError("jpeg.encode: width and height must be multiples of 16 (whole 4:2:0 MCUs, no edge padding), got %dx%d" % (w, h))
+    return n, h, w
+
+
+# ------------------------------------------------------------------------------------------------ encoding: numpy oracle
+
+def save_images_u8_np(x):
+    """The reference's utils.save_images conversion of fp32 (N, 3, H, W) in [-1, 1]: ((x + 1) * 0.5 * 255), each step rounded to
+    fp32, clamped to [0, 255] and truncated to uint8, as (N, H, W, 3).  NaN becomes 0 (the device's fmaxf / fminf clamp)."""
+    x = np.asarray(x, np.float32)
+    t = (x + np.float32(1)) * np.float32(0.5) * np.float32(255)
+    t = np.where(np.isnan(t), np.float32(0), np.clip(t, np.float32(0), np.float32(255)))
+    return t.astype(np.uint8).transpose(0, 2, 3, 1)
+
+
+def rgb_to_ycc_np(rgb):
+    """jccolor.c rgb_ycc_convert: 16-bit fixed point, ONE_HALF rounding for Y and ONE_HALF - 1 for Cb / Cr.  int64 planes."""
+    r, g, b = (rgb[..., k].astype(np.int64) for k in range(3))
+    half, offset = 1 << 15, 128 << 16
+    y = (_fix16(0.29900) * r + _fix16(0.58700) * g + _fix16(0.11400) * b + half) >> 16
+    cb = (-_fix16(0.16874) * r - _fix16(0.33126) * g + _fix16(0.5) * b + offset + half - 1) >> 16
+    cr = (_fix16(0.5) * r - _fix16(0.41869) * g - _fix16(0.08131) * b + offset + half - 1) >> 16
+    return y, cb, cr
+
+
+def downsample_h2v2_np(p):
+    """jcsample.c h2v2_downsample: (a + b + c + d + bias) >> 2 with bias 1, 2, 1, 2, ... along each output row."""
+    s = p[..., 0::2, 0::2] + p[..., 0::2, 1::2] + p[..., 1::2, 0::2] + p[..., 1::2, 1::2]
+    return (s + 1 + (np.arange(s.shape[-1]) & 1)) >> 2
+
+
+def _fdct_pass(x, last):
+    """One pass of jfdctint.c jpeg_fdct_islow over the last axis of x (..., 8), int64: the rows pass (last=False) or the columns pass."""
+    t0, t7 = x[..., 0] + x[..., 7], x[..., 0] - x[..., 7]
+    t1, t6 = x[..., 1] + x[..., 6], x[..., 1] - x[..., 6]
+    t2, t5 = x[..., 2] + x[..., 5], x[..., 2] - x[..., 5]
+    t3, t4 = x[..., 3] + x[..., 4], x[..., 3] - x[..., 4]
+    t10, t13, t11, t12 = t0 + t3, t0 - t3, t1 + t2, t1 - t2
+    sh = CONST_BITS + PASS1_BITS if last else CONST_BITS - PASS1_BITS
+    ds = lambda v, n: (v + (1 << (n - 1))) >> n  # noqa: E731 - DESCALE
+    o = [None] * 8
+    o[0] = ds(t10 + t11, PASS1_BITS) if last else (t10 + t11) << PASS1_BITS
+    o[4] = ds(t10 - t11, PASS1_BITS) if last else (t10 - t11) << PASS1_BITS
+    z1 = (t12 + t13) * F_0_541
+    o[2] = ds(z1 + t13 * F_0_765, sh)
+    o[6] = ds(z1 - t12 * F_1_847, sh)
+    z1, z2, z3, z4 = t4 + t7, t5 + t6, t4 + t6, t5 + t7
+    z5 = (z3 + z4) * F_1_175
+    t4, t5, t6, t7 = t4 * F_0_298, t5 * F_2_053, t6 * F_3_072, t7 * F_1_501
+    z1, z2 = z1 * -F_0_899, z2 * -F_2_562
+    z3, z4 = z3 * -F_1_961 + z5, z4 * -F_0_390 + z5
+    o[7], o[5], o[3], o[1] = ds(t4 + z1 + z3, sh), ds(t5 + z2 + z4, sh), ds(t6 + z2 + z3, sh), ds(t7 + z1 + z4, sh)
+    return np.stack(o, -1)
+
+
+def fdct_islow_np(blocks):
+    """jpeg_fdct_islow of uint8 / int blocks (B, 8, 8), centred by 128 first: int64 (B, 64) in natural order, scaled by 8."""
+    x = blocks.astype(np.int64) - 128
+    ws = _fdct_pass(x, False)  # rows
+    return _fdct_pass(ws.transpose(0, 2, 1), True).transpose(0, 2, 1).reshape(-1, 64)
+
+
+def quantize_np(coefs, q):
+    """jcdctmgr.c quantize() of natural-order coefficients (B, 64) with quantisation table q (64, natural order)."""
+    recip, corr, shift = reciprocals(q)
+    a = np.abs(coefs)
+    v = ((a + corr) * recip) >> shift
+    return np.where(coefs < 0, -v, v)
+
+
+def coefficients_np(rgb):
+    """Quantised coefficients of one (H, W, 3) uint8 image: int64 (blocks, 64) in zig-zag order, blocks in scan order (Y00 Y01 Y10 Y11
+    Cb Cr per MCU), and the component (0 Y, 1 Cb, 2 Cr) of each block."""
+    h, w = rgb.shape[:2]
+    y, cb, cr = rgb_to_ycc_np(rgb)
+    cb, cr = downsample_h2v2_np(cb), downsample_h2v2_np(cr)
+    q = quant_tables()
+    my, mx = h // 16, w // 16
+    # Y blocks (my, 2, mx, 2, 8, 8) -> (my, mx, 2, 2, 8, 8): MCU by MCU, then the 2x2 blocks row by row
+    yb = y.reshape(my, 2, 8, mx, 2, 8).transpose(0, 3, 1, 4, 2, 5).reshape(my * mx, 4, 8, 8)
+    cbb = cb.reshape(my, 8, mx, 8).transpose(0, 2, 1, 3).reshape(my * mx, 1, 8, 8)
+    crb = cr.reshape(my, 8, mx, 8).transpose(0, 2, 1, 3).reshape(my * mx, 1, 8, 8)
+    blocks = np.concatenate([yb, cbb, crb], 1).reshape(-1, 8, 8)
+    comp = np.tile(np.array([0, 0, 0, 0, 1, 2]), my * mx)
+    coef = fdct_islow_np(blocks)
+    coef = np.where((comp == 0)[:, None], quantize_np(coef, q[0]), quantize_np(coef, q[1]))
+    return coef[:, ZIGZAG[:64]], comp
+
+
+_NBITS = np.array([int(v).bit_length() for v in range(1 << 16)], np.int64)
+
+
+def huffman_np(zz, comp):
+    """jchuff.c encode_one_block over every block (zz (B, 64) zig-zag coefficients in scan order, comp (B,) component), as libjpeg emits
+    it: DC difference from the previous block of the same component (category code, then its bits), AC runs with ZRL (0xF0) for runs
+    past 15, EOB when zeros trail; the bits MSB first, the last partial byte padded with 1-bits, 0x00 stuffed after every 0xFF.
+    Vectorised: every code of the scan is one event (value, length), written out as a bit array."""
+    codes = {k: huffman_codes(*v) for k, v in STD_HUFFMAN.items()}
+    tbl = (comp > 0).astype(np.int64)
+    zz = zz.astype(np.int64)
+    dc = zz[:, 0]
+    diff = np.zeros_like(dc)
+    for c in range(3):
+        sel = np.flatnonzero(comp == c)
+        diff[sel] = np.diff(dc[sel], prepend=0)
+    mask = np.zeros((len(zz), 65), bool)
+    mask[:, 0] = True
+    mask[:, 1:64] = zz[:, 1:] != 0
+    mask[:, 64] = zz[:, 63] == 0
+    rows, cols = np.nonzero(mask)
+    t = tbl[rows]
+    v = np.where(cols == 0, diff[rows], zz[rows, np.minimum(cols, 63)])
+    nb = _NBITS[np.abs(v)]
+    extra = np.where(v < 0, v - 1, v) & ((1 << nb) - 1)
+    run = np.zeros_like(cols)
+    run[1:] = cols[1:] - cols[:-1] - 1
+    is_dc, is_eob = cols == 0, cols == 64
+    is_ac = ~is_dc & ~is_eob
+    sym = np.where(is_ac, ((run & 15) << 4) | nb, np.where(is_dc, nb, 0))
+    dco = np.where(t == 0, codes[(0, 0)][0][sym], codes[(0, 1)][0][sym])
+    dsi = np.where(t == 0, codes[(0, 0)][1][sym], codes[(0, 1)][1][sym])
+    aco = np.where(t == 0, codes[(1, 0)][0][sym], codes[(1, 1)][0][sym])
+    asi = np.where(t == 0, codes[(1, 0)][1][sym], codes[(1, 1)][1][sym])
+    co, si = np.where(is_dc, dco, aco), np.where(is_dc, dsi, asi)
+    val, length = np.zeros_like(co), np.zeros_like(co)
+    zrl = np.where(is_ac, run >> 4, 0)
+    zco = np.where(t == 0, codes[(1, 0)][0][0xF0], codes[(1, 1)][0][0xF0])
+    zsi = np.where(t == 0, codes[(1, 0)][1][0xF0], codes[(1, 1)][1][0xF0])
+    for j in range(3):  # a run of up to 62 zeros: at most 3 ZRLs
+        z = zrl > j
+        val, length = np.where(z, (val << zsi) | zco, val), np.where(z, length + zsi, length)
+    val, length = (val << si) | co, length + si
+    nb = np.where(is_eob, 0, nb)
+    val, length = (val << nb) | extra * (~is_eob), length + nb
+    total = int(length.sum())
+    starts = np.cumsum(length) - length
+    idx = np.repeat(np.arange(len(length)), length)
+    j = np.arange(total) - starts[idx]
+    bits = ((val[idx] >> (length[idx] - 1 - j)) & 1).astype(np.uint8)
+    bits = np.concatenate([bits, np.ones((-total) % 8, np.uint8)])
+    packed = np.packbits(bits)
+    return np.insert(packed, np.flatnonzero(packed == 0xFF) + 1, 0)
+
+
+def encode_np(images):
+    """numpy statement of the device encoder: the JPEG file bytes of every image of a uint8 (N, H, W, 3) RGB batch (or an (H, W, 3)
+    image), or of an fp32 (N, 3, H, W) generator output in [-1, 1] converted as utils.save_images does.  A list of bytes, equal to
+    Image.fromarray(rgb).save(f, format='JPEG').  H and W must be multiples of 16."""
+    images = np.asarray(images)
+    if images.dtype == np.uint8 and images.ndim == 3:
+        images = images[None]
+    n, h, w = check_encodable(images)
+    if images.dtype == np.float32:
+        images = save_images_u8_np(images)
+    head = encode_header(h, w)
+    out = []
+    for rgb in images:
+        zz, comp = coefficients_np(rgb)
+        out.append(head + huffman_np(zz, comp).tobytes() + bytes([0xFF, EOI]))
+    return out
+
+
+# ------------------------------------------------------------------------------------------------ encoding: device
+
+class EncTables(ctypes.Structure):
+    """include/hrviton_sm100_jpeg.h's hrv_jpeg_enc_tables."""
+    _fields_ = [("quant", (ctypes.c_uint16 * 64) * 2), ("code", (ctypes.c_uint16 * 256) * 4), ("size", (ctypes.c_uint8 * 256) * 4)]
+
+
+_enc_tables = {}  # device -> the EncTables of encode_header's tables, uploaded once
+
+
+def _device_tables(device):
+    t = _enc_tables.get(device)
+    if t is None:
+        e = EncTables()
+        for k, q in enumerate(quant_tables()):
+            ctypes.memmove(e.quant[k], q.astype(np.uint16).ctypes.data, 128)
+        for k, key in enumerate(((0, 0), (1, 0), (0, 1), (1, 1))):  # DC0, AC0, DC1, AC1
+            code, size = huffman_codes(*STD_HUFFMAN[key])
+            ctypes.memmove(e.code[k], code.astype(np.uint16).ctypes.data, 512)
+            ctypes.memmove(e.size[k], size.astype(np.uint8).ctypes.data, 256)
+        t = _enc_tables[device] = torch.frombuffer(bytearray(bytes(e)), dtype=torch.uint8).to(device)
+    return t
+
+
+def encode(images, stream=None, stats=None):
+    """JPEG files of a batch on the GPU, byte-identical to PIL's Image.fromarray(rgb).save(f, format='JPEG'): a list of bytes.
+    images: a CUDA uint8 (N, H, W, 3) RGB batch, or the generator's fp32 (N, 3, H, W) output in [-1, 1], which is converted as the
+    reference's utils.save_images does (see save_images_u8_np).  H and W must be multiples of 16 (ValueError otherwise).
+
+    Runs on `stream` (default: the current stream), ordered after the work that wrote `images`.  The device sends back only the
+    entropy-coded bytes: one small copy of the per-image lengths (the one wait for the device), then one copy of the bytes; the host
+    prepends the fixed header.  stats: a dict that receives 'd2h_bytes', the bytes copied from the device."""
+    n, h, w = check_encodable(images)
+    if not (torch.is_tensor(images) and images.is_cuda):
+        raise ValueError("jpeg.encode: need a CUDA tensor (encode_np encodes host arrays)")
+    device = images.device
+    kind = capi.JPEG_SRC_U8_NHWC if images.dtype == torch.uint8 else capi.JPEG_SRC_F32_NCHW
+    L = capi.lib()
+    ws_bytes, out_bytes = ctypes.c_size_t(), ctypes.c_size_t()
+    capi.check(L.hrv_jpeg_encode_bounds(n, h, w, ctypes.byref(ws_bytes), ctypes.byref(out_bytes)), "jpeg_encode_bounds")
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream(device) if stream is None else stream
+        with torch.cuda.stream(stream):
+            images = images.contiguous()
+            tables = _device_tables(device)
+            ws = torch.empty(ws_bytes.value, dtype=torch.uint8, device=device)
+            out = torch.empty(out_bytes.value, dtype=torch.uint8, device=device)
+            sizes = torch.empty(2 * n, dtype=torch.int64, device=device)
+            capi.check(L.hrv_jpeg_encode(images.data_ptr(), kind, n, h, w, tables.data_ptr(), ws.data_ptr(), ws_bytes.value, out.data_ptr(),
+                                         out_bytes.value, sizes.data_ptr(), stream.cuda_stream), "jpeg_encode")
+            host_sizes = torch.empty(2 * n, dtype=torch.int64, pin_memory=True)
+            host_sizes.copy_(sizes, non_blocking=True)
+            done = torch.cuda.Event()
+            done.record(stream)
+            done.synchronize()
+            lengths, offsets = host_sizes[0::2].tolist(), host_sizes[1::2].tolist()
+            total = offsets[-1] + lengths[-1]
+            host = torch.empty(total, dtype=torch.uint8, pin_memory=True)
+            host.copy_(out[:total], non_blocking=True)
+            done.record(stream)
+            done.synchronize()
+    if stats is not None:
+        stats["d2h_bytes"] = stats.get("d2h_bytes", 0) + total + 16 * n
+    head = encode_header(h, w)
+    mv = memoryview(host.numpy())
+    return [head + mv[o:o + l].tobytes() for o, l in zip(offsets, lengths)]

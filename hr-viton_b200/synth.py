@@ -220,3 +220,29 @@ def jpeg_corpus(seed=0):
             out.append(("%dx%d_L_q%d" % (w, h, q), save(content(w, h, 1, q == 75), quality=q)))
         out.append(("%dx%d_L_rst" % (w, h), save(content(w, h, 1, False), quality=90, restart_marker_blocks=1)))
     return out
+
+
+def encode_corpus(seed=0, sizes=((16, 16), (32, 48), (80, 64), (256, 192), (512, 384), (1024, 768))):
+    """Seeded RGB images for the JPEG encoder, as {(h, w): [(name, uint8 (h, w, 3))]}: per size uniform noise (many 0xFF bytes to
+    stuff, large AC categories), a smooth gradient, a flat colour (EOB and ZRL) and saturated 0 / 255 primaries in 8x8 cells, plus at
+    256x192 and up the image of a write_vitonhd tree resized to that size (a try-on-like picture)."""
+    import os
+    import tempfile
+
+    from PIL import Image
+    g = _rng(seed, "jpeg_encode")
+    out = {}
+    with tempfile.TemporaryDirectory() as d:
+        write_vitonhd(d, 1, seed=seed)
+        person = Image.open(os.path.join(d, "train", "image", "000000_00.jpg")).convert("RGB")
+        for h, w in sizes:
+            items = [("noise", g.integers(0, 256, (h, w, 3), dtype=np.uint8))]
+            t = g.integers(0, 256, (max(2, h // 64), max(2, w // 64), 3), dtype=np.uint8)
+            items.append(("smooth", np.asarray(Image.fromarray(t).resize((w, h), Image.BILINEAR))))
+            items.append(("flat", np.broadcast_to(g.integers(0, 256, 3).astype(np.uint8), (h, w, 3)).copy()))
+            cells = (g.integers(0, 2, (h // 8, w // 8, 3)) * 255).astype(np.uint8)
+            items.append(("primaries", cells.repeat(8, 0).repeat(8, 1)))
+            if h >= 256:
+                items.append(("person", np.asarray(person.resize((w, h), Image.BILINEAR))))
+            out[(h, w)] = items
+    return out

@@ -59,6 +59,45 @@ int hrv_jpeg_idct(const hrv_jpeg_image* images, int32_t n, const int16_t* coefs,
  * image and written to each image's dst.  max_pixels: the largest height * width of the batch. */
 int hrv_jpeg_color(const hrv_jpeg_image* images, int32_t n, const uint8_t* planes, int32_t max_pixels, hrv_stream stream);
 
+/* ---------------------------------------------------------------------------------------------------------------- encoding
+ * What PIL writes for Image.fromarray(rgb).save(f, format='JPEG'): quality 75, 4:2:0 (Y 2x2, Cb / Cr 1x1), libjpeg-turbo's colour
+ * conversion, h2v2 downsampling, islow FDCT and quantisation, the standard Huffman tables, no restart interval.  The images of a batch
+ * have one size, with height and width multiples of 16 (whole MCUs: no edge padding).  The device writes the entropy-coded data of
+ * each image, 0x00-stuffed and followed by EOI; the host prepends the header (SOI .. SOS), which is fixed for a size
+ * (hrviton_b200.jpeg.encode_header). */
+
+/* Source layouts of hrv_jpeg_encode. */
+enum hrv_jpeg_src { HRV_JPEG_SRC_U8_NHWC = 0, HRV_JPEG_SRC_F32_NCHW = 1 };
+
+/* The tables the device encodes with, built on the host from the ones the header carries. */
+typedef struct hrv_jpeg_enc_tables {
+  uint16_t quant[2][64];  /* quantisation tables, natural order: luminance, chrominance */
+  uint16_t code[4][256];  /* Huffman code of each symbol: DC luminance, AC luminance, DC chrominance, AC chrominance */
+  uint8_t size[4][256];   /* its length in bits (0: no code) */
+} hrv_jpeg_enc_tables;
+
+/* Device memory hrv_jpeg_encode needs for n images of height x width: the workspace, and `out`.  Both are worst cases computed from
+ * the shape.  A block codes to at most 1665 bits: a DC code of up to 16 bits with up to 11 magnitude bits, and for each of the 63 AC
+ * coefficients at most one code of up to 16 bits with up to 10 magnitude bits.  A ZRL or an EOB stands in for at least one zero
+ * coefficient, which codes nothing itself, so it fits inside that bound.  Per image, out_bytes holds 2 * ceil(blocks * 1665 / 8)
+ * + 2 bytes: every byte stuffed, plus EOI.  Blocks = height * width / 256 * 6. */
+int hrv_jpeg_encode_bounds(int32_t n, int32_t height, int32_t width, size_t* workspace_bytes, size_t* out_bytes);
+
+/* Encodes n images.  src: uint8 (n, height, width, 3) RGB (HRV_JPEG_SRC_U8_NHWC), or fp32 (n, 3, height, width) in [-1, 1]
+ * (HRV_JPEG_SRC_F32_NCHW) converted as the reference's utils.save_images does: (x + 1) * 0.5 * 255 with each operation rounded
+ * (no FMA), clamped to [0, 255] by fmaxf / fminf (NaN becomes 0), truncated.  Launches, in order:
+ *   colour + FDCT + quantisation   64 threads per MCU: int16 coefficients, zig-zag order, blocks in scan order (Y00 Y01 Y10 Y11 Cb Cr)
+ *   length pass                    one thread per block: its bit count, DC predicted from the previous block of its component
+ *   scan                           one CTA per image: bit offset of every block
+ *   write pass                     one thread per block: its codes at its offset (integer atomicOr on the words it shares)
+ *   0xFF count, scan               4096-byte chunks: stuffed length of each image
+ *   sizes                          sizes[2 i] = byte length of image i's data after the header (EOI included), sizes[2 i + 1] =
+ *                                  its offset in `out`; images are back to back from offset 0
+ *   stuffing                       every byte at its stuffed position, 0x00 after each 0xFF, EOI
+ * The caller copies `sizes` (int64 [2 n], device) to the host, then the sum of the lengths from `out`. */
+int hrv_jpeg_encode(const void* src, int32_t src_kind, int32_t n, int32_t height, int32_t width, const hrv_jpeg_enc_tables* tables,
+                    void* workspace, size_t workspace_bytes, uint8_t* out, size_t out_bytes, int64_t* sizes, hrv_stream stream);
+
 #ifdef __cplusplus
 }
 #endif
