@@ -53,6 +53,21 @@ __device__ __forceinline__ void st8(float* p, const float (&f)[8]) {
   reinterpret_cast<float4*>(p)[0] = make_float4(f[0], f[1], f[2], f[3]);
   reinterpret_cast<float4*>(p)[1] = make_float4(f[4], f[5], f[6], f[7]);
 }
+// The first k < 8 elements of a group (a view's last channels), the rest zero: nothing past the view is read.
+__device__ __forceinline__ Vec8<__nv_bfloat16> ldv8_head(const __nv_bfloat16* p, int k) {
+  const unsigned short* q = reinterpret_cast<const unsigned short*>(p);
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    w[i] = (2 * i < k ? (uint32_t)__ldg(q + 2 * i) : 0u) | ((2 * i + 1 < k ? (uint32_t)__ldg(q + 2 * i + 1) : 0u) << 16);
+  return Vec8<__nv_bfloat16>{make_uint4(w[0], w[1], w[2], w[3])};
+}
+__device__ __forceinline__ Vec8<float> ldv8_head(const float* p, int k) {
+  float f[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) f[i] = i < k ? __ldg(p + i) : 0.f;
+  return Vec8<float>{make_float4(f[0], f[1], f[2], f[3]), make_float4(f[4], f[5], f[6], f[7])};
+}
 template <typename T> __device__ __forceinline__ Vec8<T> zero8();
 template <> __device__ __forceinline__ Vec8<__nv_bfloat16> zero8<__nv_bfloat16>() { return Vec8<__nv_bfloat16>{make_uint4(0, 0, 0, 0)}; }
 template <> __device__ __forceinline__ Vec8<float> zero8<float>() { return Vec8<float>{make_float4(0.f, 0.f, 0.f, 0.f), make_float4(0.f, 0.f, 0.f, 0.f)}; }
@@ -417,8 +432,11 @@ __global__ void space_to_depth_kernel(View src, View dst, int G, int Gd, long lo
   const int sub = gd / G, g = gd % G;
   if (sub < 4) {
     const int sy = 2 * Y + (sub >> 1), sx = 2 * X + (sub & 1);
-    if (sy < src.h && sx < src.w)
-      v = ldv8(reinterpret_cast<const T*>(src.ptr) + (((long long)n * src.h + sy) * src.w + sx) * src.pitch + g * 8);
+    if (sy < src.h && sx < src.w) {
+      const T* p = reinterpret_cast<const T*>(src.ptr) + (((long long)n * src.h + sy) * src.w + sx) * src.pitch + g * 8;
+      // a partial last group copies the view's channels only: [c, c8) of each sub-image is zero, whatever lies past the view
+      v = g * 8 + 8 <= src.c ? ldv8(p) : ldv8_head(p, src.c - g * 8);
+    }
   }
   stv8(reinterpret_cast<T*>(const_cast<void*>(dst.ptr)) + pix * dst.pitch + gd * 8, v);
 }

@@ -208,8 +208,8 @@ int hrv_seg_softmax_cat(const float* input1, int32_t c1, const float* input2, in
 /* bf16|f32 NHWC view -> fp32 NCHW contiguous [n][c][h][w]. */
 int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream);
 
-/* Space-to-depth by 2 with zero fill of odd edges: dst[n,Y,X,(py*2+px)*src.c + ci] = src[n,2Y+py,2X+px,ci];
- * dst.h = ceil(src.h/2), dst.w = ceil(src.w/2), dst.c >= 4*src.c (extra channels zeroed). Turns the
+/* Space-to-depth by 2 with zero fill of odd edges: dst[n,Y,X,(py*2+px)*C8 + ci] = src[n,2Y+py,2X+px,ci], C8 = 8*ceil(src.c/8);
+ * dst.h = ceil(src.h/2), dst.w = ceil(src.w/2), dst.c >= 4*C8 (every other channel zeroed; nothing past the view is read). Turns the
  * stride-2 convolutions (networks.py:185; network_generator.py:263-269; networks.py:360-372) into stride-1
  * 2x2 implicit GEMMs.  fp32 storage: src and dst fp32. */
 int hrv_space_to_depth(const hrv_tensor* src, const hrv_tensor* dst, hrv_stream stream);
