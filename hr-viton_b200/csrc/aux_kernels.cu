@@ -356,9 +356,29 @@ struct SegCatSrc {
   const float* cm;
   int c1, c2, K, cm_channel, mode, softmax;
 };
-__device__ __forceinline__ float seg_cat_score(const SegCatSrc& S, const float* seg_px, long long hw, int k, float m) {
+// The per-pixel decisions that seg_softmax_cat_kernel and seg_iou_kernel share, so that both compose and soft-max alike.
+// seg_cm_factor: the composition factor of the pixel (mode 0: 1, mode 1: cm, mode 2: cm > 0.5).  seg_score: the composed score of
+// channel k (seg_px points at channel 0 of the pixel, planes hw apart; cm_channel < 0: none is composed).  SegSoftmax: the channel
+// maximum and the sum of expf(score - maximum) in channel order, so that p_k = seg_prob(score_k) = expf(score_k - mx) / sum.
+__device__ __forceinline__ float seg_cm_factor(const float* cm, long long pix, int mode) {
+  if (mode == 0) return 1.f;
+  const float m = __ldg(cm + pix);
+  return mode == 2 ? (m > 0.5f ? 1.f : 0.f) : m;
+}
+__device__ __forceinline__ float seg_score(const float* seg_px, long long hw, int k, int cm_channel, float m) {
   const float s = __ldg(seg_px + (long long)k * hw);
-  return k == S.cm_channel ? __fmul_rn(s, m) : s;
+  return k == cm_channel ? __fmul_rn(s, m) : s;
+}
+struct SegSoftmax {
+  float mx, sum;
+  __device__ __forceinline__ SegSoftmax(const float* seg_px, long long hw, int K, int cm_channel, float m) : mx(-INFINITY), sum(0.f) {
+    for (int k = 0; k < K; ++k) mx = fmaxf(mx, seg_score(seg_px, hw, k, cm_channel, m));
+    for (int k = 0; k < K; ++k) sum += expf(seg_score(seg_px, hw, k, cm_channel, m) - mx);
+  }
+  __device__ __forceinline__ float prob(float s) const { return __fdiv_rn(expf(s - mx), sum); }
+};
+__device__ __forceinline__ float seg_cat_score(const SegCatSrc& S, const float* seg_px, long long hw, int k, float m) {
+  return seg_score(seg_px, hw, k, S.cm_channel, m);
 }
 template <typename T>
 __global__ void seg_softmax_cat_kernel(SegCatSrc S, View dst, float* __restrict__ seg_out, int G, long long npix) {
@@ -367,16 +387,8 @@ __global__ void seg_softmax_cat_kernel(SegCatSrc S, View dst, float* __restrict_
   const long long hw = (long long)dst.h * dst.w;
   const long long n = pix / hw, rem = pix - n * hw;
   const float* seg_px = S.seg + n * S.K * hw + rem;
-  float m = 1.f;
-  if (S.mode != 0) {
-    m = __ldg(S.cm + pix);
-    if (S.mode == 2) m = m > 0.5f ? 1.f : 0.f;
-  }
-  float mx = -INFINITY, sum = 0.f;
-  if (S.softmax) {
-    for (int k = 0; k < S.K; ++k) mx = fmaxf(mx, seg_cat_score(S, seg_px, hw, k, m));
-    for (int k = 0; k < S.K; ++k) sum += expf(seg_cat_score(S, seg_px, hw, k, m) - mx);
-  }
+  const float m = seg_cm_factor(S.cm, pix, S.mode);
+  SegSoftmax sm = S.softmax ? SegSoftmax(seg_px, hw, S.K, S.cm_channel, m) : SegSoftmax(seg_px, hw, 0, S.cm_channel, m);
   if (seg_out)
     for (int k = 0; k < S.K; ++k) seg_out[n * S.K * hw + (long long)k * hw + rem] = seg_cat_score(S, seg_px, hw, k, m);
   const int c12 = S.c1 + S.c2;
@@ -392,13 +404,69 @@ __global__ void seg_softmax_cat_kernel(SegCatSrc S, View dst, float* __restrict_
         f[i] = __ldg(S.in2 + (n * S.c2 + (c - S.c1)) * hw + rem);
       } else if (c < c12 + S.K) {
         const float s = seg_cat_score(S, seg_px, hw, c - c12, m);
-        f[i] = S.softmax ? __fdiv_rn(expf(s - mx), sum) : s;
+        f[i] = S.softmax ? sm.prob(s) : s;
       } else {
         f[i] = 0.f;
       }
     }
     st8(out + g * 8, f);
   }
+}
+
+// The stage-1 validation IoU (train_condition.py:18-36 on F.softmax(fake_segmap * cloth_mask, 1), :314-356).  grid (blocks, N),
+// thread = pixels of one sample, strided: the pixel's scores composed ('warp_grad': channel SEG_IOU_CM_CHANNEL times cm) and
+// soft-maxed by the functions seg_softmax_cat_kernel uses, then per channel pred = p > 0.5, lab = (parse == 1).  Each warp adds its
+// counts with integer reductions and writes (P, L, I) to its own slot of `partial`; no shared memory, no atomics.
+constexpr int SEG_IOU_THREADS = 256, SEG_IOU_WARPS = SEG_IOU_THREADS / 32, SEG_IOU_MAX_BLOCKS = 64, SEG_IOU_CM_CHANNEL = 3;
+__global__ void __launch_bounds__(SEG_IOU_THREADS) seg_iou_count_kernel(const float* __restrict__ seg, const float* __restrict__ cm,
+                                                                        const float* __restrict__ parse, int K, long long hw,
+                                                                        int4* __restrict__ partial) {
+  const int n = blockIdx.y;
+  const float* seg_n = seg + (long long)n * K * hw;
+  const float* lab_n = parse + (long long)n * K * hw;
+  int P = 0, L = 0, I = 0;
+  for (long long rem = (long long)blockIdx.x * blockDim.x + threadIdx.x; rem < hw; rem += (long long)gridDim.x * blockDim.x) {
+    const float m = seg_cm_factor(cm, (long long)n * hw + rem, 1);
+    const SegSoftmax sm(seg_n + rem, hw, K, SEG_IOU_CM_CHANNEL, m);
+    for (int k = 0; k < K; ++k) {
+      const int pred = sm.prob(seg_score(seg_n + rem, hw, k, SEG_IOU_CM_CHANNEL, m)) > 0.5f;
+      const int lab = __ldg(lab_n + (long long)k * hw + rem) == 1.f;
+      P += pred;
+      L += lab;
+      I += pred & lab;
+    }
+  }
+  P = __reduce_add_sync(0xffffffffu, P);
+  L = __reduce_add_sync(0xffffffffu, L);
+  I = __reduce_add_sync(0xffffffffu, I);
+  if ((threadIdx.x & 31) == 0)
+    partial[((long long)n * gridDim.x + blockIdx.x) * SEG_IOU_WARPS + (threadIdx.x >> 5)] = make_int4(P, L, I, 0);
+}
+
+// One warp: per sample (in order) the counts of its `parts` slots, then the reference's fp32 arithmetic.  iou_metric computes
+// intersection = sum(y_pred[y_true == 1]) (int64 I), union = sum(y_pred) + sum(y_true) (int64 P promoted to fp32, plus the fp32 sum
+// of the 0/1 labels, exactly L below 2^24), and iou += (intersection + 1e-7) / (union - intersection + 1e-7) / B from iou = 0, each
+// operation rounded to fp32.  Restated:  iou = sum over n in order of ((f32(I) + 1e-7f) / ((f32(P) + f32(L)) - f32(I) + 1e-7f)) / f32(B).
+__global__ void seg_iou_finish_kernel(const int4* __restrict__ partial, int parts, int N, float* __restrict__ iou) {
+  const int lane = threadIdx.x;
+  float acc = 0.f;
+  for (int n = 0; n < N; ++n) {
+    int P = 0, L = 0, I = 0;
+    for (int i = lane; i < parts; i += 32) {
+      const int4 v = partial[(long long)n * parts + i];
+      P += v.x;
+      L += v.y;
+      I += v.z;
+    }
+    P = __reduce_add_sync(0xffffffffu, P);
+    L = __reduce_add_sync(0xffffffffu, L);
+    I = __reduce_add_sync(0xffffffffu, I);
+    const float fi = __int2float_rn(I);
+    const float uni = __fadd_rn(__int2float_rn(P), __int2float_rn(L));
+    const float t = __fdiv_rn(__fdiv_rn(__fadd_rn(fi, 1e-7f), __fadd_rn(__fsub_rn(uni, fi), 1e-7f)), __int2float_rn(N));
+    acc = __fadd_rn(acc, t);
+  }
+  if (lane == 0) *iou = acc;
 }
 
 // thread = (pixel); loops channels; writes are coalesced per plane.
@@ -824,6 +892,35 @@ extern "C" int hrv_seg_softmax_cat(const float* input1, int32_t c1, const float*
   const long long npix = (long long)dst->n * dst->h * dst->w;
   HRV_LAUNCH_STORAGE(dt, seg_softmax_cat_kernel, blocks_for(npix, 128), 128, 0, (cudaStream_t)stream, S, mk(dst), seg_out, G, npix);
   return launch_ok("seg_softmax_cat");
+}
+
+static int seg_iou_blocks(long long hw) {
+  const long long b = (hw + SEG_IOU_THREADS - 1) / SEG_IOU_THREADS;
+  return b < SEG_IOU_MAX_BLOCKS ? (int)b : SEG_IOU_MAX_BLOCKS;
+}
+
+extern "C" size_t hrv_seg_iou_workspace_bytes(int32_t n, int32_t h, int32_t w) {
+  if (n < 1 || h < 1 || w < 1) return 0;
+  return (size_t)n * seg_iou_blocks((long long)h * w) * SEG_IOU_WARPS * sizeof(int4);
+}
+
+extern "C" int hrv_seg_iou(const float* seg, int32_t k, const float* cm, const float* parse, int32_t n, int32_t h, int32_t w, float* iou,
+                           void* workspace, size_t workspace_bytes, hrv_stream stream) {
+  if (!seg || !cm || !parse || !iou) return set_error(HRV_EINVAL, "seg_iou: null argument");
+  if (n < 1 || h < 1 || w < 1 || k <= SEG_IOU_CM_CHANNEL)
+    return set_error(HRV_EINVAL, "seg_iou: need n, h, w >= 1 and k > %d (the composed cloth channel), got n=%d h=%d w=%d k=%d",
+                     SEG_IOU_CM_CHANNEL, n, h, w, k);
+  const long long hw = (long long)h * w;
+  if ((long long)k * hw > 0x7fffffffLL) return set_error(HRV_EINVAL, "seg_iou: %d x %lld labels per sample overflow the int32 counts", k, hw);
+  const size_t need = hrv_seg_iou_workspace_bytes(n, h, w);
+  if (!workspace || workspace_bytes < need) return set_error(HRV_EINVAL, "seg_iou: workspace too small (%zu < %zu)", workspace_bytes, need);
+  const int blocks = seg_iou_blocks(hw);
+  cudaStream_t st = (cudaStream_t)stream;
+  seg_iou_count_kernel<<<dim3(blocks, n), SEG_IOU_THREADS, 0, st>>>(seg, cm, parse, k, hw, (int4*)workspace);
+  int rc = launch_ok("seg_iou");
+  if (rc) return rc;
+  seg_iou_finish_kernel<<<1, 32, 0, st>>>((const int4*)workspace, blocks * SEG_IOU_WARPS, n, iou);
+  return launch_ok("seg_iou finish");
 }
 
 extern "C" int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream) {

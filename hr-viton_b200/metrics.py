@@ -229,6 +229,36 @@ def ssim(im1, im2, data_range=255):
     return out.cpu().numpy() if as_numpy else out
 
 
+SEG_CHANNELS = 13  # the condition generator's segmentation classes (train_condition.py's --semantic_nc / output_nc)
+
+
+def segmentation_iou(fake_segmap, warped_cm, parse, composition="warp_grad"):
+    """The IoU train_condition.py validates stage 1 with (:18-36, :346-356): iou_metric(F.softmax(fake_segmap * cloth_mask, 1), parse),
+    cloth_mask = ones with channel 3 = warped_cm.  fake_segmap: the tocg's (N,13,H,W) scores; warped_cm: its warped cloth mask
+    (N,1,H,W); parse: the one-hot (N,13,H,W) label, values in {0, 1}; all fp32 cuda.  Returns a 0-dim fp32 cuda tensor equal to
+    iou_metric's value bit for bit (the mean over the batch of each sample's IoU over all 13 channels), without synchronising.
+    Only composition 'warp_grad' (the one stage-1 training uses) is computed."""
+    if composition != "warp_grad":
+        raise ValueError("segmentation_iou computes composition 'warp_grad' only (the one stage-1 training uses), got %r" % (composition,))
+    ts = {"fake_segmap": fake_segmap, "warped_cm": warped_cm, "parse": parse}
+    for name, t in ts.items():
+        if not torch.is_tensor(t):
+            raise TypeError("segmentation_iou: %s must be a tensor, got %s" % (name, type(t).__name__))
+        if not t.is_cuda:
+            raise RuntimeError("segmentation_iou runs on the GPU only (no CPU fallback): %s is on %s" % (name, t.device))
+        if t.dtype != torch.float32 or t.dim() != 4:
+            raise ValueError("segmentation_iou: %s must be a float32 (N,C,H,W) tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
+    n, c, h, w = fake_segmap.shape
+    want = {"fake_segmap": (n, SEG_CHANNELS, h, w), "warped_cm": (n, 1, h, w), "parse": (n, SEG_CHANNELS, h, w)}
+    if any(tuple(ts[k].shape) != v for k, v in want.items()) or n < 1 or h < 1 or w < 1:
+        raise ValueError("segmentation_iou: want fake_segmap (N,%d,H,W), warped_cm (N,1,H,W) and parse (N,%d,H,W) with N, H, W >= 1; got %s"
+                         % (SEG_CHANNELS, SEG_CHANNELS, {k: tuple(t.shape) for k, t in ts.items()}))
+    if len({t.device for t in ts.values()}) != 1:
+        raise ValueError("segmentation_iou: the inputs are on different devices")
+    with torch.cuda.device(fake_segmap.device):
+        return ops.seg_iou(fake_segmap, warped_cm, parse)
+
+
 # ----------------------------------------------------------------------------------------------- Inception-v3
 
 INCEPTION_SIZE = 299

@@ -177,6 +177,21 @@ def seg_softmax_cat(input1, input2, seg, cm=None, cm_channel=3, composition="war
     return (out, seg_out) if want_seg else out
 
 
+def seg_iou(seg, cm, parse):
+    """train_condition.iou_metric(F.softmax(seg * cloth_mask, 1), parse), cloth_mask = ones with channel 3 = cm (composition
+    'warp_grad'), as a 0-dim fp32 cuda tensor (hrv_seg_iou; no synchronisation).  seg, parse: fp32 (N,K,H,W) cuda; cm: (N,1,H,W).
+    Shapes and dtypes are the caller's to check (metrics.segmentation_iou)."""
+    seg, cm, parse = seg.contiguous(), cm.contiguous(), parse.contiguous()
+    n, k, h, w = seg.shape
+    out = torch.empty((), dtype=torch.float32, device=seg.device)
+    L = capi.lib()
+    ws = torch.empty(max(int(L.hrv_seg_iou_workspace_bytes(n, h, w)), 16), dtype=torch.uint8, device=seg.device)
+    with _Timed("glue", 0.0, launches=2, label="seg_iou"):
+        capi.check(L.hrv_seg_iou(seg.data_ptr(), k, cm.data_ptr(), parse.data_ptr(), n, h, w, out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                 _stream()), "seg_iou")
+    return out
+
+
 # ----------------------------------------------------------------------------------------------- weights
 
 def pick_bk(cin):

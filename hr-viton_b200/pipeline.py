@@ -259,6 +259,29 @@ class ConditionGraph(_GraphRunner):
         return self._run_batch(inputs, datasetting)
 
 
+class SegmentationGraph(_GraphRunner):
+    """The stage-1 validation of train_condition.py:314-356 on one batch, replayed from a CUDA graph: the eval-mode tocg on the paired
+    cloth (its mask thresholded at 0.5, test_condition.py:84) and metrics.segmentation_iou of its segmentation ('warp_grad'
+    composition) against the batch's one-hot `parse`.  The contract of TryOnGraph: one graph per (input shapes, storage precision),
+    the tocg in eval mode, CUDA float32 inputs at the tocg resolution (cloth, cloth_mask, parse_agnostic, densepose, parse; cloth /
+    cloth_mask as tensors or {setting: tensor} dicts), recapture when its weights or BatchNorm running statistics changed.  Returns
+    the batch IoU as a 0-dim fp32 cuda tensor, owned by the runner until its next call."""
+
+    def __init__(self, tocg):
+        super().__init__([tocg])
+        self.tocg = tocg
+        self._channels = {"cloth": 3, "cloth_mask": 1, "parse_agnostic": tocg.io[1] - 3, "densepose": 3, "parse": tocg.io[2]}
+
+    def _body(self, static):
+        from . import metrics
+        with torch.no_grad():
+            _, _, outs = _condition(self.tocg, static, None, "paired")
+            return metrics.segmentation_iou(outs[1], outs[3], static["parse"])
+
+    def __call__(self, inputs, datasetting="paired"):
+        return self._run_batch(inputs, datasetting)
+
+
 class GeneratorGraph(_GraphRunner):
     """generator(x, seg) under torch.no_grad() replayed from a CUDA graph, with the contract of TryOnGraph: one graph per (x shape,
     seg shape, storage precision), eval mode, CUDA float32 inputs, recapture when the weights or the precision changed, fresh SPADE

@@ -1,6 +1,6 @@
 """Training runs of both stages to completion on the graph step (train_step) fed by the GPU loader (data.VitonHDLoader): the
 reference's learning-rate schedule, checkpoints in the reference's names and format, a sidecar state file from which a fresh process
-resumes bit for bit, periodic LPIPS on test try-ons, and the loss prints of train_condition.py / train_generator.py.
+resumes bit for bit, periodic LPIPS on test try-ons (stage 2) or segmentation IoU on test conditions (stage 1), and the loss prints of train_condition.py / train_generator.py.
 
     run = TrainRun("stage2", trainer, loader, "checkpoints/name", keep_step=100000, decay_step=100000)
     run.resume("checkpoints/name/state_step_010000.pth")     # optional, before start()
@@ -26,6 +26,8 @@ MODEL_FILES = {"stage1": {"tocg": ("tocg_step_%06d.pth", "tocg_final.pth"), "D":
 STATE_FILES = ("state_step_%06d.pth", "state_final.pth")
 LPIPS_SAMPLES = 500  # train_generator.py:620: Subset(test_dataset, np.arange(500))
 EVAL_KEYS = ("cloth", "cloth_mask", "agnostic", "densepose", "parse_agnostic", "image")
+VAL_SAMPLES = 2000  # train_condition.py:485: Subset(test_dataset, np.arange(2000))
+VAL_KEYS = ("cloth", "cloth_mask", "parse_agnostic", "densepose", "parse")
 
 
 def lr_lambda(k, load_step, keep_step, decay_step, interval=1000):
@@ -79,33 +81,42 @@ class TrainRun:
     Steps are counted as the reference counts them: the run trains steps load_step .. end - 1, end = keep_step (stage 1) or
     keep_step + decay_step (stage 2).  Stage 2 follows the reference's LambdaLR (lr_factor), whose scheduler steps every `interval`
     steps (1000 in the reference); stage 1 has no schedule, as train_condition.py has none.  Every save_count steps rank 0 writes the
-    model files of MODEL_FILES and a state file (state_step_%06d.pth); display_count prints the losses; lpips_count runs evaluate().
+    model files of MODEL_FILES and a state file (state_step_%06d.pth); display_count prints the losses; lpips_count runs evaluate() (stage
+    2) and val_count validate() (stage 1).
     A process group (torchrun) makes this one rank of a data-parallel run: the trainer's reducers and the sharded loader do the
     data-parallel work, and rank 0 writes the files.
 
     evaluator: for stage 2, (test_loader, lpips_model) — a VitonHDLoader in mode "test" with batch 1 and shard=False, and
     eval_models.PerceptualLoss or anything called as it (pred, target) -> (N,1,1,1).
+    validator: for stage 1, a VitonHDLoader in mode "test" with keys VAL_KEYS, the training's per-rank batch size, shuffle=False and
+    shard=False.
     on_step(step, losses): called after every step with the step's loss tensors (overwritten by the next replay)."""
 
     def __init__(self, stage, trainer, loader, checkpoint_dir, keep_step, decay_step=0, load_step=0, interval=1000, save_count=10000,
-                 display_count=100, lpips_count=None, evaluator=None, lpips_samples=LPIPS_SAMPLES, log=print, on_step=None):
+                 display_count=100, lpips_count=None, evaluator=None, lpips_samples=LPIPS_SAMPLES, val_count=None, validator=None,
+                 val_samples=VAL_SAMPLES, log=print, on_step=None):
         if stage not in STAGES:
             raise ValueError("stage must be one of %s, not %r" % (STAGES, stage))
         if stage == "stage2" and not trainer.tensor_lr:
             raise ValueError("stage 2 follows the reference's LR schedule: build the trainer with tensor_lr=True")
         if stage == "stage2" and lpips_count and evaluator is None and _dist()[1] == 0:  # only rank 0 evaluates
             raise ValueError("lpips_count needs an evaluator (test loader, LPIPS model) on rank 0")
+        if stage == "stage1" and val_count and validator is None and _dist()[1] == 0:  # only rank 0 validates
+            raise ValueError("val_count needs a validator (test loader) on rank 0")
         self.stage, self.trainer, self.loader, self.dir = stage, trainer, loader, checkpoint_dir
         self.keep_step, self.decay_step, self.load_step, self.interval = int(keep_step), int(decay_step), int(load_step), int(interval)
         self.end = self.keep_step + (self.decay_step if stage == "stage2" else 0)
         self.save_count, self.display_count, self.lpips_count = save_count, display_count, lpips_count
         self.evaluator, self.lpips_samples = evaluator, lpips_samples
+        self.val_count, self.validator, self.val_samples = val_count, validator, val_samples
         self.log, self.on_step = log, on_step
         self.step = self.load_step
         self.origin = self.load_step  # the load_step of the run's first process: the schedule's origin
         self.modules = {"stage1": {"tocg": trainer.tocg, "D": trainer.D}, "stage2": {"G": getattr(trainer, "G", None), "D": trainer.D}}[stage]
         self.lpips = []  # (step, value)
+        self.iou = []  # (step, value)
         self._tryon = None
+        self._seg = None
 
     # ---------------------------------------------------------------- schedule
     def factor(self, step=None):
@@ -216,6 +227,10 @@ class TrainRun:
                 value = self.evaluate()
                 self.lpips.append((self.step, value))
                 self.log("step: %8d, LPIPS: %.6f" % (self.step, value))
+            if self.stage == "stage1" and self.val_count and self.step % self.val_count == 0 and rank == 0:
+                value = self.validate()
+                self.iou.append((self.step, value))
+                self.log("step: %8d, IoU: %.6f" % (self.step, value))
             if self.display_count and self.step % self.display_count == 0 and rank == 0:
                 self.log("step: %8d, lr factor: %.6f, %s" % (self.step, factor, ", ".join("%s: %.4f" % (k, float(v)) for k, v in losses.items())))
             if self.save_count and self.step % self.save_count == 0:
@@ -252,6 +267,39 @@ class TrainRun:
             G.train()
         return value
 
+    def validate(self):
+        """train_condition.py:314-360: validation_iou of the tocg in eval mode over the validator, through one
+        pipeline.SegmentationGraph that re-captures once per validation (the weights changed since the last).  Eval mode leaves the
+        BatchNorm statistics alone and validation_iou forks the random streams, so a validation does not change the training that
+        follows."""
+        from . import pipeline
+        tocg = self.trainer.tocg
+        tocg.eval()
+        try:
+            if self._seg is None:
+                self._seg = pipeline.SegmentationGraph(tocg)
+            return validation_iou(self._seg, self.validator, self.val_samples)
+        finally:
+            tocg.train()
+
+
+def validation_iou(runner, loader, samples=VAL_SAMPLES):
+    """The value train_condition.py's validation logs: the IoU of runner (a pipeline.SegmentationGraph) on the first min(samples,
+    len) samples of `loader` (a VitonHDLoader in mode "test", keys VAL_KEYS, shuffle=False) in full batches of its batch size
+    (drop_last), paired cloth.  Each batch's IoU stays on the device; the result is np.mean of the batch IoUs as Python floats (the
+    reference's np.mean(iou_list)), read with one copy.  Every call starts at the first sample, whereas the reference reads its test
+    loader from wherever the previous validation stopped (DESIGN.md)."""
+    import numpy as np
+    batches = min(samples, len(loader.dataset)) // loader.batch_size
+    if batches < 1:
+        raise ValueError("validation_iou: %d test samples make no batch of %d" % (min(samples, len(loader.dataset)), loader.batch_size))
+    with torch.random.fork_rng(devices=[loader.device]), torch.no_grad():
+        loader.start_at(0, 0)
+        ious = torch.empty(batches, dtype=torch.float32, device=loader.device)
+        for i in range(batches):
+            ious[i] = runner(loader.next_batch())
+        return float(np.mean(ious.tolist()))
+
 
 # -------------------------------------------------------------------------------------------------------------------- command line
 
@@ -282,12 +330,14 @@ def parse_args(stage, argv=None):
     p.add_argument("--occlusion", action="store_true")
     p.add_argument("--seed", type=int, default=0, help="model initialisation, data order and noise")
     p.add_argument("--resume", default=None, help="a state file (state_step_%%06d.pth) written by an earlier run")
+    p.add_argument("--test_dataroot", default="./data/")
+    p.add_argument("--test_data_list", default="test_pairs.txt")
     if s2:
         p.add_argument("--decay_step", type=int, default=100000)
         p.add_argument("--lpips_count", type=int, default=1000)
-        p.add_argument("--test_dataroot", default="./data/")
-        p.add_argument("--test_data_list", default="test_pairs.txt")
         p.add_argument("--lr_interval", type=int, default=1000, help="steps between scheduler steps (the reference's 1000)")
+    else:
+        p.add_argument("--val_count", type=int, default=None, help="steps between validations (segmentation IoU); default: none")
     opt = p.parse_args(argv)
     opt.stage = stage
     positive = ["workers", "batch_size", "fine_width", "fine_height", "display_count", "save_count", "keep_step"] + (["lpips_count", "lr_interval"]
@@ -295,6 +345,8 @@ def parse_args(stage, argv=None):
     for k in positive:
         if getattr(opt, k) < (0 if k == "workers" else 1):
             p.error("--%s must be %s, got %d" % (k, "non-negative" if k == "workers" else "positive", getattr(opt, k)))
+    if not s2 and opt.val_count is not None and opt.val_count < 1:
+        p.error("--val_count must be positive, got %d" % opt.val_count)
     if opt.load_step < 0 or (s2 and opt.decay_step < 0):
         p.error("--load_step and --decay_step must be non-negative")
     end = opt.keep_step + (opt.decay_step if s2 else 0)
@@ -307,7 +359,7 @@ def parse_args(stage, argv=None):
     want = data.resized_size(1024, 768, opt.fine_width)
     if (opt.fine_height, opt.fine_width) != want:
         p.error("--fine_height %d: VITON-HD's 1024x768 images resize to %dx%d at --fine_width %d" % (opt.fine_height, want[0], want[1], opt.fine_width))
-    for k in ("dataroot",) + (("tocg_checkpoint",) if s2 else ()):
+    for k in ("dataroot",) + (("tocg_checkpoint",) if s2 else ()) + (("test_dataroot",) if not s2 and opt.val_count else ()):
         if not os.path.exists(getattr(opt, k)):
             p.error("--%s %s does not exist" % (k, getattr(opt, k)))
     if opt.resume is not None and not os.path.isfile(opt.resume):
@@ -384,10 +436,14 @@ def build(opt, log=print):
         test_loader = data.VitonHDLoader(opt.test_dataroot, "test", opt.test_data_list, opt.fine_height, opt.fine_width, 1,
                                          workers=opt.workers, mode="test", keys=EVAL_KEYS, shuffle=False, shard=False)
         evaluator = (test_loader, eval_models.PerceptualLoss(model="net-lin", net="alex", use_gpu=True, gpu_ids=[dev.index]))
+    validator = None
+    if not s2 and opt.val_count and rank == 0:
+        validator = data.VitonHDLoader(opt.test_dataroot, "test", opt.test_data_list, opt.fine_height, opt.fine_width, opt.batch_size // world,
+                                       workers=opt.workers, mode="test", keys=VAL_KEYS, shuffle=False, shard=False)
     run = TrainRun(opt.stage, trainer, loader, os.path.join(opt.checkpoint_dir, opt.name), opt.keep_step,
                    decay_step=opt.decay_step if s2 else 0, load_step=opt.load_step, interval=opt.lr_interval if s2 else 1000,
                    save_count=opt.save_count, display_count=opt.display_count, lpips_count=opt.lpips_count if s2 else None,
-                   evaluator=evaluator, log=log)
+                   evaluator=evaluator, val_count=None if s2 else opt.val_count, validator=validator, log=log)
     if opt.resume:
         run.resume(opt.resume)
     return run

@@ -205,6 +205,18 @@ int hrv_seg_softmax_cat(const float* input1, int32_t c1, const float* input2, in
                         const float* cm, int32_t cm_channel, int32_t mode, int32_t softmax, const hrv_tensor* dst,
                         float* seg_out, hrv_stream stream);
 
+/* The stage-1 validation IoU (train_condition.py:18-36, :314-356): iou_metric(F.softmax(seg * cloth_mask, 1), parse) as one fp32 value.
+ * Per pixel, channel 3 of seg is multiplied by cm (composition 'warp_grad') and the k channels are soft-maxed with the functions of
+ * hrv_seg_softmax_cat; pred = p > 0.5 (p = 0.5 exactly is not predicted), lab = (parse == 1).  Per sample, integer counts over
+ * every channel and pixel: P = #pred, L = #lab, I = #(pred and lab).  Then, in the reference's fp32 arithmetic, summed over the
+ * samples in order:  *iou = sum_n ((f32(I) + 1e-7f) / ((f32(P) + f32(L)) - f32(I) + 1e-7f)) / f32(n).
+ * seg, parse: fp32 [n][k][h][w] contiguous (parse one-hot, values in {0, 1}); cm: fp32 [n][1][h][w]; iou: one fp32 on the device.
+ * Per-warp partial counts go to `workspace` (hrv_seg_iou_workspace_bytes(n, h, w) bytes) and are added by a one-warp finishing
+ * kernel: no floating-point atomics, the same result on every run.  Needs k > 3 and k*h*w < 2^31. */
+size_t hrv_seg_iou_workspace_bytes(int32_t n, int32_t h, int32_t w);
+int hrv_seg_iou(const float* seg, int32_t k, const float* cm, const float* parse, int32_t n, int32_t h, int32_t w, float* iou,
+                void* workspace, size_t workspace_bytes, hrv_stream stream);
+
 /* bf16|f32 NHWC view -> fp32 NCHW contiguous [n][c][h][w]. */
 int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream);
 
