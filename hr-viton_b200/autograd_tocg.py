@@ -134,6 +134,44 @@ class FlowWarpNchwFn(torch.autograd.Function):
         return dflo, None, None, None, None
 
 
+class FlowTVFn(torch.autograd.Function):
+    """loss = hrv_flow_tv(flows, mask): the flow TV of train_condition.py:183-232, edge-aware where mask is given (see ops.flow_tv for
+    the weights); backward = hrv_flow_tv_bwd, a fixed-order gather into every flow and the mask (torch's bilinear-interpolate
+    backward, which the reference's expression needs, is refused under torch.use_deterministic_algorithms(True) on CUDA)."""
+
+    @staticmethod
+    def forward(ctx, mask, edge_weights, plain_weights, *flows):
+        flows = [f.contiguous() for f in flows]
+        mask = mask.contiguous() if mask is not None else None
+        loss, _ = ops.flow_tv(flows, edge_weights, plain_weights, mask)
+        ctx.save_for_backward(mask, *flows)
+        ctx.weights = (edge_weights, plain_weights)
+        return loss
+
+    @staticmethod
+    def backward(ctx, dloss):
+        mask, *flows = ctx.saved_tensors
+        dflows, dmask = ops.flow_tv_bwd(flows, *ctx.weights, mask, dloss.float().contiguous().reshape(1),
+                                        want_dmask=ctx.needs_input_grad[0])
+        return (dmask, None, None) + tuple(d if need else None for d, need in zip(dflows, ctx.needs_input_grad[3:]))
+
+
+def flow_tv(flow_list, mask, edgeawaretv, add_lasttv=False):
+    """train_condition.py:201-232 (--edgeawaretv last_only|weighted, --add_lasttv) as one FlowTVFn: 'last_only' the edge-aware TV of the
+    last flow, 'weighted' of all five with weights 1/2^(4-i); add_lasttv adds the plain TV of the last flow.  mask (N,1,H,W): the warped
+    cloth mask whose bilinear down-samplings weight the flow differences; gradients reach it and every flow."""
+    if edgeawaretv == "last_only":
+        flows, edge = list(flow_list[-1:]), [1.0]
+    elif edgeawaretv == "weighted":
+        flows, edge = list(flow_list), [1.0 / (2 ** (4 - i)) for i in range(len(flow_list))]
+    else:
+        raise ValueError("edgeawaretv must be 'last_only' or 'weighted', got %r" % (edgeawaretv,))
+    plain = [0.0] * len(flows)
+    if add_lasttv:
+        plain[-1] = 1.0
+    return FlowTVFn.apply(mask, tuple(edge), tuple(plain), *flows)
+
+
 def _resblock(rb, x_buf):
     """ResBlock.forward in training mode (networks.py:171-198)."""
     if rb.kind == "down":

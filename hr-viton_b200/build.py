@@ -14,7 +14,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libhrviton_sm100.so")
 SHARED = ["capi.cu"]
 KERNEL_TUS = ["conv_igemm.cu", "aux_kernels.cu", "norm_bwd.cu", "conv_wgrad.cu", "glue_kernels.cu", "conv_f32.cu", "syncbn.cu", "metrics.cu", "data_kernels.cu",
-             "jpeg_kernels.cu", "jpeg_encode.cu"]
+             "jpeg_kernels.cu", "jpeg_encode.cu", "tv_kernels.cu"]
 SINGLE = ("conv_f32.cu", "metrics.cu", "data_kernels.cu", "jpeg_kernels.cu", "jpeg_encode.cu")  # no 16-bit storage: compiled once
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",

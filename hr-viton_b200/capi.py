@@ -19,7 +19,7 @@ EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_i
            "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
            "hrv_grad_unscale_check", "hrv_syncbn_combine", "hrv_syncbn_fwd_finalize", "hrv_syncbn_bwd_finalize", "hrv_seg_softmax_cat", "hrv_seg_iou", "hrv_seg_iou_workspace_bytes",
-           "hrv_last_error",
+           "hrv_flow_tv", "hrv_flow_tv_bwd", "hrv_flow_tv_workspace_bytes", "hrv_last_error",
            "hrv_version", "hrv_device_sm_count"]
 # include/hrviton_sm100_metrics.h: fp32 / fp64 only, one flavour (no _f16 twin)
 METRICS_EXPORTS = ["hrv_lpips_input", "hrv_maxpool3s2", "hrv_lpips_dist", "hrv_ssim", "hrv_ssim_workspace_bytes", "hrv_resize_bilinear_nhwc",
@@ -38,6 +38,14 @@ JPEG_SRC_U8_NHWC, JPEG_SRC_F32_NCHW = 0, 1
 class Tensor(ctypes.Structure):
     _fields_ = [("ptr", ctypes.c_void_p), ("n", ctypes.c_int32), ("h", ctypes.c_int32), ("w", ctypes.c_int32),
                 ("c", ctypes.c_int32), ("pitch", ctypes.c_int32), ("dtype", ctypes.c_int32)]
+
+
+class TvFlow(ctypes.Structure):
+    _fields_ = [("flow", ctypes.c_void_p), ("h", ctypes.c_int32), ("w", ctypes.c_int32), ("edge_weight", ctypes.c_float),
+                ("plain_weight", ctypes.c_float)]
+
+
+TV_MAX_FLOWS = 5  # HRV_TV_MAX_FLOWS
 
 
 class VitonPlanes(ctypes.Structure):
@@ -109,6 +117,10 @@ def lib(dtype=None):
     L.hrv_seg_softmax_cat.argtypes = [vp, i32, vp, i32, vp, i32, vp, i32, i32, i32, TP, vp, vp]
     L.hrv_seg_iou.argtypes = [vp, i32, vp, vp, i32, i32, i32, vp, vp, sz, vp]
     L.hrv_seg_iou_workspace_bytes.argtypes = [i32, i32, i32]
+    TVP = ctypes.POINTER(TvFlow)
+    L.hrv_flow_tv_workspace_bytes.argtypes = [TVP, i32, i32]
+    L.hrv_flow_tv.argtypes = [TVP, i32, i32, vp, i32, i32, vp, vp, ctypes.POINTER(vp), vp, sz, vp]
+    L.hrv_flow_tv_bwd.argtypes = [TVP, i32, i32, vp, i32, i32, vp, ctypes.POINTER(vp), vp, vp, sz, vp]
     L.hrv_space_to_depth.argtypes = [TP, TP, vp]
     L.hrv_avgpool3s2.argtypes = [TP, TP, vp]
     L.hrv_bilinear_up2_add.argtypes = [TP, TP, TP, vp]

@@ -5,6 +5,7 @@
 // partials land in slabs that a second kernel adds in a fixed order.
 #include <type_traits>
 
+#include "hrv_bilinear.cuh"
 #include "hrv_host.h"
 
 namespace hrv_metrics {
@@ -227,11 +228,6 @@ int ssim_tiles(int h, int w, int* tiles_x) {
 // (u8 / 255, correctly rounded).  kNormBefore maps every tap v to 2v - 1 before the blend (torchvision Inception on [0, 1] images),
 // kNormAfter maps the blended value (pytorch-fid: F.interpolate, then 2x - 1); 2v is exact, so either is one rounding, as in torch.
 // One thread per output element of the first 8-channel groups; channels [c, c8) are written as zeros.
-__device__ __forceinline__ float bilinear_src(float scale, int d) {
-  const float s = __fmaf_rn(scale, __fadd_rn((float)d, 0.5f), -0.5f);  // scale * (d + 0.5) - 0.5, contracted as in torch's kernel
-  return s < 0.f ? 0.f : s;
-}
-
 struct NchwF32 {
   const float* p;
   int c, h, w;
@@ -261,26 +257,13 @@ __global__ void resize_bilinear_kernel(Src src, float rh, float rw, float* __res
   if (ch < src.c) {
     const int ox = (int)(pix % ow), oy = (int)((pix / ow) % oh);
     const long long img = pix / ((long long)ow * oh);
-    const float h1r = bilinear_src(rh, oy);
-    const int h1 = h1r;
-    const int h1p = (h1 < h - 1) ? 1 : 0;
-    const float h1lambda = h1r - h1;
-    const float h0lambda = static_cast<float>(1) - h1lambda;
-    const float w1r = bilinear_src(rw, ox);
-    const int w1 = w1r;
-    const int w1p = (w1 < w - 1) ? 1 : 0;
-    const float w1lambda = w1r - w1;
-    const float w0lambda = static_cast<float>(1) - w1lambda;
-    float v00 = src(img, ch, h1, w1), v01 = src(img, ch, h1, w1 + w1p);
-    float v10 = src(img, ch, h1 + h1p, w1), v11 = src(img, ch, h1 + h1p, w1 + w1p);
+    const hrv_bilinear::Taps ty = hrv_bilinear::bilinear_taps(rh, oy, h), tx = hrv_bilinear::bilinear_taps(rw, ox, w);
+    float v00 = src(img, ch, ty.i0, tx.i0), v01 = src(img, ch, ty.i0, tx.i1);
+    float v10 = src(img, ch, ty.i1, tx.i0), v11 = src(img, ch, ty.i1, tx.i1);
     if (kNorm == kNormBefore) {
       v00 = to_signed_unit(v00); v01 = to_signed_unit(v01); v10 = to_signed_unit(v10); v11 = to_signed_unit(v11);
     }
-    // h0lambda * (w0lambda * v00 + w1lambda * v01) + h1lambda * (w0lambda * v10 + w1lambda * v11), with the fma contraction torch's
-    // kernel is compiled with spelled out: left to the compiler, the contraction differs between instantiations of this template
-    const float top = __fmaf_rn(w0lambda, v00, __fmul_rn(w1lambda, v01));
-    const float bottom = __fmaf_rn(w0lambda, v10, __fmul_rn(w1lambda, v11));
-    val = __fmaf_rn(h0lambda, top, __fmul_rn(h1lambda, bottom));
+    val = hrv_bilinear::bilinear_blend(ty, tx, v00, v01, v10, v11);
     if (kNorm == kNormAfter) val = to_signed_unit(val);
   }
   dst[pix * pitch + ch] = val;

@@ -192,6 +192,55 @@ def seg_iou(seg, cm, parse):
     return out
 
 
+def _tv_flows(flows, edge_weights, plain_weights, mask):
+    if not 1 <= len(flows) <= capi.TV_MAX_FLOWS or not len(flows) == len(edge_weights) == len(plain_weights):
+        raise ValueError("flow_tv: 1..%d flows with one edge and one plain weight each, got %d / %d / %d"
+                         % (capi.TV_MAX_FLOWS, len(flows), len(edge_weights), len(plain_weights)))
+    n = flows[0].shape[0]
+    for f in flows:
+        if not f.is_cuda or f.dtype != torch.float32 or f.dim() != 4 or f.shape[0] != n or f.shape[3] != 2 or not f.is_contiguous():
+            raise ValueError("flow_tv: flows must be contiguous float32 (N,h,w,2) cuda tensors, got %s %s" % (tuple(f.shape), f.dtype))
+    if mask is not None and (not mask.is_cuda or mask.dtype != torch.float32 or mask.dim() != 4 or mask.shape[:2] != (n, 1)
+                             or not mask.is_contiguous()):
+        raise ValueError("flow_tv: mask must be a contiguous float32 (N,1,H,W) cuda tensor, got %s %s" % (tuple(mask.shape), mask.dtype))
+    arr = (capi.TvFlow * len(flows))(*[capi.TvFlow(f.data_ptr(), f.shape[1], f.shape[2], float(we), float(wp))
+                                       for f, we, wp in zip(flows, edge_weights, plain_weights)])
+    mh, mw = (mask.shape[2], mask.shape[3]) if mask is not None else (0, 0)
+    L = capi.lib()
+    ws = torch.empty(int(L.hrv_flow_tv_workspace_bytes(arr, len(flows), n)), dtype=torch.uint8, device=flows[0].device)
+    return L, arr, n, mh, mw, ws
+
+
+def flow_tv(flows, edge_weights, plain_weights, mask=None, want_mask_down=False):
+    """The stage-1 flow TV (hrv_flow_tv): sum over i of edge_weights[i] * (edge-aware TV of flows[i], weighted by exp(-150 |D m_i|),
+    m_i = F.interpolate(mask, flows[i]'s size, bilinear); the plain TV without mask) + plain_weights[i] * (plain TV of flows[i]).
+    flows: contiguous fp32 (N,h,w,2) cuda; mask: contiguous fp32 (N,1,H,W) or None.  Returns (loss 0-dim, per-flow terms (len,)) fp32 on
+    the device, reproducible bit for bit, no synchronisation; want_mask_down=True (with mask) adds the list of m_i (N,1,h_i,w_i)."""
+    L, arr, n, mh, mw, ws = _tv_flows(flows, edge_weights, plain_weights, mask)
+    loss = torch.empty((), dtype=torch.float32, device=flows[0].device)
+    terms = torch.empty(len(flows), dtype=torch.float32, device=flows[0].device)
+    downs = [torch.empty((n, 1, f.shape[1], f.shape[2]), dtype=torch.float32, device=f.device) for f in flows] if want_mask_down else None
+    dptrs = (ctypes.c_void_p * len(flows))(*[d.data_ptr() for d in downs]) if want_mask_down else None
+    with _Timed("glue", 0.0, launches=3 if mask is not None else 2, label="flow_tv"):
+        capi.check(L.hrv_flow_tv(arr, len(flows), n, _p(mask), mh, mw, loss.data_ptr(), terms.data_ptr(), dptrs, ws.data_ptr(), ws.numel(),
+                                 _stream()), "flow_tv")
+    return (loss, terms, downs) if want_mask_down else (loss, terms)
+
+
+def flow_tv_bwd(flows, edge_weights, plain_weights, mask, dloss, want_dmask=True):
+    """Gradients of flow_tv for the upstream scalar dloss (a 1-element fp32 cuda tensor): ([dflow_i (N,h,w,2)], dmask (N,1,H,W) or None),
+    from gathers in a fixed order (hrv_flow_tv_bwd)."""
+    L, arr, n, mh, mw, ws = _tv_flows(flows, edge_weights, plain_weights, mask)
+    assert dloss.is_cuda and dloss.dtype == torch.float32 and dloss.numel() == 1
+    dflows = [torch.empty_like(f) for f in flows]
+    dmask = torch.empty_like(mask) if (mask is not None and want_dmask) else None
+    dptrs = (ctypes.c_void_p * len(flows))(*[d.data_ptr() for d in dflows])
+    with _Timed("glue", 0.0, launches=(1 if mask is not None else 0) + 1 + (1 if dmask is not None else 0), label="flow_tv_bwd"):
+        capi.check(L.hrv_flow_tv_bwd(arr, len(flows), n, _p(mask), mh, mw, dloss.data_ptr(), dptrs, _p(dmask), ws.data_ptr(), ws.numel(),
+                                     _stream()), "flow_tv_bwd")
+    return dflows, dmask
+
+
 # ----------------------------------------------------------------------------------------------- weights
 
 def pick_bk(cin):

@@ -28,6 +28,9 @@ LPIPS_SAMPLES = 500  # train_generator.py:620: Subset(test_dataset, np.arange(50
 EVAL_KEYS = ("cloth", "cloth_mask", "agnostic", "densepose", "parse_agnostic", "image")
 VAL_SAMPLES = 2000  # train_condition.py:485: Subset(test_dataset, np.arange(2000))
 VAL_KEYS = ("cloth", "cloth_mask", "parse_agnostic", "densepose", "parse")
+# the stage-1 loss options a resumed run must share, with the values a state file that does not record them was trained with
+STAGE1_OPTIONS = {"edgeawaretv": "no_edge", "add_lasttv": False, "clothmask_composition": "warp_grad", "no_gan_loss": False,
+                  "g_d_separate": False, "tvlambda": 2.0, "ce_lambda": 10.0, "gan_lambda": 1.0}
 
 
 def lr_lambda(k, load_step, keep_step, decay_step, interval=1000):
@@ -126,9 +129,12 @@ class TrainRun:
 
     # ---------------------------------------------------------------- files
     def config(self):
-        """What a resumed run must share with the run it continues beyond the schedule: both base learning rates, --occlusion and,
-        for stage 2, the frozen tocg (a SHA-256 of its state, so another --tocg_checkpoint file with the same weights is accepted)."""
+        """What a resumed run must share with the run it continues beyond the schedule: both base learning rates, --occlusion, for
+        stage 1 the loss options of STAGE1_OPTIONS and, for stage 2, the frozen tocg (a SHA-256 of its state, so another --tocg_checkpoint
+        file with the same weights is accepted)."""
         cfg = {"base_lr": dict(self.trainer.base_lr), "occlusion": getattr(self.trainer, "occlusion", None)}
+        if self.stage == "stage1":
+            cfg.update((k, getattr(self.trainer, k, v)) for k, v in STAGE1_OPTIONS.items())  # a trainer without them trains the defaults
         if self.stage == "stage2":
             h = hashlib.sha256()
             for k, v in self.trainer.tocg.state_dict().items():
@@ -174,7 +180,9 @@ class TrainRun:
             if self.stage == "stage2" and st[k] != getattr(self, k):
                 raise ValueError("%s was saved with %s=%r, this run has %r" % (path, k, st[k], getattr(self, k)))
         cfg = self.config()
-        for k, v in st["config"].items():
+        saved = dict(STAGE1_OPTIONS) if self.stage == "stage1" else {}  # a state file written before the options were recorded
+        saved.update(st["config"])
+        for k, v in saved.items():
             if cfg.get(k) != v:
                 raise ValueError("%s was saved with %s=%r, this run has %r" % (path, k, v, cfg.get(k)))
         if len(st["rng"]) != world:
@@ -338,6 +346,16 @@ def parse_args(stage, argv=None):
         p.add_argument("--lr_interval", type=int, default=1000, help="steps between scheduler steps (the reference's 1000)")
     else:
         p.add_argument("--val_count", type=int, default=None, help="steps between validations (segmentation IoU); default: none")
+        p.add_argument("--edgeawaretv", choices=train_step.EDGEAWARETV, default="no_edge", help="edge-aware flow TV")
+        p.add_argument("--add_lasttv", action="store_true", help="with --edgeawaretv: add the plain TV of the last flow")
+        p.add_argument("--clothmask_composition", choices=train_step.CLOTHMASK_COMPOSITIONS, default="warp_grad")
+        p.add_argument("--no_GAN_loss", action="store_true", help="train the tocg without the discriminator")
+        p.add_argument("--G_D_seperate", action="store_true", help="step G first, then D on a new tocg forward")
+        p.add_argument("--tvlambda", type=float, default=2.0)
+        p.add_argument("--CElamda", type=float, default=10.0)
+        p.add_argument("--GANlambda", type=float, default=1.0)
+        for flag in ("--lasttvonly", "--interflowloss", "--Ddownx2", "--Ddropout"):  # the README's stage-1 command line
+            p.add_argument(flag, action="store_true", help="always on: accepted so that the README's command line parses")
     opt = p.parse_args(argv)
     opt.stage = stage
     positive = ["workers", "batch_size", "fine_width", "fine_height", "display_count", "save_count", "keep_step"] + (["lpips_count", "lr_interval"]
@@ -347,6 +365,8 @@ def parse_args(stage, argv=None):
             p.error("--%s must be %s, got %d" % (k, "non-negative" if k == "workers" else "positive", getattr(opt, k)))
     if not s2 and opt.val_count is not None and opt.val_count < 1:
         p.error("--val_count must be positive, got %d" % opt.val_count)
+    if not s2 and opt.val_count and opt.clothmask_composition != "warp_grad":
+        p.error("--val_count validates the 'warp_grad' composition only, not --clothmask_composition %s" % opt.clothmask_composition)
     if opt.load_step < 0 or (s2 and opt.decay_step < 0):
         p.error("--load_step and --decay_step must be non-negative")
     end = opt.keep_step + (opt.decay_step if s2 else 0)
@@ -365,6 +385,13 @@ def parse_args(stage, argv=None):
     if opt.resume is not None and not os.path.isfile(opt.resume):
         p.error("--resume %s is not a file" % opt.resume)
     return opt
+
+
+def stage1_options(opt):
+    """The Stage1Trainer keywords (the keys of STAGE1_OPTIONS) of parsed stage-1 flags."""
+    return {"edgeawaretv": opt.edgeawaretv, "add_lasttv": opt.add_lasttv, "clothmask_composition": opt.clothmask_composition,
+            "no_gan_loss": opt.no_GAN_loss, "g_d_separate": opt.G_D_seperate, "tvlambda": opt.tvlambda, "ce_lambda": opt.CElamda,
+            "gan_lambda": opt.GANlambda}
 
 
 def build(opt, log=print):
@@ -426,7 +453,7 @@ def build(opt, log=print):
                                            loss_scale=loss_scale, tensor_lr=True)
     else:
         trainer = train_step.Stage1Trainer(tocg, D, vgg, lr=opt.G_lr, d_lr=opt.D_lr, occlusion=opt.occlusion, reducers=reducers,
-                                           loss_scale=loss_scale)
+                                           loss_scale=loss_scale, **stage1_options(opt))
     keys = data.STAGE2_KEYS if s2 else data.STAGE1_KEYS
     loader = data.VitonHDLoader(opt.dataroot, opt.datamode, opt.data_list, opt.fine_height, opt.fine_width, opt.batch_size // world,
                                 workers=opt.workers, keys=keys, seed=opt.seed)

@@ -406,17 +406,35 @@ def synthetic_batch(n, h, w, device, seed=0):
 
 # ------------------------------------------------------------------------------------------------ stage 1 (train_condition.py)
 
+EDGEAWARETV = ("no_edge", "last_only", "weighted")  # train_condition.py --edgeawaretv
+CLOTHMASK_COMPOSITIONS = ("warp_grad", "detach", "no_composition")  # train_condition.py --clothmask_composition
+
+
 class Stage1Trainer(_GraphMixin, _TrainState, _LossScaling):
-    """One train_condition.py step (train_condition.py:133-286) with the README's flags (--Ddownx2 --Ddropout --lasttvonly
+    """One train_condition.py step (train_condition.py:133-312) with the README's flags (--Ddownx2 --Ddropout --lasttvonly
     --interflowloss --occlusion): tocg forward+backward on this repo's kernels (train-mode BatchNorm), L1 + VGG + TV + CE + LSGAN.
     loss_scale: None or "dynamic" (as Stage2Trainer).  lr: both optimisers' (--G_lr, --D_lr), unless d_lr is given.  tensor_lr: see
-    _TrainState."""
+    _TrainState.
+
+    The reference's other loss options, each defaulting to the README's run:
+      edgeawaretv ('no_edge' | 'last_only' | 'weighted'): flow TV weighted by exp(-150 |D warped_cm|) (autograd_tocg.flow_tv, on
+        hrv_flow_tv); lasttvonly is then ignored, and add_lasttv adds the plain TV of the last flow;
+      clothmask_composition ('warp_grad' | 'detach' | 'no_composition'): how the warped cloth mask enters the segmentation;
+      no_gan_loss: no discriminator at all (D, its Adam state and its loss scaler are left alone);
+      g_d_separate: the G step first, then D on a new no-grad, train-mode tocg forward (train_condition.py:283-312)."""
 
     def __init__(self, tocg, D, vgg, lr=2e-4, lasttvonly=True, interflowloss=True, occlusion=True, tvlambda=2.0, ce_lambda=10.0,
-                 gan_lambda=1.0, reducers=None, loss_scale=None, d_lr=None, tensor_lr=False):
+                 gan_lambda=1.0, reducers=None, loss_scale=None, d_lr=None, tensor_lr=False, edgeawaretv="no_edge", add_lasttv=False,
+                 clothmask_composition="warp_grad", no_gan_loss=False, g_d_separate=False):
+        if edgeawaretv not in EDGEAWARETV:
+            raise ValueError("edgeawaretv must be one of %s, got %r" % ("/".join(EDGEAWARETV), edgeawaretv))
+        if clothmask_composition not in CLOTHMASK_COMPOSITIONS:
+            raise ValueError("clothmask_composition must be one of %s, got %r" % ("/".join(CLOTHMASK_COMPOSITIONS), clothmask_composition))
         self.tocg, self.D, self.vgg = tocg, D, vgg
         self.lasttvonly, self.interflowloss, self.occlusion = lasttvonly, interflowloss, occlusion
         self.tvlambda, self.ce_lambda, self.gan_lambda = tvlambda, ce_lambda, gan_lambda
+        self.edgeawaretv, self.add_lasttv, self.clothmask_composition = edgeawaretv, bool(add_lasttv), clothmask_composition
+        self.no_gan_loss, self.g_d_separate = bool(no_gan_loss), bool(g_d_separate)
         self.vgg_weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
         self._make_optimizers(tocg.parameters(), D.parameters(), lr, lr if d_lr is None else d_lr, (0.5, 0.999), tensor_lr)
         self.reducers = reducers or {}
@@ -442,17 +460,25 @@ class Stage1Trainer(_GraphMixin, _TrainState, _LossScaling):
         input1 = torch.cat([c_paired, cm_paired], 1)
         input2 = torch.cat([batch["parse_agnostic"], batch["densepose"]], 1)
         flow_list, seg, warped_c, warped_cm = autograd_tocg.tocg_forward_train(self.tocg, input1, input2)
-        mask = torch.ones_like(seg.detach())
-        mask = torch.cat([mask[:, :3], warped_cm, mask[:, 4:]], 1)  # clothmask_composition == 'warp_grad'
-        seg = seg * mask
+        if self.clothmask_composition == "warp_grad":
+            mask = torch.ones_like(seg.detach())
+            mask = torch.cat([mask[:, :3], warped_cm, mask[:, 4:]], 1)
+            seg = seg * mask
+        elif self.clothmask_composition == "detach":  # the pre-occlusion mask, thresholded, without gradient (warped_cm_onehot)
+            mask = torch.ones_like(seg.detach())
+            mask = torch.cat([mask[:, :3], (warped_cm.detach() > 0.5).float(), mask[:, 4:]], 1)
+            seg = seg * mask
         if self.occlusion:
             warped_cm = self._remove_overlap(F.softmax(seg, dim=1), warped_cm)
             warped_c = warped_c * warped_cm + (1 - warped_cm)
         loss_l1 = F.l1_loss(warped_cm, pcm)
         loss_vgg = autograd_g.vgg_loss(self.vgg, self.vgg_weights, warped_c, im_c)
         loss_tv = 0
-        for flow in (flow_list[-1:] if self.lasttvonly else flow_list):
-            loss_tv = loss_tv + (flow[:, 1:] - flow[:, :-1]).abs().mean() + (flow[:, :, 1:] - flow[:, :, :-1]).abs().mean()
+        if self.edgeawaretv == "no_edge":
+            for flow in (flow_list[-1:] if self.lasttvonly else flow_list):
+                loss_tv = loss_tv + (flow[:, 1:] - flow[:, :-1]).abs().mean() + (flow[:, :, 1:] - flow[:, :, :-1]).abs().mean()
+        else:  # the mask is the (post-occlusion) warped cloth mask, not detached: its gradient reaches the segmentation and the flow
+            loss_tv = autograd_tocg.flow_tv(flow_list, warped_cm, self.edgeawaretv, self.add_lasttv)
         n, _, ih, iw = c_paired.shape
         if self.interflowloss:
             # F.interpolate(size, bilinear) + normalise + base grid + grid_sample(border) of cloth and mask: hrv_flow_warp_nchw and its
@@ -464,12 +490,22 @@ class Stage1Trainer(_GraphMixin, _TrainState, _LossScaling):
                 loss_l1 = loss_l1 + F.l1_loss(wcm, pcm) / (2 ** (4 - i))
                 loss_vgg = loss_vgg + autograd_g.vgg_loss(self.vgg, self.vgg_weights, wc, im_c) / (2 ** (4 - i))
         ce = cross_entropy_ignore(seg, batch["parse_onehot"][:, 0].long(), ignore_index=250)  # utils.cross_entropy2d
+        out = {"l1": loss_l1.detach(), "vgg": loss_vgg.detach(), "ce": ce.detach()}
+        if self.no_gan_loss:  # train_condition.py:263-268: G alone
+            loss_g = (10 * loss_l1 + loss_vgg + self.tvlambda * loss_tv) + ce * self.ce_lambda
+            self.opt_g.zero_grad(set_to_none=not self.scalers)
+            self._backward(loss_g, "G")
+            if "G" in self.reducers and self._explicit_reduce:
+                self.reducers["G"].reduce()
+            self._opt_step(self.opt_g, "G")
+            return {"loss_g": loss_g.detach(), **out}
         soft = torch.softmax(seg, 1)
         d_in = torch.cat((input1.detach(), input2.detach(), soft), 1)
         loss_g_gan = self._lsgan(autograd_tocg.tocg_discriminator_forward_train(self.D, d_in), True)
-        pred_fake = autograd_tocg.tocg_discriminator_forward_train(self.D, d_in.detach())
-        pred_real = autograd_tocg.tocg_discriminator_forward_train(self.D, torch.cat((input1.detach(), input2.detach(), batch["parse"]), 1))
-        loss_d = self._lsgan(pred_fake, False) + self._lsgan(pred_real, True)
+        if not self.g_d_separate:
+            pred_fake = autograd_tocg.tocg_discriminator_forward_train(self.D, d_in.detach())
+            pred_real = autograd_tocg.tocg_discriminator_forward_train(self.D, torch.cat((input1.detach(), input2.detach(), batch["parse"]), 1))
+            loss_d = self._lsgan(pred_fake, False) + self._lsgan(pred_real, True)
         loss_g = (10 * loss_l1 + loss_vgg + self.tvlambda * loss_tv) + (ce * self.ce_lambda + loss_g_gan * self.gan_lambda)
         self.opt_g.zero_grad(set_to_none=not self.scalers)
         self.opt_d.zero_grad(set_to_none=not self.scalers)
@@ -479,12 +515,20 @@ class Stage1Trainer(_GraphMixin, _TrainState, _LossScaling):
             self.reducers["G"].reduce()
         self._opt_step(self.opt_g, "G")
         del d_stale
+        if self.g_d_separate:
+            # train_condition.py:290-300: a train-mode tocg forward with the updated weights (BatchNorm running statistics move a second
+            # time), and D's fake input is the soft-max of its uncomposed segmentation
+            with torch.no_grad():
+                seg2 = autograd_tocg.tocg_forward_train(self.tocg, input1, input2)[1]
+            pred_fake = autograd_tocg.tocg_discriminator_forward_train(self.D, torch.cat((input1.detach(), input2.detach(), torch.softmax(seg2, 1)), 1))
+            pred_real = autograd_tocg.tocg_discriminator_forward_train(self.D, torch.cat((input1.detach(), input2.detach(), batch["parse"]), 1))
+            loss_d = self._lsgan(pred_fake, False) + self._lsgan(pred_real, True)
         self.opt_d.zero_grad(set_to_none=not self.scalers)
         self._backward(loss_d, "D")
         if "D" in self.reducers and self._explicit_reduce:
             self.reducers["D"].reduce()
         self._opt_step(self.opt_d, "D")
-        return {"loss_g": loss_g.detach(), "loss_d": loss_d.detach(), "l1": loss_l1.detach(), "vgg": loss_vgg.detach(), "ce": ce.detach()}
+        return {"loss_g": loss_g.detach(), "loss_d": loss_d.detach(), **out}
 
 
 def cross_entropy_ignore(logits, target, ignore_index=250):

@@ -217,6 +217,31 @@ size_t hrv_seg_iou_workspace_bytes(int32_t n, int32_t h, int32_t w);
 int hrv_seg_iou(const float* seg, int32_t k, const float* cm, const float* parse, int32_t n, int32_t h, int32_t w, float* iou,
                 void* workspace, size_t workspace_bytes, hrv_stream stream);
 
+/* The stage-1 flow TV loss, plain and edge-aware (train_condition.py:183-232, --edgeawaretv / --add_lasttv), in fp32 in either flavour.
+ * flows[i].flow: fp32 [n][h][w][2] contiguous (h, w >= 2).  With mask (fp32 [n][1][mh][mw]), m_i = F.interpolate(mask, (h, w),
+ * 'bilinear', align_corners=False), bit-identical to torch's CUDA kernel (the arithmetic of hrv_resize_bilinear_nhwc), and
+ *   e_y = exp(-150 |m_i[y+1][x] - m_i[y][x]|),  e_x = exp(-150 |m_i[y][x+1] - m_i[y][x]|)  (broadcast over the two flow channels);
+ *   terms[i] = edge_weight * (sum |D_y flow| e_y / Dy + sum |D_x flow| e_x / Dx) + plain_weight * (sum |D_y flow| / Dy + sum |D_x flow| / Dx)
+ * with Dy = n (h-1) w 2 and Dx = n h (w-1) 2 (the means).  Without mask, e = 1.  *loss = sum of terms[i] in order (terms: optional,
+ * nflows floats); mask_down (optional, with mask): nflows pointers that receive m_i as fp32 [n][h_i][w_i].  Per-block partial sums go
+ * to workspace slabs (hrv_flow_tv_workspace_bytes bytes) that a one-warp kernel adds in a fixed order: the same bits on every run.
+ * 1 <= nflows <= HRV_TV_MAX_FLOWS.
+ * hrv_flow_tv_bwd: from the device scalar *dloss, writes dflows[i] (fp32 [n][h_i][w_i][2], every element) and, with mask, dmask
+ * (fp32 [n][1][mh][mw], every element): through exp, |.| (sgn(0) = 0 for both |D flow| and |D m|) and the adjoint of the
+ * interpolation, gathered over the few output pixels that read each mask pixel, summed over i in order.  No atomics. */
+#define HRV_TV_MAX_FLOWS 5
+typedef struct hrv_tv_flow {
+  const float* flow;
+  int32_t h, w;
+  float edge_weight;  /* weight of the mask-weighted TV (the plain TV when mask is NULL) */
+  float plain_weight; /* weight of the plain TV of the same flow (--add_lasttv) */
+} hrv_tv_flow;
+size_t hrv_flow_tv_workspace_bytes(const hrv_tv_flow* flows, int32_t nflows, int32_t n);
+int hrv_flow_tv(const hrv_tv_flow* flows, int32_t nflows, int32_t n, const float* mask, int32_t mh, int32_t mw, float* loss, float* terms,
+                float* const* mask_down, void* workspace, size_t workspace_bytes, hrv_stream stream);
+int hrv_flow_tv_bwd(const hrv_tv_flow* flows, int32_t nflows, int32_t n, const float* mask, int32_t mh, int32_t mw, const float* dloss,
+                    float* const* dflows, float* dmask, void* workspace, size_t workspace_bytes, hrv_stream stream);
+
 /* bf16|f32 NHWC view -> fp32 NCHW contiguous [n][c][h][w]. */
 int hrv_nhwc_to_nchw(const hrv_tensor* src, float* dst, hrv_stream stream);
 
