@@ -14,7 +14,8 @@ RES_ADD, RES_GATE_RELU, RES_GATE_LRELU = 0, 1, 2
 
 EXPORTS = ["hrv_conv2d_fwd", "hrv_instnorm_stats", "hrv_instnorm_stats2", "hrv_instnorm_apply", "hrv_norm_apply_affine", "hrv_norm_bwd_reduce", "hrv_norm_bwd_apply", "hrv_act_bwd_bias", "hrv_conv2d_wgrad", "hrv_conv2d_wgrad_workspace_bytes", "hrv_nchw_to_nhwc", "hrv_nhwc_to_nchw",
            "hrv_space_to_depth", "hrv_avgpool3s2", "hrv_bilinear_up2_add", "hrv_flow_warp", "hrv_bilinear_up2_bwd", "hrv_flow_warp_bwd", "hrv_pack_conv_weight", "hrv_pack_conv_weight_tf32x2", "hrv_space_to_depth_bwd", "hrv_maxpool2_fwd", "hrv_maxpool2_bwd",
-           "hrv_avgpool3s2_bwd", "hrv_parse_blur_argmax", "hrv_gaussian_blur", "hrv_flow_warp_nchw", "hrv_onehot_u8", "hrv_im2col", "hrv_l1_sum", "hrv_l1_bwd",
+           "hrv_avgpool3s2_bwd", "hrv_parse_blur_argmax", "hrv_parse_blur_argmax_cm", "hrv_gaussian_blur", "hrv_flow_warp_nchw", "hrv_onehot_u8",
+           "hrv_onehot_u8_lut", "hrv_im2col", "hrv_l1_sum", "hrv_l1_bwd",
            "hrv_instnorm_stats_workspace_bytes", "hrv_instnorm_stats2_workspace_bytes", "hrv_norm_bwd_reduce_workspace_bytes",
            "hrv_norm_bwd_apply_workspace_bytes", "hrv_act_bwd_bias_ordered", "hrv_act_bwd_bias_ordered_workspace_bytes", "hrv_flow_warp_bwd_ordered",
            "hrv_flow_warp_bwd_ordered_workspace_bytes", "hrv_l1_sum_workspace_bytes", "hrv_flow_warp_nchw_bwd", "hrv_flow_warp_nchw_bwd_workspace_bytes",
@@ -131,7 +132,9 @@ def lib(dtype=None):
     L.hrv_maxpool2_bwd.argtypes = [TP, TP, TP, i32, vp]
     L.hrv_avgpool3s2_bwd.argtypes = [TP, TP, vp]
     L.hrv_parse_blur_argmax.argtypes = [vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_int32), i32, vp, vp, ctypes.c_uint32, vp, vp]
+    L.hrv_parse_blur_argmax_cm.argtypes = L.hrv_parse_blur_argmax.argtypes[:-1] + [vp, i32, i32, vp]
     L.hrv_onehot_u8.argtypes = [vp, i32, i32, i32, i32, vp, vp]
+    L.hrv_onehot_u8_lut.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_uint8), vp, vp]
     L.hrv_gaussian_blur.argtypes = [vp, i32, i32, i32, i32, f32, vp, vp]
     L.hrv_flow_warp_nchw.argtypes = [vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, vp, i32, i32, f32, f32, vp, vp, vp, vp, i32, vp]
     L.hrv_im2col.argtypes = [TP, TP, i32, i32, i32, vp]

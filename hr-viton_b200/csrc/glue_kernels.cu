@@ -130,14 +130,19 @@ __global__ void avgpool3s2_bwd_kernel(GView dy, GView dx, int G, long long total
 //   b_c   = 15x15 Gaussian(sigma 3), zero padding, separable                               train_generator.py:154,247
 //   k     = argmax_c b_c  (first maximum)                                                  train_generator.py:248
 // outputs: idx (n,H,W) int64 and/or onehot (n,groups,H,W) fp32 with onehot[group_of[k]] = 1   train_generator.py:251-273
+// cm (optional, (n,1,h,w) fp32 at the scores' resolution): the cloth-mask composition of train_generator.py:218-229 / test_generator.py
+// :163-176, seg_cm_channel *= cm (mode 1, 'warp_grad') or *= (cm > 0.5) (mode 2, 'detach'), applied to each low-resolution tap before
+// the interpolation with a rounded multiply (no FMA contraction with the weights): the torch product followed by the cm-less kernel.
+__device__ __forceinline__ float cm_factor(float cm, int mode) { return mode == 2 ? (cm > 0.5f ? 1.f : 0.f) : cm; }
 constexpr int kTile = 32, kHalo = 7, kU = kTile + 2 * kHalo;  // 46
 struct ParseArgs {
   const float* seg;
+  const float* cm;
   long long* idx;
   float* onehot;
   float* overlap;       // optional (n,1,H,W): sum over the classes in occl_mask of softmax_c(blurred scores)  (remove_overlap's operand)
   unsigned occl_mask;
-  int n, C, h, w, H, W, groups;
+  int n, C, h, w, H, W, groups, cm_channel, cm_mode;
   float sy, sx;
   float g[15];
   int group_of[32];
@@ -153,6 +158,7 @@ __global__ void __launch_bounds__(256) parse_blur_argmax_kernel(const __grid_con
   float sm_all[4] = {0.f, 0.f, 0.f, 0.f}, sm_sel[4] = {0.f, 0.f, 0.f, 0.f};  // online softmax sums relative to the running maximum `best`
   for (int c = 0; c < a.C; ++c) {
     const float* s = a.seg + ((long long)n * a.C + c) * a.h * a.w;
+    const float* m = (a.cm && c == a.cm_channel) ? a.cm + (long long)n * a.h * a.w : nullptr;
     for (int i = tid; i < kU * kU; i += 256) {
       const int uy = i / kU, ux = i - uy * kU;
       const int Y = ty0 + uy - kHalo, X = tx0 + ux - kHalo;
@@ -162,7 +168,13 @@ __global__ void __launch_bounds__(256) parse_blur_argmax_kernel(const __grid_con
         const int y0 = (int)fy, x0 = (int)fx;
         const int y1 = min(y0 + 1, a.h - 1), x1 = min(x0 + 1, a.w - 1);
         const float ly = fy - (float)y0, lx = fx - (float)x0;
-        const float v00 = __ldg(s + y0 * a.w + x0), v01 = __ldg(s + y0 * a.w + x1), v10 = __ldg(s + y1 * a.w + x0), v11 = __ldg(s + y1 * a.w + x1);
+        float v00 = __ldg(s + y0 * a.w + x0), v01 = __ldg(s + y0 * a.w + x1), v10 = __ldg(s + y1 * a.w + x0), v11 = __ldg(s + y1 * a.w + x1);
+        if (m) {
+          v00 = __fmul_rn(v00, cm_factor(__ldg(m + y0 * a.w + x0), a.cm_mode));
+          v01 = __fmul_rn(v01, cm_factor(__ldg(m + y0 * a.w + x1), a.cm_mode));
+          v10 = __fmul_rn(v10, cm_factor(__ldg(m + y1 * a.w + x0), a.cm_mode));
+          v11 = __fmul_rn(v11, cm_factor(__ldg(m + y1 * a.w + x1), a.cm_mode));
+        }
         v = (1.f - ly) * ((1.f - lx) * v00 + lx * v01) + ly * ((1.f - lx) * v10 + lx * v11);
       }
       U[uy][ux] = v;
@@ -426,12 +438,18 @@ __global__ void __launch_bounds__(256) resize_adjoint_cols_kernel(const float2* 
 
 // ---------------------------------------------------------------------------------------------- label map -> one-hot planes
 // Input feeding (SURVEY.md 8f N4; cp_dataset.py:150-172 builds the 13-channel one-hot parse map on the CPU and ships it as fp32):
-// the host ships ONE byte per pixel, this kernel expands it on the device.  out[n,c,p] = (label[n,p] == c).  thread = pixel.
-__global__ void __launch_bounds__(256) onehot_u8_kernel(const unsigned char* __restrict__ lab, float* __restrict__ out, int C, long long hw, long long npix) {
+// the host ships ONE byte per pixel, this kernel expands it on the device.  out[n,c,p] = (class(label[n,p]) == c), class = lut.v[]
+// (LUT) or the identity.  thread = pixel.
+struct ClassLut {
+  unsigned char v[256];
+};
+template <bool LUT>
+__global__ void __launch_bounds__(256) onehot_u8_kernel(const unsigned char* __restrict__ lab, float* __restrict__ out, int C, long long hw, long long npix,
+                                                        const __grid_constant__ ClassLut lut) {
   const long long pix = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (pix >= npix) return;
   const long long n = pix / hw, p = pix - n * hw;
-  const int l = (int)__ldg(lab + pix);
+  const int l = LUT ? (int)lut.v[__ldg(lab + pix)] : (int)__ldg(lab + pix);
   float* o = out + n * C * hw + p;
   for (int c = 0; c < C; ++c) o[(long long)c * hw] = (c == l) ? 1.f : 0.f;
 }
@@ -686,16 +704,18 @@ extern "C" int hrv_avgpool3s2_bwd(const hrv_tensor* dy, const hrv_tensor* dx, hr
   return launched("avgpool3s2_bwd");
 }
 
-extern "C" int hrv_parse_blur_argmax(const float* seg, int32_t n, int32_t c, int32_t h, int32_t w, int32_t H, int32_t W,
-                                     const int32_t* group_of, int32_t groups, int64_t* idx, float* onehot, uint32_t occl_mask,
-                                     float* overlap, hrv_stream stream) {
+extern "C" int hrv_parse_blur_argmax_cm(const float* seg, int32_t n, int32_t c, int32_t h, int32_t w, int32_t H, int32_t W,
+                                        const int32_t* group_of, int32_t groups, int64_t* idx, float* onehot, uint32_t occl_mask,
+                                        float* overlap, const float* cm, int32_t cm_channel, int32_t mode, hrv_stream stream) {
   if (!seg || (!idx && !onehot && !overlap) || n < 1 || c < 1 || c > 32 || h < 1 || w < 1 || H < 1 || W < 1)
     return set_error(HRV_EINVAL, "parse_blur_argmax: bad arguments (c must be <= 32)");
   if (onehot && (!group_of || groups < 1)) return set_error(HRV_EINVAL, "parse_blur_argmax: onehot needs group_of / groups");
+  if (cm && (mode < 1 || mode > 2 || cm_channel < 0 || cm_channel >= c))
+    return set_error(HRV_EINVAL, "parse_blur_argmax: cm needs mode 1 (multiply by cm) or 2 (by cm > 0.5) and 0 <= cm_channel < %d", c);
   ParseArgs a;
   memset(&a, 0, sizeof(a));
-  a.seg = seg; a.idx = (long long*)idx; a.onehot = onehot; a.overlap = overlap; a.occl_mask = occl_mask;
-  a.n = n; a.C = c; a.h = h; a.w = w; a.H = H; a.W = W; a.groups = groups;
+  a.seg = seg; a.cm = cm; a.idx = (long long*)idx; a.onehot = onehot; a.overlap = overlap; a.occl_mask = occl_mask;
+  a.n = n; a.C = c; a.h = h; a.w = w; a.H = H; a.W = W; a.groups = groups; a.cm_channel = cm_channel; a.cm_mode = mode;
   a.sy = (float)h / (float)H; a.sx = (float)w / (float)W;
   double g[15], sum = 0;
   for (int k = 0; k < 15; ++k) { g[k] = (double)expf(-(float)((k - 7) * (k - 7)) / 18.f); sum += g[k]; }
@@ -712,11 +732,29 @@ extern "C" int hrv_parse_blur_argmax(const float* seg, int32_t n, int32_t c, int
   return launched("parse_blur_argmax");
 }
 
-extern "C" int hrv_onehot_u8(const uint8_t* labels, int32_t n, int32_t classes, int32_t h, int32_t w, float* out, hrv_stream stream) {
+extern "C" int hrv_parse_blur_argmax(const float* seg, int32_t n, int32_t c, int32_t h, int32_t w, int32_t H, int32_t W,
+                                     const int32_t* group_of, int32_t groups, int64_t* idx, float* onehot, uint32_t occl_mask,
+                                     float* overlap, hrv_stream stream) {
+  return hrv_parse_blur_argmax_cm(seg, n, c, h, w, H, W, group_of, groups, idx, onehot, occl_mask, overlap, nullptr, 0, 0, stream);
+}
+
+extern "C" int hrv_onehot_u8_lut(const uint8_t* labels, int32_t n, int32_t classes, int32_t h, int32_t w, const uint8_t* lut, float* out,
+                                 hrv_stream stream) {
   if (!labels || !out || n < 1 || classes < 1 || h < 1 || w < 1) return set_error(HRV_EINVAL, "onehot_u8: bad arguments");
   const long long hw = (long long)h * w, npix = hw * n;
-  onehot_u8_kernel<<<nblocks(npix, 256), 256, 0, (cudaStream_t)stream>>>(labels, out, classes, hw, npix);
+  ClassLut t;
+  memset(&t, 0, sizeof(t));
+  if (lut) {
+    memcpy(t.v, lut, sizeof(t.v));
+    onehot_u8_kernel<true><<<nblocks(npix, 256), 256, 0, (cudaStream_t)stream>>>(labels, out, classes, hw, npix, t);
+  } else {
+    onehot_u8_kernel<false><<<nblocks(npix, 256), 256, 0, (cudaStream_t)stream>>>(labels, out, classes, hw, npix, t);
+  }
   return launched("onehot_u8");
+}
+
+extern "C" int hrv_onehot_u8(const uint8_t* labels, int32_t n, int32_t classes, int32_t h, int32_t w, float* out, hrv_stream stream) {
+  return hrv_onehot_u8_lut(labels, n, classes, h, w, nullptr, out, stream);
 }
 
 extern "C" int hrv_gaussian_blur(const float* src, int32_t planes, int32_t h, int32_t w, int32_t ksize, float sigma, float* dst,

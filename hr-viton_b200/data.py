@@ -21,7 +21,7 @@ import torch
 from PIL import Image, ImageDraw
 
 from . import capi, jpeg
-from .train_step import BatchFeeder
+from .train_step import GROUP_OF_13, LABELS7, BatchFeeder
 
 PRECISION_BITS = 22  # Pillow's fixed-point precision for 8-bit resampling
 # cp_dataset.py:150-164: group g of the 13-channel parse map collects these labels of the 20-label parse
@@ -41,7 +41,8 @@ PAIRED_KEYS = ("cloth", "cloth_mask")  # {'paired': ..., 'unpaired': ...} in the
 # the source planes a key is computed from
 _NEEDS = {"cloth": ("cloth",), "cloth_mask": ("cloth_mask",), "image": ("image",), "pose": ("pose",), "densepose": ("densepose",),
           "parse_agnostic": ("parse_agnostic",), "parse": ("parse",), "pcm": ("parse",), "parse_onehot": ("parse",),
-          "parse_cloth": ("image", "parse"), "agnostic": ("image", "parse", "keypoints")}
+          "parse_cloth": ("image", "parse"), "agnostic": ("image", "parse", "keypoints"), "gen_parse": ("parse",)}
+GEN_PARSE_NC = len(LABELS7)  # gen_parse: the 13-channel parse regrouped into the generator's 7 classes (train_generator.py:250-273)
 _RGB_ORDER = ("image", "cloth", "pose", "densepose")
 
 
@@ -200,7 +201,7 @@ class VitonHDDataset(torch.utils.data.Dataset):
         self.keys = tuple(TRAIN_KEYS if keys is None else keys)
         unknown = [k for k in self.keys if k not in _NEEDS]
         if unknown:
-            raise ValueError("unknown keys %s (known: %s)" % (unknown, ", ".join(TRAIN_KEYS)))
+            raise ValueError("unknown keys %s (known: %s)" % (unknown, ", ".join(_NEEDS)))
         self.fine_height, self.fine_width = int(fine_height), int(fine_width)
         self.data_path = osp.join(dataroot, datamode)
         self.im_names, self.c_unpaired = [], []
@@ -537,9 +538,9 @@ class VitonHDLoader(BatchFeeder):
             jpeg.raise_errors(codes.numpy(), names)
 
     def consume(self, out):
-        unknown = [k for k in out if k not in TRAIN_KEYS]
+        unknown = [k for k in out if k not in _NEEDS]
         if unknown:  # a graph input the loader does not write would keep stale data
-            raise KeyError("consume(): %s are not keys of a VITON-HD batch (%s)" % (unknown, ", ".join(TRAIN_KEYS)))
+            raise KeyError("consume(): %s are not keys of a VITON-HD batch (%s)" % (unknown, ", ".join(_NEEDS)))
         missing = [k for k in out if k not in self.keys]
         if missing:
             raise KeyError("consume(): the loader was built without keys %s (keys=%s)" % (missing, self.keys))
@@ -598,6 +599,8 @@ class VitonHDLoader(BatchFeeder):
                         getattr(dst, k)[s] = tt.data_ptr()
             elif k in ONEHOT_KEYS:
                 self._check_out(k, t, SEMANTIC_NC)
+            elif k == "gen_parse":
+                self._check_out(k, t, GEN_PARSE_NC)
             elif k in ("image", "pose", "densepose", "agnostic", "parse_cloth"):
                 self._check_out(k, t, 3)
                 setattr(dst, k, t.data_ptr())
@@ -609,6 +612,8 @@ class VitonHDLoader(BatchFeeder):
         for k in ONEHOT_KEYS:
             if k in out:
                 ops.onehot_u8(lab[ds.lab_planes.index(k)], SEMANTIC_NC, out=out[k])
+        if "gen_parse" in out:  # argmax -> scatter_ -> 7-group sum of the one-hot 13-plane map: its label through the group table
+            ops.onehot_u8(lab[ds.lab_planes.index("parse")], GEN_PARSE_NC, lut=GROUP_OF_13, out=out["gen_parse"])
 
     def _check_out(self, key, t, c):
         want = (self.batch_size, c, self.dataset.fine_height, self.dataset.fine_width)
@@ -619,7 +624,7 @@ class VitonHDLoader(BatchFeeder):
     def empty_batch(self):
         """A dict of device tensors for one batch of this loader's keys (cloth / cloth_mask per cloth set)."""
         ds, n = self.dataset, self.batch_size
-        chans = {"cloth_mask": 1, "pcm": 1, "parse_onehot": 1, "parse": SEMANTIC_NC, "parse_agnostic": SEMANTIC_NC}
+        chans = {"cloth_mask": 1, "pcm": 1, "parse_onehot": 1, "parse": SEMANTIC_NC, "parse_agnostic": SEMANTIC_NC, "gen_parse": GEN_PARSE_NC}
 
         def new(k):
             return torch.empty((n, chans.get(k, 3), ds.fine_height, ds.fine_width), dtype=torch.float32, device=self.device)

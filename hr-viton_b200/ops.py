@@ -568,12 +568,24 @@ def grad_unscale_check(grads, inv_scale, found_inf, table=None):
     return table
 
 
-def parse_blur_argmax(seg, size, group_of=None, groups=0, want_idx=True, overlap_classes=None):
+def parse_blur_argmax(seg, size, group_of=None, groups=0, want_idx=True, overlap_classes=None, cm=None, cm_channel=3,
+                      composition="warp_grad"):
     """seg (n,c,h,w) fp32 cuda -> (idx (n,1,H,W) int64 | None, onehot (n,groups,H,W) fp32 | None[, overlap (n,1,H,W)]);
-    hrv_parse_blur_argmax.  overlap_classes: class ids whose softmax (over the blurred scores) is summed into `overlap`."""
+    hrv_parse_blur_argmax.  overlap_classes: class ids whose softmax (over the blurred scores) is summed into `overlap`.
+    cm: (n,1,h,w) fp32 cuda, the cloth-mask composition of the scores first (channel cm_channel multiplied by cm for 'warp_grad',
+    by (cm > 0.5) for 'detach'; 'no_composition' or cm=None: none), as seg_softmax_cat composes."""
     assert seg.is_cuda and seg.dtype == torch.float32
+    if composition not in SEG_CAT_MODES:
+        raise ValueError("composition must be one of %s, got %r" % ("/".join(SEG_CAT_MODES), composition))
+    mode = 0 if cm is None else SEG_CAT_MODES[composition]
     seg = seg.contiguous()
     n, c, h, w = seg.shape
+    if mode:
+        if not (cm.is_cuda and cm.dtype == torch.float32 and tuple(cm.shape) == (n, 1, h, w)):
+            raise ValueError("parse_blur_argmax: cm must be a CUDA float32 %s tensor, got %s %s" % ((n, 1, h, w), cm.dtype, tuple(cm.shape)))
+        cm = cm.contiguous()
+    else:
+        cm = None
     H, W = size
     idx = torch.empty((n, 1, H, W), dtype=torch.int64, device=seg.device) if want_idx else None
     onehot = torch.empty((n, groups, H, W), dtype=torch.float32, device=seg.device) if group_of is not None else None
@@ -583,22 +595,29 @@ def parse_blur_argmax(seg, size, group_of=None, groups=0, want_idx=True, overlap
     for k in (overlap_classes or ()):
         mask |= 1 << int(k)
     with _Timed("glue", 0.0, label="parse_blur_argmax"):
-        capi.check(capi.lib().hrv_parse_blur_argmax(seg.data_ptr(), n, c, h, w, H, W, garr, groups, _p(idx), _p(onehot), mask, _p(overlap), _stream()),
-                   "parse_blur_argmax")
+        capi.check(capi.lib().hrv_parse_blur_argmax_cm(seg.data_ptr(), n, c, h, w, H, W, garr, groups, _p(idx), _p(onehot), mask, _p(overlap),
+                                                    _p(cm), cm_channel, mode, _stream()), "parse_blur_argmax")
     return (idx, onehot, overlap) if overlap_classes else (idx, onehot)
 
 
-def onehot_u8(labels, classes, out=None):
+def onehot_u8(labels, classes, lut=None, out=None):
     """(N,1,H,W) or (N,H,W) uint8 label map (cuda) -> (N,classes,H,W) fp32 one-hot planes (hrv_onehot_u8): the device half of the
-    input feeding — the host ships one byte per pixel instead of `classes` floats (cp_dataset.py:150-172)."""
+    input feeding — the host ships one byte per pixel instead of `classes` floats (cp_dataset.py:150-172).  lut: a sequence of
+    class ids indexed by label (at most 256; labels beyond it, and ids >= classes, set no channel), e.g. train_step.GROUP_OF_13 for
+    the 13 -> 7 regrouping of train_generator.py:261-273; None: class = label."""
     assert labels.is_cuda and labels.dtype == torch.uint8
     labels = labels.contiguous()
     n, h, w = labels.shape[0], labels.shape[-2], labels.shape[-1]
     if out is None:
         out = torch.empty((n, classes, h, w), dtype=torch.float32, device=labels.device)
     assert out.is_contiguous() and out.shape == (n, classes, h, w)
+    table = None
+    if lut is not None:
+        if len(lut) > 256 or any(not 0 <= int(v) < 256 for v in lut):
+            raise ValueError("onehot_u8: lut must hold at most 256 class ids in [0, 255]")
+        table = (ctypes.c_uint8 * 256)(*([int(v) for v in lut] + [255] * (256 - len(lut))))
     with _Timed("glue", 0.0, label="onehot_u8"):
-        capi.check(capi.lib().hrv_onehot_u8(labels.data_ptr(), n, classes, h, w, out.data_ptr(), _stream()), "onehot_u8")
+        capi.check(capi.lib().hrv_onehot_u8_lut(labels.data_ptr(), n, classes, h, w, table, out.data_ptr(), _stream()), "onehot_u8")
     return out
 
 

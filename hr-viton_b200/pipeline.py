@@ -106,26 +106,25 @@ def tryon_forward(tocg, generator, inputs, opt=None, occlusion=True, clothmask_c
         input1 = torch.cat([F.interpolate(clothes, size=(256, 192), mode="bilinear"), F.interpolate(pre_cm, size=(256, 192), mode="nearest")], 1)
         input2 = torch.cat([F.interpolate(parse_agnostic, size=(256, 192), mode="nearest"), F.interpolate(densepose, size=(256, 192), mode="bilinear")], 1)
         flow_list, fake_segmap, _, warped_cm = tocg(input1, input2) if opt is None else tocg(opt, input1, input2)
+        # test_generator.py:163-176: the cloth-mask composition of the scores, inside the kernel that makes the parse map
+        comp = dict(cm=None if clothmask_composition == "no_composition" else warped_cm.float(), composition=clothmask_composition)
         if discriminator is not None:
             # the kernel that builds the discriminator's input also writes the composed scores the parse map is made of
-            composed = clothmask_composition != "no_composition"
-            a = ops.seg_softmax_cat(input1, input2, fake_segmap.float(), cm=warped_cm if composed else None,
-                                    composition=clothmask_composition, want_seg=composed)
+            composed = comp["cm"] is not None
+            a = ops.seg_softmax_cat(input1, input2, fake_segmap.float(), cm=comp["cm"], composition=clothmask_composition, want_seg=composed)
             if composed:
                 a, fake_segmap = a
+                comp["cm"] = None
             l = d_logit(discriminator.forward_act(a))
             score = l / (1 - l) / norm_const
-        elif clothmask_composition != "no_composition":
-            cm = (warped_cm > 0.5).float() if clothmask_composition == "detach" else warped_cm   # test_generator.py:163-176
-            fake_segmap = torch.cat([fake_segmap[:, :3], fake_segmap[:, 3:4] * cm, fake_segmap[:, 4:]], 1)
         n, _, ih, iw = clothes.shape
         div = ((96 - 1.0) / 2.0, (128 - 1.0) / 2.0)
         if occlusion:
             _, parse, overlap = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False,
-                                                      overlap_classes=OCCLUSION_CLASSES)
+                                                      overlap_classes=OCCLUSION_CLASSES, **comp)
             warped_cloth, _, _ = ops.flow_warp_nchw(flow_list[-1], clothes.float(), (ih, iw), div, mask=pre_cm, overlap=overlap, composite=True)
         else:
-            _, parse = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False)
+            _, parse = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False, **comp)
             warped_cloth, _ = ops.flow_warp_nchw(flow_list[-1], clothes.float(), (ih, iw), div)
         output = generator(torch.cat((agnostic, densepose, warped_cloth), 1), parse)
     return (output, warped_cloth, parse) if discriminator is None else (output, warped_cloth, parse, score)

@@ -26,11 +26,15 @@ MODEL_FILES = {"stage1": {"tocg": ("tocg_step_%06d.pth", "tocg_final.pth"), "D":
 STATE_FILES = ("state_step_%06d.pth", "state_final.pth")
 LPIPS_SAMPLES = 500  # train_generator.py:620: Subset(test_dataset, np.arange(500))
 EVAL_KEYS = ("cloth", "cloth_mask", "agnostic", "densepose", "parse_agnostic", "image")
+EVAL_GT_KEYS = train_step.GT_KEYS  # --GT: the ground-truth parse and cloth (train_generator.py:570-572)
 VAL_SAMPLES = 2000  # train_condition.py:485: Subset(test_dataset, np.arange(2000))
 VAL_KEYS = ("cloth", "cloth_mask", "parse_agnostic", "densepose", "parse")
 # the stage-1 loss options a resumed run must share, with the values a state file that does not record them was trained with
 STAGE1_OPTIONS = {"edgeawaretv": "no_edge", "add_lasttv": False, "clothmask_composition": "warp_grad", "no_gan_loss": False,
                   "g_d_separate": False, "tvlambda": 2.0, "ce_lambda": 10.0, "gan_lambda": 1.0}
+# the same for stage 2 (train_generator.py); no_ganFeat_loss is the discriminator's option, as in the reference
+STAGE2_OPTIONS = {"gt": False, "clothmask_composition": "warp_grad", "no_vgg_loss": False, "no_ganFeat_loss": False, "lambda_feat": 10.0,
+                  "lambda_vgg": 10.0}
 
 
 def lr_lambda(k, load_step, keep_step, decay_step, interval=1000):
@@ -129,13 +133,16 @@ class TrainRun:
 
     # ---------------------------------------------------------------- files
     def config(self):
-        """What a resumed run must share with the run it continues beyond the schedule: both base learning rates, --occlusion, for
-        stage 1 the loss options of STAGE1_OPTIONS and, for stage 2, the frozen tocg (a SHA-256 of its state, so another --tocg_checkpoint
-        file with the same weights is accepted)."""
+        """What a resumed run must share with the run it continues beyond the schedule: both base learning rates, --occlusion, the loss
+        options of STAGE1_OPTIONS / STAGE2_OPTIONS and, for stage 2 with a tocg, the frozen tocg (a SHA-256 of its state, so another
+        --tocg_checkpoint file with the same weights is accepted)."""
         cfg = {"base_lr": dict(self.trainer.base_lr), "occlusion": getattr(self.trainer, "occlusion", None)}
         if self.stage == "stage1":
             cfg.update((k, getattr(self.trainer, k, v)) for k, v in STAGE1_OPTIONS.items())  # a trainer without them trains the defaults
         if self.stage == "stage2":
+            cfg.update((k, getattr(self.trainer, k, v)) for k, v in STAGE2_OPTIONS.items())
+            cfg["no_ganFeat_loss"] = bool(getattr(self.trainer.D, "no_ganFeat_loss", False))
+        if self.stage == "stage2" and self.trainer.tocg is not None:
             h = hashlib.sha256()
             for k, v in self.trainer.tocg.state_dict().items():
                 h.update(k.encode())
@@ -180,7 +187,7 @@ class TrainRun:
             if self.stage == "stage2" and st[k] != getattr(self, k):
                 raise ValueError("%s was saved with %s=%r, this run has %r" % (path, k, st[k], getattr(self, k)))
         cfg = self.config()
-        saved = dict(STAGE1_OPTIONS) if self.stage == "stage1" else {}  # a state file written before the options were recorded
+        saved = dict(STAGE1_OPTIONS if self.stage == "stage1" else STAGE2_OPTIONS)  # a state file written before the options were recorded
         saved.update(st["config"])
         for k, v in saved.items():
             if cfg.get(k) != v:
@@ -211,7 +218,8 @@ class TrainRun:
         n, h, w, dev = self.loader.batch_size, ds.fine_height, ds.fine_width, self.loader.device
         if self.stage == "stage2":
             self.trainer.set_lr_factor(self.factor())
-            self.trainer.capture(train_step.synthetic_batch(n, h, w, dev), h, w, rollback=True)
+            synthetic = train_step.synthetic_batch_gt if getattr(self.trainer, "gt", False) else train_step.synthetic_batch
+            self.trainer.capture(synthetic(n, h, w, dev), h, w, rollback=True)
         else:
             b = train_step.synthetic_batch_stage1(n, h, w, dev)
             self.trainer.capture({k: b[k] for k in data.STAGE1_KEYS}, rollback=True)
@@ -249,9 +257,11 @@ class TrainRun:
 
     def evaluate(self):
         """train_generator.py:480-584: the try-ons of the first LPIPS_SAMPLES test samples (batch 1, paired cloth) through
-        pipeline.TryOnGraph, each scored by lpips(T2(image), T2(output)) with T2 = transforms.Resize((128, 128)), summed on the device
-        in sample order and divided by the count.  The try-on noise is drawn from a fork of the CUDA generator, so evaluations
-        leave the training's random stream (and a resumed run) unchanged; the reference draws it from the training stream."""
+        pipeline.TryOnGraph with the trainer's cloth-mask composition (under --GT: the generator alone through pipeline.GeneratorGraph,
+        on the ground-truth parse and cloth of a test loader with keys EVAL_GT_KEYS), each scored by lpips(T2(image), T2(output)) with
+        T2 = transforms.Resize((128, 128)), summed on the device in sample order and divided by the count.  The try-on noise is drawn
+        from a fork of the CUDA generator, so evaluations leave the training's random stream (and a resumed run) unchanged; the
+        reference draws it from the training stream."""
         from torchvision.transforms import transforms
 
         from . import pipeline
@@ -259,16 +269,22 @@ class TrainRun:
         n = min(self.lpips_samples, len(test_loader.dataset))
         T2 = transforms.Compose([transforms.Resize((128, 128))])
         G, tocg = self.trainer.G, self.trainer.tocg
+        gt = getattr(self.trainer, "gt", False)
         G.eval()
         try:
             with torch.random.fork_rng(devices=[test_loader.device]), torch.no_grad():
                 if self._tryon is None:
-                    self._tryon = pipeline.TryOnGraph(tocg, G, occlusion=self.trainer.occlusion)
+                    self._tryon = (pipeline.GeneratorGraph(G) if gt else
+                                   pipeline.TryOnGraph(tocg, G, occlusion=self.trainer.occlusion,
+                                                       clothmask_composition=getattr(self.trainer, "clothmask_composition", "warp_grad")))
                 test_loader.start_at(0, 0)
                 total = 0.0
                 for _ in range(n):
                     b = test_loader.next_batch()
-                    out = self._tryon({k: b[k] for k in EVAL_KEYS if k != "image"})[0]
+                    if gt:  # train_generator.py:569-576
+                        out = self._tryon(torch.cat((b["agnostic"], b["densepose"], b["parse_cloth"]), 1), b["gen_parse"])
+                    else:
+                        out = self._tryon({k: b[k] for k in EVAL_KEYS if k != "image"})[0]
                     total += lpips.forward(T2(b["image"]), T2(out))
                 value = float(total / n)
         finally:
@@ -328,7 +344,7 @@ def parse_args(stage, argv=None):
     p.add_argument("--fine_width", type=int, default=768 if s2 else 192)
     p.add_argument("--fine_height", type=int, default=1024 if s2 else 256)
     p.add_argument("--checkpoint_dir", default="checkpoints")
-    p.add_argument("--tocg_checkpoint", default=None if s2 else "", required=s2)
+    p.add_argument("--tocg_checkpoint", default=None if s2 else "")
     p.add_argument("--display_count", type=int, default=100)
     p.add_argument("--save_count", type=int, default=10000)
     p.add_argument("--load_step", type=int, default=0)
@@ -344,6 +360,12 @@ def parse_args(stage, argv=None):
         p.add_argument("--decay_step", type=int, default=100000)
         p.add_argument("--lpips_count", type=int, default=1000)
         p.add_argument("--lr_interval", type=int, default=1000, help="steps between scheduler steps (the reference's 1000)")
+        p.add_argument("--GT", action="store_true", help="train on the ground-truth parse and cloth: no tocg")
+        p.add_argument("--clothmask_composition", choices=train_step.CLOTHMASK_COMPOSITIONS, default="warp_grad")
+        p.add_argument("--no_ganFeat_loss", action="store_true", help="no discriminator feature-matching term")
+        p.add_argument("--no_vgg_loss", action="store_true", help="no VGG term")
+        p.add_argument("--lambda_feat", type=float, default=10.0)
+        p.add_argument("--lambda_vgg", type=float, default=10.0)
     else:
         p.add_argument("--val_count", type=int, default=None, help="steps between validations (segmentation IoU); default: none")
         p.add_argument("--edgeawaretv", choices=train_step.EDGEAWARETV, default="no_edge", help="edge-aware flow TV")
@@ -374,12 +396,19 @@ def parse_args(stage, argv=None):
         p.error("--load_step %d leaves nothing to train (the run ends at step %d)" % (opt.load_step, end))
     if opt.G_lr <= 0 or opt.D_lr <= 0:
         p.error("--G_lr and --D_lr must be positive")
+    if s2 and opt.GT:  # each of these acts on the tocg, which a --GT run does not have
+        for flag, given in (("--tocg_checkpoint", opt.tocg_checkpoint is not None), ("--occlusion", opt.occlusion),
+                            ("--clothmask_composition", opt.clothmask_composition != "warp_grad")):
+            if given:
+                p.error("%s acts on the condition generator, which a --GT run does not have" % flag)
+    elif s2 and opt.tocg_checkpoint is None:
+        p.error("the following arguments are required: --tocg_checkpoint (unless --GT)")
     if opt.resume is not None and opt.load_step:
         p.error("--resume takes the step from the state file; --load_step starts a new run")
     want = data.resized_size(1024, 768, opt.fine_width)
     if (opt.fine_height, opt.fine_width) != want:
         p.error("--fine_height %d: VITON-HD's 1024x768 images resize to %dx%d at --fine_width %d" % (opt.fine_height, want[0], want[1], opt.fine_width))
-    for k in ("dataroot",) + (("tocg_checkpoint",) if s2 else ()) + (("test_dataroot",) if not s2 and opt.val_count else ()):
+    for k in ("dataroot",) + (("tocg_checkpoint",) if s2 and not opt.GT else ()) + (("test_dataroot",) if not s2 and opt.val_count else ()):
         if not os.path.exists(getattr(opt, k)):
             p.error("--%s %s does not exist" % (k, getattr(opt, k)))
     if opt.resume is not None and not os.path.isfile(opt.resume):
@@ -392,6 +421,12 @@ def stage1_options(opt):
     return {"edgeawaretv": opt.edgeawaretv, "add_lasttv": opt.add_lasttv, "clothmask_composition": opt.clothmask_composition,
             "no_gan_loss": opt.no_GAN_loss, "g_d_separate": opt.G_D_seperate, "tvlambda": opt.tvlambda, "ce_lambda": opt.CElamda,
             "gan_lambda": opt.GANlambda}
+
+
+def stage2_options(opt):
+    """The keys of STAGE2_OPTIONS of parsed stage-2 flags (no_ganFeat_loss goes to the discriminator, the rest to Stage2Trainer)."""
+    return {"gt": opt.GT, "clothmask_composition": opt.clothmask_composition, "no_vgg_loss": opt.no_vgg_loss,
+            "no_ganFeat_loss": opt.no_ganFeat_loss, "lambda_feat": opt.lambda_feat, "lambda_vgg": opt.lambda_vgg}
 
 
 def build(opt, log=print):
@@ -420,21 +455,24 @@ def build(opt, log=print):
     loss_scale = "dynamic" if opt.fp16 else None
     torch.manual_seed(opt.seed)
     s2 = opt.stage == "stage2"
+    gt = s2 and opt.GT
+    s2_opts = stage2_options(opt) if s2 else {}
     topt = types.SimpleNamespace(warp_feature="T1", out_layer="relu", cuda=True)
-    tocg = networks.ConditionGenerator(topt, 4, 16, 13, ngf=96, norm_layer=torch.nn.BatchNorm2d)
+    tocg = None if gt else networks.ConditionGenerator(topt, 4, 16, 13, ngf=96, norm_layer=torch.nn.BatchNorm2d)
     if opt.tocg_checkpoint:
         networks.load_checkpoint(tocg, opt.tocg_checkpoint, topt)
-    vgg = networks.Vgg19().to(dev).eval()
+    vgg = None if s2_opts.get("no_vgg_loss") else networks.Vgg19().to(dev).eval()
     if s2:
         import network_generator
         gopt = types.SimpleNamespace(norm_G="spectralaliasinstance", gen_semantic_nc=7, ngf=64, num_upsampling_layers="most",
                                      fine_height=opt.fine_height, fine_width=opt.fine_width, cuda=True, ndf=64, norm_D="spectralinstance",
-                                     n_layers_D=3, num_D=2, no_ganFeat_loss=False, init_type="xavier", init_variance=0.02)
+                                     n_layers_D=3, num_D=2, no_ganFeat_loss=s2_opts.pop("no_ganFeat_loss"), init_type="xavier",
+                                     init_variance=0.02)
         G = network_generator.SPADEGenerator(gopt, 9).to(dev)
         G.init_weights(gopt.init_type, gopt.init_variance)
         D = network_generator.MultiscaleDiscriminator(gopt).to(dev)
         D.init_weights(gopt.init_type, gopt.init_variance)  # utils.create_network
-        tocg = tocg.to(dev).eval()
+        tocg = None if gt else tocg.to(dev).eval()
         trained = (G.train(), D.train())
     else:
         if world > 1:  # every rank normalises over the global batch and holds the same running statistics (INTEGRATION.md)
@@ -445,23 +483,24 @@ def build(opt, log=print):
     reducers = {}
     if world > 1:
         for m in (tocg,) + trained:
-            ddp.broadcast_module_state(m)
+            if m is not None:
+                ddp.broadcast_module_state(m)
         reducers = {"G": ddp.GradBucketReducer(list(trained[0].parameters())), "D": ddp.GradBucketReducer(list(trained[1].parameters()))}
     torch.cuda.manual_seed(opt.seed * 1000 + rank)  # per-rank noise and dropout
     if s2:
         trainer = train_step.Stage2Trainer(tocg, G, D, vgg, g_lr=opt.G_lr, d_lr=opt.D_lr, reducers=reducers, occlusion=opt.occlusion,
-                                           loss_scale=loss_scale, tensor_lr=True)
+                                           loss_scale=loss_scale, tensor_lr=True, **s2_opts)
     else:
         trainer = train_step.Stage1Trainer(tocg, D, vgg, lr=opt.G_lr, d_lr=opt.D_lr, occlusion=opt.occlusion, reducers=reducers,
                                            loss_scale=loss_scale, **stage1_options(opt))
-    keys = data.STAGE2_KEYS if s2 else data.STAGE1_KEYS
+    keys = (train_step.GT_KEYS if gt else data.STAGE2_KEYS) if s2 else data.STAGE1_KEYS
     loader = data.VitonHDLoader(opt.dataroot, opt.datamode, opt.data_list, opt.fine_height, opt.fine_width, opt.batch_size // world,
                                 workers=opt.workers, keys=keys, seed=opt.seed)
     evaluator = None
     if s2 and rank == 0:
         import eval_models
         test_loader = data.VitonHDLoader(opt.test_dataroot, "test", opt.test_data_list, opt.fine_height, opt.fine_width, 1,
-                                         workers=opt.workers, mode="test", keys=EVAL_KEYS, shuffle=False, shard=False)
+                                         workers=opt.workers, mode="test", keys=EVAL_GT_KEYS if gt else EVAL_KEYS, shuffle=False, shard=False)
         evaluator = (test_loader, eval_models.PerceptualLoss(model="net-lin", net="alex", use_gpu=True, gpu_ids=[dev.index]))
     validator = None
     if not s2 and opt.val_count and rank == 0:

@@ -28,11 +28,18 @@ def gaussian_blur_15_3(x):
     return F.conv2d(x, g.view(1, 1, 15, 1).expand(c, 1, 15, 1), padding=(7, 0), groups=c)
 
 
-def make_generator_inputs(tocg, batch, fine_h, fine_w, occlusion=False, unfused_parse=False):
-    """train_generator.py:201-275 (opt.GT False, clothmask_composition 'warp_grad').
+def make_generator_inputs(tocg, batch, fine_h, fine_w, occlusion=False, unfused_parse=False, clothmask_composition="warp_grad", gt=False):
+    """train_generator.py:201-275: (generator input, 7-class parse map).
+    clothmask_composition ('warp_grad' | 'detach' | 'no_composition'): how the tocg's warped cloth mask scales the cloth channel of its
+    segmentation (train_generator.py:218-229).  gt=True (--GT): the ground-truth parse (batch["gen_parse"], the loader's 7-class map)
+    and cloth (batch["parse_cloth"]); tocg is not run and may be None.
     unfused_parse=True keeps the parse-map post-processing as the separate torch ops of the reference (what the tests use to
     check the fused kernel, also on CPU tensors); the product path is the kernel and needs CUDA tensors."""
     from .tocg import make_grid
+    if clothmask_composition not in CLOTHMASK_COMPOSITIONS:
+        raise ValueError("clothmask_composition must be one of %s, got %r" % ("/".join(CLOTHMASK_COMPOSITIONS), clothmask_composition))
+    if gt:  # train_generator.py:249-252
+        return torch.cat((batch["agnostic"], batch["densepose"], batch["parse_cloth"]), 1), batch["gen_parse"]
     cm, c_paired = batch["cloth_mask"], batch["cloth"]
     with torch.no_grad():
         pre_cm_down = F.interpolate(cm, size=(256, 192), mode="nearest")
@@ -42,11 +49,13 @@ def make_generator_inputs(tocg, batch, fine_h, fine_w, occlusion=False, unfused_
         input1 = torch.cat([clothes_down, pre_cm_down], 1)
         input2 = torch.cat([parse_agn_down, dense_down], 1)
         flow_list, fake_segmap, _, warped_cm = tocg(input1, input2)
-        mask = torch.ones_like(fake_segmap)
-        mask[:, 3:4] = warped_cm
-        fake_segmap = fake_segmap * mask
+        composed_cm = None if clothmask_composition == "no_composition" else warped_cm
         n, _, ih, iw = c_paired.shape
         if unfused_parse or not c_paired.is_cuda:
+            if composed_cm is not None:
+                mask = torch.ones_like(fake_segmap)
+                mask[:, 3:4] = (composed_cm > 0.5).float() if clothmask_composition == "detach" else composed_cm
+                fake_segmap = fake_segmap * mask
             key = (n, ih, iw, str(c_paired.device))
             if key not in _GRID_CACHE:  # the reference rebuilds this on the CPU and copies it every step (networks.py:162-165)
                 _GRID_CACHE[key] = make_grid(n, ih, iw).to(c_paired.device)
@@ -57,18 +66,20 @@ def make_generator_inputs(tocg, batch, fine_h, fine_w, occlusion=False, unfused_
             warped_cloth = F.grid_sample(c_paired, warped_grid, padding_mode="border", align_corners=False)
             warped_clothmask = F.grid_sample(cm, warped_grid, padding_mode="border", align_corners=False)
         else:
-            # product path: parse post-processing in one kernel (bilinear resize -> 15x15 Gaussian -> argmax -> one-hot -> 13->7 regroup,
-            # plus, under --occlusion, the softmax-overlap plane), then the hi-res warp of cloth + mask (flow x8 up-sampling, normalise,
-            # base grid, grid_sample, remove_overlap, white composite) in one kernel: no (N,H,W,2) grid, no 13 blurred planes in HBM
+            # product path: parse post-processing in one kernel (cloth-mask composition -> bilinear resize -> 15x15 Gaussian -> argmax ->
+            # one-hot -> 13->7 regroup, plus, under --occlusion, the softmax-overlap plane), then the hi-res warp of cloth + mask (flow x8
+            # up-sampling, normalise, base grid, grid_sample, remove_overlap, white composite) in one kernel: no (N,H,W,2) grid, no 13
+            # blurred planes in HBM
             from . import ops
             div = ((96 - 1.0) / 2.0, (128 - 1.0) / 2.0)
+            comp = dict(cm=None if composed_cm is None else composed_cm.float(), composition=clothmask_composition)
             if occlusion:
                 _, parse, overlap = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False,
-                                                          overlap_classes=OCCLUSION_CLASSES)
+                                                          overlap_classes=OCCLUSION_CLASSES, **comp)
                 warped_cloth, _, warped_clothmask = ops.flow_warp_nchw(flow_list[-1], c_paired.float(), (ih, iw), div, mask=cm, overlap=overlap,
                                                                        composite=True)
             else:
-                _, parse = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False)
+                _, parse = ops.parse_blur_argmax(fake_segmap.float(), (ih, iw), group_of=GROUP_OF_13, groups=7, want_idx=False, **comp)
                 warped_cloth, _ = ops.flow_warp_nchw(flow_list[-1], c_paired.float(), (ih, iw), div)
             g_in = torch.cat((batch["agnostic"], batch["densepose"], warped_cloth), 1)
             return g_in.detach(), parse.detach()
@@ -108,7 +119,7 @@ class BatchFeeder:
     COPY stream into one of two device staging slots while the previous step still computes; one-hot maps (13-channel parse maps, half
     of the batch's bytes as fp32) travel as ONE byte per pixel and are expanded on the device (hrv_onehot_u8).  consume() hands the
     staged batch to the step as fp32 tensors (the graph's static inputs, or a per-step dict)."""
-    ONEHOT = ("parse_agnostic", "parse")
+    ONEHOT = ("parse_agnostic", "parse", "gen_parse")
 
     def __init__(self, batch_cpu, device):
         self.host, self.classes = {}, {}
@@ -324,23 +335,35 @@ class _LossScaling:
 
 class Stage2Trainer(_GraphMixin, _TrainState, _LossScaling):
     """Holds the optimisers / criteria of train_generator.py:145-159 and runs one step.  loss_scale: None or "dynamic" (fp16 storage:
-    apex O1's dynamic loss scaling, see loss_scale.py and _LossScaling).  tensor_lr: see _TrainState."""
+    apex O1's dynamic loss scaling, see loss_scale.py and _LossScaling).  tensor_lr: see _TrainState.
+
+    The reference's options, each defaulting to the README's run:
+      gt (--GT): the generator trains on the ground-truth parse and cloth (batch keys gen_parse, parse_cloth); no tocg (tocg=None);
+      clothmask_composition ('warp_grad' | 'detach' | 'no_composition'): see make_generator_inputs;
+      no_vgg_loss: no VGG term (vgg may be None);
+      the feature-matching term follows the discriminator's opt.no_ganFeat_loss, as in the reference."""
 
     def __init__(self, tocg, generator, discriminator, vgg, lambda_feat=10.0, lambda_vgg=10.0, g_lr=1e-4, d_lr=4e-4,
-                 reducers=None, occlusion=True, loss_scale=None, tensor_lr=False):
+                 reducers=None, occlusion=True, loss_scale=None, tensor_lr=False, gt=False, clothmask_composition="warp_grad",
+                 no_vgg_loss=False):
         from .spade import GANLoss
+        if clothmask_composition not in CLOTHMASK_COMPOSITIONS:
+            raise ValueError("clothmask_composition must be one of %s, got %r" % ("/".join(CLOTHMASK_COMPOSITIONS), clothmask_composition))
+        if tocg is None and not gt:
+            raise ValueError("Stage2Trainer: a tocg is needed unless gt=True")
         self.tocg, self.G, self.D, self.vgg = tocg, generator, discriminator, vgg
         self.crit_gan = GANLoss("hinge")
         self.vgg_weights = [1.0 / 32, 1.0 / 16, 1.0 / 8, 1.0 / 4, 1.0]
         self.lambda_feat, self.lambda_vgg = lambda_feat, lambda_vgg
         self.occlusion = occlusion  # opt.occlusion: the README trains stage 2 with --occlusion
+        self.gt, self.clothmask_composition, self.no_vgg_loss = bool(gt), clothmask_composition, bool(no_vgg_loss)
         self._make_optimizers(generator.parameters(), discriminator.parameters(), g_lr, d_lr, (0.0, 0.9), tensor_lr)
         self.reducers = reducers or {}  # {"G": GradBucketReducer, "D": ...} for data-parallel runs
         self._explicit_reduce = _attach_reducers(self.reducers)
         self._init_loss_scale(loss_scale, {"G": self.opt_g, "D": self.opt_d})
 
     def modules(self):
-        return [self.tocg, self.G, self.D, self.vgg]
+        return [m for m in (self.tocg, self.G, self.D, self.vgg) if m is not None]
 
     @staticmethod
     def _split(pred):
@@ -351,7 +374,8 @@ class Stage2Trainer(_GraphMixin, _TrainState, _LossScaling):
     def step(self, batch, fine_h, fine_w):
         from . import autograd_g
         ops.require_trainable_storage("Stage2Trainer.step")
-        g_in, parse = make_generator_inputs(self.tocg, batch, fine_h, fine_w, occlusion=self.occlusion)
+        g_in, parse = make_generator_inputs(self.tocg, batch, fine_h, fine_w, occlusion=self.occlusion,
+                                            clothmask_composition=self.clothmask_composition, gt=self.gt)
         im = batch["image"]
         # ---------------- generator update (train_generator.py:279-322)
         out = self.G(g_in, parse)
@@ -364,8 +388,11 @@ class Stage2Trainer(_GraphMixin, _TrainState, _LossScaling):
         for i in range(num_d):
             for j in range(len(pred[i]) - 1):  # intermediate features: [fake; real] halves of one pixel-major buffer
                 loss_feat = loss_feat + autograd_g.FeatMatchFn.apply(pred[i][j]) * self.lambda_feat / num_d
-        loss_vgg = autograd_g.vgg_loss(self.vgg, self.vgg_weights, out, im) * self.lambda_vgg
-        loss_gen = (loss_gan + loss_feat + loss_vgg).mean()
+        loss_gen = loss_gan + loss_feat
+        if not self.no_vgg_loss:
+            loss_vgg = autograd_g.vgg_loss(self.vgg, self.vgg_weights, out, im) * self.lambda_vgg
+            loss_gen = loss_gen + loss_vgg
+        loss_gen = loss_gen.mean()
         self.opt_g.zero_grad(set_to_none=not self.scalers)
         self._backward(loss_gen, "G")  # data-parallel: bucket all-reduces are launched from gradient hooks DURING this call (ddp.py)
         if "G" in self.reducers and self._explicit_reduce:
@@ -383,8 +410,12 @@ class Stage2Trainer(_GraphMixin, _TrainState, _LossScaling):
         if "D" in self.reducers and self._explicit_reduce:
             self.reducers["D"].reduce()
         self._opt_step(self.opt_d, "D")
-        return {"loss_gen": loss_gen.detach(), "loss_dis": loss_dis.detach(), "gan": loss_gan.detach(),
-                "feat": loss_feat.detach() if torch.is_tensor(loss_feat) else loss_feat, "vgg": loss_vgg.detach()}
+        losses = {"loss_gen": loss_gen.detach(), "loss_dis": loss_dis.detach(), "gan": loss_gan.detach()}
+        if torch.is_tensor(loss_feat):  # the disabled terms leave the dict, as they leave the reference's G_losses
+            losses["feat"] = loss_feat.detach()
+        if not self.no_vgg_loss:
+            losses["vgg"] = loss_vgg.detach()
+        return losses
 
 
 def synthetic_batch(n, h, w, device, seed=0):
@@ -402,6 +433,16 @@ def synthetic_batch(n, h, w, device, seed=0):
     b = {"cloth": smooth(3), "cloth_mask": (smooth(1) > 0).float(), "parse_agnostic": onehot(13), "densepose": smooth(3),
          "agnostic": smooth(3), "image": smooth(3)}
     return {k: v.to(device) for k, v in b.items()}
+
+
+GT_KEYS = ("agnostic", "densepose", "parse_cloth", "gen_parse", "image")  # what a --GT step reads
+
+
+def synthetic_batch_gt(n, h, w, device, seed=0):
+    """A synthetic batch of GT_KEYS (--GT): synthetic_batch_stage1's ground-truth parse and cloth, the parse as the 7-class map."""
+    b = synthetic_batch_stage1(n, h, w, "cpu", seed)
+    b["gen_parse"] = torch.zeros(n, 7, h, w).scatter_(1, torch.tensor(GROUP_OF_13)[b["parse_onehot"].long()], 1.0)
+    return {k: b[k].to(device) for k in GT_KEYS}
 
 
 # ------------------------------------------------------------------------------------------------ stage 1 (train_condition.py)

@@ -315,10 +315,21 @@ int hrv_avgpool3s2_bwd(const hrv_tensor* dy, const hrv_tensor* dx, hrv_stream st
 int hrv_parse_blur_argmax(const float* seg, int32_t n, int32_t c, int32_t h, int32_t w, int32_t H, int32_t W,
                           const int32_t* group_of, int32_t groups, int64_t* idx, float* onehot, uint32_t occl_mask,
                           float* overlap, hrv_stream stream);
+/* hrv_parse_blur_argmax with the cloth-mask composition of train_generator.py:218-229 applied to the scores before the resize.
+ * cm: (n,1,h,w) fp32 at the scores' resolution; channel cm_channel is multiplied by cm (mode 1, 'warp_grad') or by (cm > 0.5)
+ * (mode 2, 'detach'), each product rounded on its own, so the result equals the torch composition followed by
+ * hrv_parse_blur_argmax.  cm NULL: no composition (mode and cm_channel are ignored). */
+int hrv_parse_blur_argmax_cm(const float* seg, int32_t n, int32_t c, int32_t h, int32_t w, int32_t H, int32_t W,
+                             const int32_t* group_of, int32_t groups, int64_t* idx, float* onehot, uint32_t occl_mask,
+                             float* overlap, const float* cm, int32_t cm_channel, int32_t mode, hrv_stream stream);
 
 /* Input feeding (cp_dataset.py:150-172 ships a one-hot fp32 parse map; here the host ships one byte per pixel):
  * out (n,classes,h,w) fp32 with out[n,c,y,x] = (labels[n,y,x] == c). */
 int hrv_onehot_u8(const uint8_t* labels, int32_t n, int32_t classes, int32_t h, int32_t w, float* out, hrv_stream stream);
+/* hrv_onehot_u8 through a class table: out[n,c,y,x] = (lut[labels[n,y,x]] == c), lut a HOST array of 256 entries (e.g. the
+ * 13 -> 7 label regrouping of train_generator.py:261-273); an entry >= classes sets no channel.  lut NULL: hrv_onehot_u8. */
+int hrv_onehot_u8_lut(const uint8_t* labels, int32_t n, int32_t classes, int32_t h, int32_t w, const uint8_t* lut, float* out,
+                      hrv_stream stream);
 
 /* tgm.image.GaussianBlur((ksize,ksize),(sigma,sigma)) on `planes` fp32 planes of h x w (train_generator.py:181,247;
  * test_generator.py:91,185): separable, zero padding ksize/2, taps exp(-d^2/(2 sigma^2)) normalised to sum 1; odd ksize <= 31. */
