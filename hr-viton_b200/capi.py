@@ -30,7 +30,8 @@ GRAM_F32, GRAM_F64 = 0, 1
 FID_SRC_F32_NCHW, FID_SRC_U8_NHWC = 0, 1
 POOL3X3_AVG_EXCL_PAD, POOL3X3_MAX = 0, 1
 # include/hrviton_sm100_data.h: uint8 in, fp32 out, one flavour (no _f16 twin)
-DATA_EXPORTS = ["hrv_pil_resample_pass", "hrv_pil_nearest", "hrv_agnostic_composite", "hrv_viton_assemble"]
+DATA_EXPORTS = ["hrv_pil_resample_pass", "hrv_pil_nearest", "hrv_agnostic_composite", "hrv_viton_assemble", "hrv_draw_workspace_bytes",
+                "hrv_agnostic_bits", "hrv_parse_agnostic"]
 # include/hrviton_sm100_jpeg.h: uint8 in and out, one flavour (no _f16 twin)
 JPEG_EXPORTS = ["hrv_jpeg_huffman", "hrv_jpeg_idct", "hrv_jpeg_color", "hrv_jpeg_encode_bounds", "hrv_jpeg_encode"]
 JPEG_SRC_U8_NHWC, JPEG_SRC_F32_NCHW = 0, 1
@@ -179,6 +180,9 @@ def lib(dtype=None):
     L.hrv_pil_nearest.argtypes = [vp, i32, i32, i32, vp, i32, vp, i32, vp, vp, vp]
     L.hrv_agnostic_composite.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp]
     L.hrv_viton_assemble.argtypes = [ctypes.POINTER(VitonPlanes), ctypes.POINTER(VitonOutputs), i32, i32, i32, vp]
+    L.hrv_draw_workspace_bytes.argtypes = [i32, i32]
+    L.hrv_agnostic_bits.argtypes = [vp, i32, i32, i32, vp, vp, sz, vp]
+    L.hrv_parse_agnostic.argtypes = [vp, vp, i32, i32, i32, vp, vp, sz, vp]
     L.hrv_jpeg_huffman.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     L.hrv_jpeg_idct.argtypes = [vp, i32, vp, vp, i32, vp]
     L.hrv_jpeg_color.argtypes = [vp, i32, vp, i32, vp]

@@ -4,8 +4,9 @@ VITON-HD tree (jpg / png / json), with the pixel work on the GPU.
 The CPU workers (VitonHDDataset, run by a torch DataLoader) read each JPEG's header and ship the files the device decodes
 (jpeg.device_decodable: baseline, grayscale or YCbCr, 4:4:4 / 4:2:2 / 4:2:0) as their entropy-coded bytes, which hrviton_b200.jpeg
 decodes on the device bit for bit as PIL does, straight into the batch's staged uint8 planes; every other file (the PNGs, and JPEGs
-such as progressive ones) they decode with PIL and ship as uint8 at source resolution.  They also rasterise get_agnostic's pose
-shapes as one bit plane.  The file's header selects the path; there is no option.  The device (include/hrviton_sm100_data.h) composites the agnostic image,
+such as progressive ones) they decode with PIL and ship as uint8 at source resolution.  For the agnostic image they ship the
+OpenPose keypoints, from which the device rasterises get_agnostic's pose shapes as one bit plane (hrviton_b200.draw), bit for bit as
+ImageDraw draws them in agnostic_bits.  The file's header selects the path; there is no option.  The device (include/hrviton_sm100_data.h) composites the agnostic image,
 resizes with Pillow's own fixed-point arithmetic (tables built here), regroups the 20 parse labels to 13 and writes the fp32 outputs
 in one assembly launch; the 13-channel maps are expanded from one byte per pixel by hrv_onehot_u8.  VitonHDLoader stages each batch
 on a copy stream with two slots (train_step.BatchFeeder), so `Stage2Trainer.replay(feeder=loader)` trains from disk.
@@ -20,7 +21,7 @@ import numpy as np
 import torch
 from PIL import Image, ImageDraw
 
-from . import capi, jpeg
+from . import capi, draw, jpeg
 from .train_step import GROUP_OF_13, LABELS7, BatchFeeder
 
 PRECISION_BITS = 22  # Pillow's fixed-point precision for 8-bit resampling
@@ -192,9 +193,12 @@ class VitonHDDataset(torch.utils.data.Dataset):
 
     Raises ValueError on input the device path does not reproduce: an image, pose or densepose file that is not RGB (ToTensor would
     keep its other channels), a cloth mask that is not mode 'L', parse labels above 19, planes of different sizes, or a fine_height
-    other than torchvision's height for fine_width."""
+    other than torchvision's height for fine_width.
 
-    def __init__(self, dataroot, datamode, data_list, fine_height, fine_width, mode="train", keys=None):
+    device_agnostic=True ships each sample's (25, 2) fp64 keypoints ('keypoints') instead of the agnostic bit plane ('bits'), for
+    the device to rasterise (draw.agnostic_bits); such a sample raises ValueError on keypoints draw.keypoints_array refuses."""
+
+    def __init__(self, dataroot, datamode, data_list, fine_height, fine_width, mode="train", keys=None, device_agnostic=False):
         if mode not in ("train", "test"):
             raise ValueError("mode must be 'train' or 'test', not %r" % (mode,))
         self.mode = mode
@@ -217,6 +221,7 @@ class VitonHDDataset(torch.utils.data.Dataset):
         self.lab_planes = [p for p in ("parse", "parse_agnostic") if p in needs]
         self.mask_sets = len(self.sets) if "cloth_mask" in needs else 0
         self.keypoints = "keypoints" in needs
+        self.device_agnostic = bool(device_agnostic)
         if not self.im_names:
             raise ValueError("%s lists no samples" % osp.join(dataroot, data_list))
         first = self._open(self._paths(0)[self.rgb_planes[0] if self.rgb_planes else (self.lab_planes or ["cloth_mask"])[0]])
@@ -311,7 +316,10 @@ class VitonHDDataset(torch.utils.data.Dataset):
         if self.keypoints:
             with open(paths["keypoints"]) as f:
                 pose = np.array(json.load(f)["people"][0]["pose_keypoints_2d"]).reshape((-1, 3))[:, :2]
-            out["bits"] = agnostic_bits(pose, (self.src_w, self.src_h))
+            if self.device_agnostic:
+                out["keypoints"] = draw.keypoints_array(pose, paths["keypoints"])
+            else:
+                out["bits"] = agnostic_bits(pose, (self.src_w, self.src_h))
         return out
 
 
@@ -341,8 +349,9 @@ def collate(samples):
     if items:
         out["jpeg_bytes"] = jpeg.pack_entropy(items)
         out["jpeg"], out["jpeg_to"] = items, item_to
-    if "bits" in samples[0]:
-        out["bits"] = torch.from_numpy(np.stack([s["bits"] for s in samples]))
+    for k in ("bits", "keypoints"):
+        if k in samples[0]:
+            out[k] = torch.from_numpy(np.stack([s[k] for s in samples]))
     out["im_name"] = [s["im_name"] for s in samples]
     out["c_name"] = {k: [s["c_name"][k] for s in samples] for k in samples[0]["c_name"]}
     return out
@@ -409,12 +418,16 @@ class VitonHDLoader(BatchFeeder):
     so a captured trainer replays with replay(feeder=loader).  Incomplete batches are dropped (drop_last, as in the reference).
 
     With an initialised process group of world size W, rank r reads a disjoint 1/W of each epoch's permutation (shard_indices);
-    shard=False reads the whole set on every rank.  position() and start_at() save and restore where the batches stand."""
+    shard=False reads the whole set on every rank.  position() and start_at() save and restore where the batches stand.
+
+    The agnostic image's shapes are rasterised on the device from the keypoints the workers ship (device_agnostic=True), or drawn
+    by ImageDraw in the workers (False); the batches are the same bit for bit."""
 
     def __init__(self, dataroot, datamode, data_list, fine_height, fine_width, batch_size, workers=4, mode="train", keys=None, shuffle=True,
-                 seed=0, shard=True):
+                 seed=0, shard=True, device_agnostic=True):
         import torch.distributed as dist
-        self.dataset = VitonHDDataset(dataroot, datamode, data_list, fine_height, fine_width, mode=mode, keys=keys)
+        self.dataset = VitonHDDataset(dataroot, datamode, data_list, fine_height, fine_width, mode=mode, keys=keys,
+                                      device_agnostic=device_agnostic)
         ds = self.dataset
         self.keys, self.batch_size, self.seed = ds.keys, int(batch_size), seed
         rank, world = (dist.get_rank(), dist.get_world_size()) if shard and dist.is_available() and dist.is_initialized() else (0, 1)
@@ -504,16 +517,21 @@ class VitonHDLoader(BatchFeeder):
                 s["cm"] = torch.empty((ds.mask_sets, n, h, w), dtype=torch.uint8, device=dev)
             if ds.keypoints:
                 s["bits"] = torch.empty((n, h, w), dtype=torch.uint8, device=dev)
+            if ds.keypoints and ds.device_agnostic:
+                s["keypoints"] = torch.empty((n, 25, 2), dtype=torch.float64, device=dev)
+                s["draw_ws"] = torch.empty(draw.workspace_bytes(n, h), dtype=torch.uint8, device=dev)
             self.slots[slot] = s
         st = self.slots[slot]
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(self.free[slot])  # the batch that used this slot last has been assembled
             for k, v in b.items():
-                if k in ("rgb", "lab", "cm", "bits"):
+                if k in ("rgb", "lab", "cm", "bits", "keypoints"):
                     st[k][:v.shape[0]].copy_(v, non_blocking=True)
                 elif k in ("rgb_pil", "cm_pil"):
                     for (p, i), img in zip(b[k[:-4] + "_to"], v):
                         st[k[:-4]][p, i].copy_(img, non_blocking=True)
+            if "keypoints" in b:
+                draw.agnostic_bits(st["keypoints"], out=st["bits"], workspace=st["draw_ws"])
             if "jpeg" in b:
                 batch = jpeg.Batch(b["jpeg"], b["jpeg_bytes"])
                 batch.set_destinations([st[k][p, i] for k, p, i in b["jpeg_to"]])
@@ -523,7 +541,7 @@ class VitonHDLoader(BatchFeeder):
                 self._jpeg_pending[1].record(self.copy_stream)
                 self.device_decoded += len(b["jpeg"])
             self.ready[slot].record(self.copy_stream)
-        self.bytes_per_step = int(sum(v.numel() for k, v in b.items() if torch.is_tensor(v))) + len(b.get("jpeg", ())) * jpeg.DESCRIPTOR_BYTES
+        self.bytes_per_step = int(sum(v.numel() * v.element_size() for k, v in b.items() if torch.is_tensor(v))) + len(b.get("jpeg", ())) * jpeg.DESCRIPTOR_BYTES
         self.host[slot], self.names[slot], self.epochs[slot], self.positions[slot] = b, (b["im_name"], b["c_name"]), epoch, (epoch, index)
 
     def _check_jpeg_errors(self):

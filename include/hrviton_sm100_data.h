@@ -37,6 +37,24 @@ int hrv_pil_nearest(const uint8_t* src, int32_t planes, int32_t h, int32_t w, co
 int hrv_agnostic_composite(const uint8_t* image, const uint8_t* parse, const uint8_t* bits, int32_t n, int32_t h, int32_t w, uint8_t* dst,
                            hrv_stream stream);
 
+/* The ImageDraw shapes of the reference's agnostic masks, rasterised pixel for pixel as Pillow 12.2 draws them (csrc/draw_kernels.cu
+ * states the rules).  keypoints: (n, 25, 2) fp64 OpenPose keypoints as read from the JSON, a keypoint (0, 0) being absent; every
+ * coordinate finite and within +-4096 (the Python layer checks this).  workspace: device memory of hrv_draw_workspace_bytes(n, h)
+ * bytes that no other launch uses until this one has finished.
+ *
+ * hrv_agnostic_bits: cp_dataset.get_agnostic's shapes as the bit plane of hrviton_b200.data.agnostic_bits, bits (n, h, w) uint8:
+ * bit 0 = a grey torso / neck / arm shape, bits 1 / 2 = the label-14 / label-15 arm masks.  get_agnostic draws the arm masks on a
+ * 768 x 1024 canvas whatever the image size, so the result is the reference's only for h = 1024, w = 768.
+ *
+ * hrv_parse_agnostic: get_parse_agnostic.get_im_parse_agnostic(labels, keypoints, w, h) on a batch: labels (n, h, w) uint8,
+ * out (n, h, w) uint8 = 0 where the pixel is labelled 5, 6, 7 or 10, or labelled 14 / 15 and covered by that label's arm mask
+ * (r = 10: lines of width 100, joint ellipses of radius 150, the hand's of radius 40), else the label. */
+size_t hrv_draw_workspace_bytes(int32_t n, int32_t h);
+int hrv_agnostic_bits(const double* keypoints, int32_t n, int32_t h, int32_t w, uint8_t* bits, void* workspace, size_t workspace_bytes,
+                      hrv_stream stream);
+int hrv_parse_agnostic(const double* keypoints, const uint8_t* labels, int32_t n, int32_t h, int32_t w, uint8_t* out, void* workspace,
+                       size_t workspace_bytes, hrv_stream stream);
+
 /* Fine-size uint8 planes of one batch (NULL: absent).  RGB planes are (n, h, w, 3); cloth[s] / cloth_mask[s] hold the paired (s = 0)
  * and unpaired (s = 1) cloth; parse holds the regrouped label ids 0-12, (n, h, w). */
 typedef struct hrv_viton_planes {
