@@ -35,6 +35,9 @@ DATA_EXPORTS = ["hrv_pil_resample_pass", "hrv_pil_nearest", "hrv_agnostic_compos
 # include/hrviton_sm100_jpeg.h: uint8 in and out, one flavour (no _f16 twin)
 JPEG_EXPORTS = ["hrv_jpeg_huffman", "hrv_jpeg_idct", "hrv_jpeg_color", "hrv_jpeg_encode_bounds", "hrv_jpeg_encode"]
 JPEG_SRC_U8_NHWC, JPEG_SRC_F32_NCHW = 0, 1
+# include/hrviton_sm100_png.h: uint8 / fp32 in, uint8 out, one flavour (no _f16 twin)
+PNG_EXPORTS = ["hrv_png_encode_bounds", "hrv_png_encode", "hrv_condition_grid"]
+GRID_NO_COMPOSITION, GRID_DETACH, GRID_WARP_GRAD = 0, 1, 2
 
 
 class Tensor(ctypes.Structure):
@@ -59,6 +62,12 @@ class VitonOutputs(ctypes.Structure):
     _fields_ = [("image", ctypes.c_void_p), ("cloth", ctypes.c_void_p * 2), ("cloth_mask", ctypes.c_void_p * 2), ("pose", ctypes.c_void_p),
                 ("densepose", ctypes.c_void_p), ("agnostic", ctypes.c_void_p), ("pcm", ctypes.c_void_p), ("parse_cloth", ctypes.c_void_p),
                 ("parse_onehot", ctypes.c_void_p)]
+
+
+class ConditionPanels(ctypes.Structure):
+    """include/hrviton_sm100_png.h's hrv_condition_panels."""
+    _fields_ = [(k, ctypes.c_void_p) for k in ("cloth", "cloth_mask", "parse_agnostic", "densepose", "parse_cloth", "pcm", "warped_cloth",
+                                                "warped_cm", "parse", "seg", "image")]
 
 
 class ConvParams(ctypes.Structure):
@@ -188,7 +197,10 @@ def lib(dtype=None):
     L.hrv_jpeg_color.argtypes = [vp, i32, vp, i32, vp]
     L.hrv_jpeg_encode_bounds.argtypes = [i32, i32, i32, ctypes.POINTER(sz), ctypes.POINTER(sz)]
     L.hrv_jpeg_encode.argtypes = [vp, i32, i32, i32, i32, vp, vp, sz, vp, sz, vp, vp]
-    for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS + DATA_EXPORTS + JPEG_EXPORTS:
+    L.hrv_png_encode_bounds.argtypes = [i32, i32, i32, ctypes.POINTER(sz), ctypes.POINTER(sz)]
+    L.hrv_png_encode.argtypes = [vp, i32, i32, i32, vp, sz, vp, sz, vp, vp]
+    L.hrv_condition_grid.argtypes = [ctypes.POINTER(ConditionPanels), i32, i32, i32, i32, i32, vp, vp]
+    for name in EXPORTS + EXPORTS_F16 + METRICS_EXPORTS + DATA_EXPORTS + JPEG_EXPORTS + PNG_EXPORTS:
         fn = getattr(L, name)
         if "_workspace_bytes" in name:
             fn.restype = ctypes.c_size_t
